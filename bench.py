@@ -1,27 +1,29 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the Darknet hot path on B200 (BASELINE.json metric: "images/sec (640x640) YOLOv4
-train+infer at 1/2/4/8 B200; conv roofline %").
+"""bench.py -- images/sec of the Darknet hot path on H100 (BASELINE.json metric: "images/sec (640x640) YOLOv4
+train+infer at 1/2/4/8 GPUs; conv roofline %").
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 PRIMARY workload (the headline `value`) = BASELINE.json configs[2], the per-GPU slice of "yolov4.cfg training bs=64 on
-8xB200": yolov4.cfg, 8 images per GPU, 640x640, one process per GPU.  A "step" is one complete training step:
+8 GPUs": yolov4.cfg, 8 images per GPU, 640x640, one process per GPU.  A "step" is one complete training step:
 
-    forward (batch-statistics BatchNorm, tcgen05 convs) -> YOLO loss -> backward (dgrad / wgrad tcgen05, BN backward)
+    forward (batch-statistics BatchNorm, wgmma convs) -> YOLO loss -> backward (dgrad / wgrad wgmma, BN backward)
     -> ONE NCCL all-reduce over the flat fp32 gradient buffer (N > 1) -> fused SGD-Nesterov
 
 Per-GPU work is fixed as N grows ("scaling": "weak"; global batch = 8 N).  One JSON line on stdout (rank 0):
   value    : images/s, batch and targets resident in HBM (CUDA events around K steps, max over ranks)
   e2e      : the same step through the public API with pinned HOST uint8 images + targets: H2D copy, /256, step,
              D2H of the four loss items -- all inside the timed region
-  roofline : the tcgen05 convolution family (forward, data gradient, weight gradient) of one step, replayed back to
+  roofline : the wgmma convolution family (forward, data gradient, weight gradient) of one step, replayed back to
              back and timed live with CUDA events; FLOPs = 2 M N K of every launch
   cpu_baseline : the oracle (CPU restatement of the reference's PyTorch path) training step on the host cores (N=1)
   secondary: (N=1) YOLOv3 inference bs 32 (configs[1]), YOLOv4 inference bs 32, with their own conv rooflines
 --impl reference: the reference arm = the reference's own CPU PyTorch training step, restated in oracle/ and pinned to
-the reference by tests/test_oracle_golden.py (the reference is pure Python and /root/reference does not exist on the
-GPU box), all host threads, bounded sample.
+the reference by tests/test_oracle_golden.py, all host threads, bounded sample.
+--dump-outputs DIR: after the timed steps, write what the last timed training step computed (loss items, a fixed
+sample of the three prediction tensors and of the flat gradient buffer) as DIR/<name>.npy; the inputs are seeded, so two
+builds can be compared output for output.
 """
 import argparse
 import json
@@ -49,13 +51,9 @@ CONV_CALLS = ("b2y_conv2d_fwd", "b2y_conv2d_fwd_stats", "b2y_conv2d_bwd_data", "
 
 
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            d = json.load(f)
-        return {"hbm_gbs": d["hbm_gbs"], "tflops": d["bf16_tflops_sustained"], "tflops_burst": d["bf16_tflops"],
-                "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "tflops_burst": 1590.0, "source": "fallback"}
+    # NVIDIA's data sheet for the H100 SXM (700 W): dense FP16 / BF16 tensor rate and HBM3 bandwidth.  Denominators only:
+    # a power-limited card runs below them.
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "source": "H100 SXM data sheet (dense fp16, 700 W)"}
 
 
 class ClockSampler:
@@ -233,7 +231,7 @@ def cpu_reference_rate(kind, name, max_seconds=20.0, batch=2, max_iters=10, thre
 
 def torch_gpu_baseline(dev, batch, iters=5):
     """INFORMATIONAL (BASELINE.md section 3: "the kernel to beat"): the reference's own op sequence -- the oracle port --
-    executed by stock PyTorch on the same B200 (eager ATen + cuDNN, autocast fp16, channels_last), yolov4 forward +
+    executed by stock PyTorch on the same GPU (eager ATen + cuDNN, autocast fp16, channels_last), yolov4 forward +
     compute_loss + backward of `batch` images at 640x640 (no optimiser step, no all-reduce).  Part of the baseline leg:
     never on the product path, never used to compute `value`."""
     sys.path.insert(0, ROOT)
@@ -281,9 +279,9 @@ def torch_gpu_baseline(dev, batch, iters=5):
     e1.synchronize()
     ms = e0.elapsed_time(e1) / iters
     return {"value": batch / (ms / 1e3), "unit": "images/s", "ms_per_step": ms,
-            "what": "oracle port (the reference's op sequence) on stock PyTorch %s eager + cuDNN on this B200, autocast "
+            "what": "oracle port (the reference's op sequence) on stock PyTorch %s eager + cuDNN on this %s, autocast "
                     "fp16, channels_last: yolov4 forward + compute_loss + backward, %d images 640x640, no optimiser step"
-                    % (torch.__version__, batch)}
+                    % (torch.__version__, torch.cuda.get_device_name(dev), batch)}
 
 
 def run_reference_arm(args, rank, world):
@@ -355,7 +353,7 @@ def record_calls(fn):
 
 
 def replay_convs(calls, iters):
-    """Replay the tcgen05 convolution launches of one recorded step back to back -> (ms per step-worth, FLOPs, n)."""
+    """Replay the wgmma convolution launches of one recorded step back to back -> (ms per step-worth, FLOPs, n)."""
     from b200yolo import lib
     convs = [(n, a) for (n, a) in calls if n in CONV_CALLS]
     flops = sum(conv_desc_flops(n, a) for n, a in convs)
@@ -375,21 +373,12 @@ def replay_convs(calls, iters):
     return e0.elapsed_time(e1) / iters, flops, len(convs)
 
 
-# DRAM bytes (read + write) of the conv-family launches of ONE yolov4 training step, 8 x 640 x 640, from the ncu launch list
-# profiles/r02/final/launches_train_r02_final.csv (240 conv_tc_kernel + 110 weight-gradient launches of the second step,
-# eager, cold cache): 11.65 GB, i.e. 33.3 MB per launch -- against 13.4 GB of algorithmic bytes (every operand and result
-# of the 328 GEMM launches once: activations / gradients 16-bit, packed weight gradients fp32): no wasted re-reads, the
-# 3x3 tap re-reads and part of the producer -> consumer traffic are served by the 126 MB L2
-NCU_TRAIN_CONV_DRAM_BYTES_PER_STEP = 11651468800
-
-
-def roofline_block(conv_ms, conv_flops, n_convs, step_ms, what, traffic=None):
+def roofline_block(conv_ms, conv_flops, n_convs, step_ms, what):
     pk = peaks()
     achieved = conv_flops / (conv_ms / 1e3) / 1e12
     return {"bound": "tensor", "achieved": achieved, "peak": pk["tflops"], "unit": "TFLOP/s",
-            "frac": achieved / pk["tflops"], "traffic": traffic,
-            "peak_source": pk["source"] + " (sustained bf16, MEASURED_PEAKS.json)",
-            "kernel": "tcgen05 conv family (%s): %d launches of one step replayed back to back" % (what, n_convs),
+            "frac": achieved / pk["tflops"], "peak_source": pk["source"],
+            "kernel": "wgmma conv family (%s): %d launches of one step replayed back to back" % (what, n_convs),
             "kernel_ms_per_step": conv_ms, "share_of_step": conv_ms / step_ms,
             "algorithmic_flops_per_step": conv_flops,
             "whole_step_frac": conv_flops / (step_ms / 1e3) / 1e12 / pk["tflops"]}
@@ -399,9 +388,34 @@ def roofline_block(conv_ms, conv_flops, n_convs, step_ms, what, traffic=None):
 # primary workload: YOLOv4 training step, data parallel
 # ----------------------------------------------------------------------------------------------------------------
 def note(rank, msg):
-    """progress marker on stderr (per rank): the driver's log shows how far a failing multi-GPU run got"""
+    """progress marker on stderr (per rank): the log shows how far a failing multi-GPU run got"""
     sys.stderr.write("[bench.py rank %d] %s\n" % (rank, msg))
     sys.stderr.flush()
+
+
+DUMP_SAMPLE = 1 << 20          # elements kept per large output (fixed, seeded positions)
+
+
+def dump_outputs(d, items, pred, flat_grad):
+    """The last timed step's results as .npy files: the four loss items, and for each prediction tensor and the flat
+    fp32 gradient buffer a fixed seeded sample of DUMP_SAMPLE elements (float32, with their positions as float64) plus
+    the float64 sum of the whole tensor (about 50 MB in all)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {"loss_items": items.detach().float().cpu()}
+    for name, t in [("pred%d" % i, p) for i, p in enumerate(pred)] + [("flat_grad", flat_grad)]:
+        flat = t.detach().float().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(1234 + flat.numel())
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            arrays[name + "_sample"] = flat[idx.to(flat.device)].cpu()
+            arrays[name + "_sample_index"] = idx.double()
+        else:
+            arrays[name] = flat.cpu()
+        arrays[name + "_sum"] = flat.double().sum().reshape(1).cpu()
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a.numpy())
 
 
 def run_train(args, dev, rank, world, dd):
@@ -428,6 +442,7 @@ def run_train(args, dev, rank, world, dd):
         dp.reduce_gradients()
         dp.step(lr=lr, momentum=0.937, weight_decay=0.000484)
         state["items"] = items
+        state["pred"] = pred
 
     for _ in range(args.warmup):
         step(x_dev, t_dev)
@@ -441,6 +456,8 @@ def run_train(args, dev, rank, world, dd):
     value = world * B / (ms_step / 1e3)
     items = [float(v) for v in state["items"]]
     note(rank, "timed region done: %.3f ms/step" % ms_step)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, state["items"], state["pred"], dp.flat_grad)
 
     # ---- end to end: pinned host uint8 batch + targets -> H2D -> /256 -> step -> D2H of the loss items ----------
     copy_stream = torch.cuda.Stream()
@@ -496,12 +513,8 @@ def run_train(args, dev, rank, world, dd):
             del model.use_cuda_graph
         else:
             model.use_cuda_graph = saved
-    conv_ms, conv_flops, n_convs = replay_convs(calls, iters=max(3, min(10, args.steps)))
-    roofline = roofline_block(conv_ms, conv_flops, n_convs, ms_step, "forward + data gradient + weight gradient",
-                              traffic=NCU_TRAIN_CONV_DRAM_BYTES_PER_STEP if (TRAIN_MODEL == "yolov4" and B == 8) else None)
-    if roofline["traffic"] is not None:
-        roofline["traffic_unit"] = "bytes per step (all conv-family launches; ncu dram__bytes_read.sum + dram__bytes_write.sum)"
-        roofline["algorithmic_bytes_per_step"] = 13389727744
+    conv_ms, conv_flops, n_convs = replay_convs(calls, iters=args.steps)
+    roofline = roofline_block(conv_ms, conv_flops, n_convs, ms_step, "forward + data gradient + weight gradient")
     roofline["table_flops_per_step"] = FLOPS_TRAIN[TRAIN_MODEL] * B
     launches = len(calls)
     return {"value": value, "ms_per_step": ms_step, "clocks": clocks, "roofline": roofline, "allreduce": allreduce,
@@ -575,7 +588,7 @@ def run_infer(name, args, dev, rank, world, dd, with_e2e=True):
                 del model.use_cuda_graph
             else:
                 model.use_cuda_graph = saved
-        conv_ms, conv_flops, n_convs = replay_convs(calls, iters=max(3, min(10, args.steps)))
+        conv_ms, conv_flops, n_convs = replay_convs(calls, iters=args.steps)
         out["roofline"] = roofline_block(conv_ms, conv_flops, n_convs, ms_step, "forward")
         out["launches_per_step"] = len(calls)
         out["workload"] = "%s.cfg inference bs=%d 640x640 per GPU, fp16 fused conv path" % (name, B)
@@ -625,7 +638,7 @@ def run_nms(args, dev, dd):
 
     for _ in range(3):
         packed = step()
-    ms = timed(step, max(3, min(args.steps, 10)), dd)
+    ms = timed(step, args.steps, dd)
     return {"value": B / (ms / 1e3), "unit": "images/s", "ms_per_step": ms,
             "candidates_per_image": sum(torch.diff(packed.offsets_dev).tolist()) / B,
             "detections_per_image": sum(packed.counts) / B, "launches_per_step": 10,
@@ -669,6 +682,8 @@ def main():
     ap.add_argument("--train-batch", type=int, default=TRAIN_BATCH, help="images per GPU of the training workload")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed training step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -689,7 +704,7 @@ def main():
         raise SystemExit(rc)
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200): the hot path has no CPU fallback")
+        raise SystemExit("bench.py needs a CUDA device (H100): the hot path has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     import torch.distributed as dist
@@ -714,7 +729,7 @@ def main():
             secondary["nms_bs%d" % INFER_BATCH] = {"error": "%s: %s" % (type(e).__name__, str(e)[:300])}
         # the two remaining BASELINE configurations, per-GPU slices, each in its own process
         torch.cuda.empty_cache()
-        mb_args = ["--model", "yolov3-mobilenet", "--batch", "32", "--size", str(SIZE), "--steps", "10"]
+        mb_args = ["--model", "yolov3-mobilenet", "--batch", "32", "--size", str(SIZE), "--steps", str(args.steps)]
         mb_what = ("yolov3-mobilenet.cfg (depthwise-separable backbone) training step, 32 images / GPU, 640x640: forward + "
                    "YOLO loss + backward + gradient exchange + fused SGD-Nesterov (BASELINE configs[3]: bs 128 on 4 GPUs)")
         blk = run_tool_block("bench_train.py", mb_args, mb_what)
@@ -724,9 +739,9 @@ def main():
             blk["first_attempt"] = first
         secondary["yolov3_mobilenet_train_bs32"] = blk
         secondary["yolov3_int8_ptq_infer_bs%d" % INFER_BATCH] = run_tool_block(
-            "bench_ptq_native.py", ["--batch", str(INFER_BATCH), "--size", str(SIZE), "--steps", "10"],
+            "bench_ptq_native.py", ["--batch", str(INFER_BATCH), "--size", str(SIZE), "--steps", str(args.steps)],
             "yolov3.cfg INT8 PTQ inference bs=%d 640x640 (BASELINE configs[4] at the batch of configs[1]): native "
-            "calibration, then the tcgen05 kind::i8 graph" % INFER_BATCH)
+            "calibration, then the int8 wgmma graph" % INFER_BATCH)
 
     cpu, tgpu = None, None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
@@ -734,7 +749,7 @@ def main():
         cpu = {k: cpu[k] for k in ("value", "unit", "cores", "kind", "sample")}
         try:
             torch.cuda.empty_cache()
-            tgpu = torch_gpu_baseline(dev, tr["batch"])
+            tgpu = torch_gpu_baseline(dev, tr["batch"], iters=args.steps)
         except Exception as e:      # informational only
             tgpu = {"error": "%s: %s" % (type(e).__name__, str(e)[:200])}
 
@@ -751,10 +766,11 @@ def main():
                        "global_batch": B * world, "parallelism": "dp%d" % world,
                        "precision": "fp16 activations / weights, bf16 activation gradients, fp32 accumulation, "
                                     "statistics, weight gradients, master weights and optimiser",
-                       "l2": "activations + gradients of one step (> 8 GB) exceed the 126 MB L2; every step re-reads "
+                       "l2": "activations + gradients of one step (> 8 GB) exceed the 50 MB L2; every step re-reads "
                              "them from HBM",
                        "cuda_graph": True, "grad_allreduce_bytes": tr["grad_bytes"],
                        "launches_per_step": tr["launches_per_step"], "loss_items": tr["loss_items"]},
+            "gpu": torch.cuda.get_device_name(dev),
             "clocks": tr["clocks"],
             "e2e": tr["e2e"],
             "gpu_launches": tr["gpu_launches"],
@@ -780,15 +796,6 @@ if __name__ == "__main__":
     except SystemExit:
         raise
     except BaseException:
-        # torchrun swallows per-rank tracebacks (error_file: <N/A>): keep them where the driver can find them
-        tb = traceback.format_exc()
-        r = os.environ.get("RANK", "0")
-        sys.stderr.write("[bench.py rank %s]\n%s\n" % (r, tb))
-        try:
-            d = os.path.join(ROOT, "gpurun_out")
-            os.makedirs(d, exist_ok=True)
-            with open(os.path.join(d, "bench_rank%s.err" % r), "w") as f:
-                f.write(tb)
-        except OSError:
-            pass
+        # torchrun swallows per-rank tracebacks (error_file: <N/A>): print them with the rank
+        sys.stderr.write("[bench.py rank %s]\n%s\n" % (os.environ.get("RANK", "0"), traceback.format_exc()))
         raise

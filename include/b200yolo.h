@@ -1,5 +1,5 @@
 /*
- * b200yolo.h -- C ABI of libb200yolo.so (sm_100a kernels for the Darknet YOLOv3/v4 hot path).
+ * b200yolo.h -- C ABI of libb200yolo.so (sm_90a kernels for the Darknet YOLOv3/v4 hot path).
  *
  * The reference (SpursLipu/YOLOv3v4-ModelCompression-MultidatasetTraining-Multibackbone) is pure
  * Python on top of torch ATen; it has no FFI of its own.  The drop-in boundary is therefore the
@@ -45,7 +45,7 @@ extern "C" {
 
 /* 16-bit tensor dtypes.  Training: activation gradients (dY) are stored in bf16 (fp16 over/underflows across the ~100
  * BatchNorm layers of a Darknet); the conv data gradient dZ that feeds the tensor-core GEMMs is fp16 times a per-layer
- * power-of-two scale picked on the device (tcgen05 kind::f16 faults on mixed f16/bf16 operands) */
+ * power-of-two scale picked on the device (wgmma takes one 16-bit format for both operands) */
 #define B2Y_DT_F16 0
 #define B2Y_DT_BF16 1
 
@@ -109,7 +109,7 @@ int b2y_stem_conv_fwd(const b2y_conv_desc* d, const float* x_nchw, const float* 
                       void* stream);
 
 /* Tensor-core stem (in_c*ksize <= 16): the image is re-laid as NHWC fp16 with the kw taps unrolled into 16 channels
- * (workspace, b2y_stem_workspace_bytes), then the conv runs as a k x 1 implicit GEMM on the tcgen05 kernel.
+ * (workspace, b2y_stem_workspace_bytes), then the conv runs as a k x 1 implicit GEMM on the wgmma kernel.
  *   w_stem fp16 [out_c][k][16] from b2y_pack_stem_weights (w already BN-folded, OIHW fp32)
  *   stat_sum/stat_sqsum optional (training BN statistics, see b2y_conv2d_fwd_stats) */
 size_t b2y_stem_workspace_bytes(const b2y_conv_desc* d);
@@ -118,7 +118,7 @@ int b2y_stem_conv_fwd_tc(const b2y_conv_desc* d, const float* x_nchw, const void
                          void* workspace, void* y, float* stat_sum, float* stat_sqsum, void* stream);
 
 /* Fused tensor-core stem (in_c*ksize*ksize <= 32, out_c <= 64): the CTA builds the im2col tile in shared memory
- * straight from the image and feeds tcgen05.mma, so only the image is read and only y is written (no workspace).
+ * straight from the image and feeds wgmma, so only the image is read and only y is written (no workspace).
  *   x_nchw   NCHW image, x_dtype = B2Y_STEM_X_F32 / _F16 / _U8; value = raw / x_div
  *            (x_div = 256 for uint8 images: reference test.py:95, train.py:348, detect.py:101 "/ 256.0")
  *   w_stem   fp16 [out_c][32] from b2y_pack_stem_weights (the layout it produces when in_c*k*k <= 32)
@@ -227,7 +227,7 @@ typedef struct b2y_qconv_desc {
     int out_kind;         /* B2Y_OUT_I8: requantised int8; B2Y_OUT_F32/F16: fake-quant value (heads: linear) */
     int requant;          /* 0: write act(acc*acc_scale+bias) without requantisation (linear head, ptq_cos.py:718) */
 } b2y_qconv_desc;
-/* INT8 conv on tcgen05 kind::i8 with int32 accumulation (exact whenever the fp32 reference is). */
+/* INT8 conv on int8 wgmma with int32 accumulation (exact whenever the fp32 reference is). */
 int b2y_qconv2d_fwd(const b2y_qconv_desc* d, const void* x_i8, const void* w_i8, const float* bias, void* y,
                     void* stream);
 /* The same conv with the FOLLOWING quantised shortcut layer (ptq_cos.py:876-884 _min / 931-933 _max, eval) folded into its
@@ -280,7 +280,7 @@ int b2y_bn_act_bwd_apply(const void* x, long long x_pitch, const void* dy, long 
                          long long pixels, int c, int act, float slope, int grad_dtype /* of dy */,
                          const float* du_absmax, float* scale_out /* [s, 1/s] chosen on the device, power of two */,
                          void* stream);
-/* dX = conv_transpose(dY, W)   (data gradient; implicit GEMM on tcgen05) */
+/* dX = conv_transpose(dY, W)   (data gradient; implicit GEMM on wgmma) */
 int b2y_conv2d_bwd_data(const b2y_conv_desc* d, const void* dy, const void* w_packed_t, void* dx, int accumulate,
                         int operand_dtype /* dY and weights */, int out_dtype /* dX */,
                         const float* inv_scale_ptr /* optional device scalar multiplied into dX */, void* stream);
@@ -288,8 +288,12 @@ int b2y_conv2d_bwd_data(const b2y_conv_desc* d, const void* dy, const void* w_pa
  * (stride-s data gradients are decomposed into s*s stride-1 implicit GEMMs over dY; out_c*ksize^2*in_c elements) */
 int b2y_pack_dgrad_weights(const b2y_conv_desc* d, const float* w_oihw, void* w_packed_t, int grad_dtype,
                            void* stream);
-/* dW[o][kh][kw][i] += scale * sum_pixels dY[p][o] * X[p@(kh,kw)][i]  (weight gradient, tcgen05 GEMM over the pixel
- * dimension with MN-major operands; dw fp32 [O][kh][kw][I], caller zeroes it; split-K reduced with red.global.add) */
+/* dW[o][kh][kw][i] += scale * sum_pixels dY[p][o] * X[p@(kh,kw)][i]  (weight gradient, wgmma GEMM over the pixel
+ * dimension with MN-major operands; dw fp32 [O][kh][kw][I], caller zeroes it).  The split-K partial sums are added in
+ * double into an accumulator that belongs to the calling (device, stream) and then rounded into dw, so the result does
+ * not depend on the order of the atomics; calls on different streams may run concurrently (the same holds for the
+ * batch statistics of b2y_conv2d_fwd_stats / b2y_stem_conv_fwd_tc, b2y_bn_train_bwd_reduce, b2y_bn_act_bwd_reduce and
+ * b2y_stem_conv_bwd_weight).  The first call on a stream allocates its accumulator. */
 int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, const void* dy, float* dw, float scale,
                           int operand_dtype /* X and dY */, const float* inv_scale_ptr, void* stream);
 /* [O][kh][kw][I] fp32 -> OIHW fp32 parameter-gradient layout: dst = alpha*src (+ dst if accumulate) */

@@ -136,7 +136,7 @@ def darknet_forward(module_defs, state, x, cfg_name, training=False, emulate_fp1
     """module_defs: parsed cfg WITHOUT the [net] block; state: state_dict (reference key names).
     eval  -> (io_cat [B, rows, no], [p...])          training -> [p...]  (+ dict of updated running stats)
     emulate_fp16: weights (after BN fold) and every layer output are rounded to fp16, accumulation stays fp32 --
-    the precision policy of the B200 engine (config C1), used to gate the CUDA path tightly."""
+    the precision policy of the H100 engine (config C1), used to gate the CUDA path tightly."""
     outs = []
     yolo_out = []
     n_yolo = sum(1 for d in module_defs if d['type'] == 'yolo')

@@ -1,6 +1,6 @@
 """Generate tests/golden/map_case.npz by RUNNING THE REFERENCE (CPU): yolov3-tiny eval forward on a seeded batch,
 the reference's non_max_suppression / clip_coords / test.py matching loop / ap_per_class.  The reference's own
-detections (conf > 0.3) are the held labels, so its mAP is the self-consistency value of the pipeline; the B200 engine
+detections (conf > 0.3) are the held labels, so its mAP is the self-consistency value of the pipeline; the H100 engine
 must reproduce that mAP within 1e-4 from ITS predictions (tests/test_gpu_model.py), and oracle/metrics_oracle.py is pinned
 against every intermediate stored here (tests/test_oracle_golden.py).
 

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY (never imported by the product path).
 
-CPU restatement of the reference's detection post-processing and mAP bookkeeping, used to check that the B200 engine's
+CPU restatement of the reference's detection post-processing and mAP bookkeeping, used to check that the H100 engine's
 predictions give the same mAP as the reference's on a held synthetic batch (BASELINE north_star: |dmAP| <= 1e-4):
 
   * nms()            <- utils/utils.py:782-860  non_max_suppression (multi-label candidates, per-class offset boxes,

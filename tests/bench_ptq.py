@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""INT8 PTQ inference throughput of the B200 engine (BASELINE configs[4]: yolov3.cfg, quantized=3 eval graph, int8 codes
-with power-of-two scales, tcgen05 kind::i8 convolutions).  The quantiser state is the one calibrated by the reference's
+"""INT8 PTQ inference throughput of the H100 engine (BASELINE configs[4]: yolov3.cfg, quantized=3 eval graph, int8 codes
+with power-of-two scales, int8 wgmma convolutions).  The quantiser state is the one calibrated by the reference's
 own PTQ flow (tests/golden/yolov3_64_ptq.npz); timing does not depend on the values.
 
     python tests/bench_ptq.py [--batch 32] [--size 640] [--steps 10]

@@ -7,7 +7,7 @@ variants the benchmark actually runs -- against fixtures produced by the referen
     gradient of EVERY parameter (element-wise against the fp16-policy oracle, norms against the fp32 reference),
     BatchNorm running statistics.
 
-Every gate below is written as a constant next to the error measured on B200 (printed by the test): <= 2x measured.
+Every gate below is a constant; the test prints the measured errors.
 """
 import numpy as np
 import pytest
@@ -18,13 +18,9 @@ from helpers import anchor_vecs, attach_hyp, build_model, cfg_path, golden, modu
 pytestmark = pytest.mark.gpu
 
 SIZE = 640
-# ---- inference, fp16 activation policy (config C1).  Measured on B200 (gpurun, this file's printout, kept in
-# profiles/r02/parity_640.txt); each gate is 2x the measured value:
-#   yolov3: vs fp32 reference box_rel 8.9e-3 prob_abs 2.8e-3 | vs fp16-policy oracle box_rel 1.5e-2 prob_abs 4.4e-3
-#   yolov4: vs fp32 reference box_rel 2.2e-4 prob_abs 8.8e-5 | vs fp16-policy oracle box_rel 4.0e-4 prob_abs 8.4e-5
-# (yolov3's leaky network with the synthetic weights is the less well conditioned of the two: the policy oracle itself
-#  sits 1.5e-2 / 4.4e-3 from the engine and a similar distance from the fp32 reference -- two different roundings of
-#  the same fp16 policy (mkldnn's fp32 accumulation order vs the tensor core's) end up that far apart.)
+# ---- inference, fp16 activation policy (config C1).  Gates against the fp32 reference and the fp16-policy oracle:
+# (yolov3's leaky network with the synthetic weights is the less well conditioned of the two: two different roundings of
+#  the same fp16 policy (mkldnn's fp32 accumulation order vs the tensor core's) end up far apart.)
 TOL = {"yolov3": {"box_ref": 1.8e-2, "prob_ref": 5.6e-3, "box_emu": 3.0e-2, "prob_emu": 8.8e-3},
        "yolov4": {"box_ref": 4.4e-4, "prob_ref": 1.8e-4, "box_emu": 8.0e-4, "prob_emu": 1.7e-4}}
 
@@ -72,12 +68,6 @@ def test_eval_forward_640_bs32(name):
     be, pe = _errs(io2, io_emu)
     print("\n[%s 640x640 bs32] vs fp32 reference (sampled rows): box_rel=%.3g prob_abs=%.3g | vs fp16-policy oracle "
           "(all rows): box_rel=%.3g prob_abs=%.3g" % (name, bf, pf, be, pe))
-    import json, os
-    os.makedirs(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out"), exist_ok=True)
-    with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out",
-                           "parity_640_%s.json" % name), "w") as f:
-        json.dump({"box_rel_vs_fp32_reference": bf, "prob_abs_vs_fp32_reference": pf,
-                   "box_rel_vs_fp16_policy_oracle": be, "prob_abs_vs_fp16_policy_oracle": pe}, f)
     tol = TOL[name]
     assert bf <= tol["box_ref"] and pf <= tol["prob_ref"]
     assert be <= tol["box_emu"] and pe <= tol["prob_emu"]
@@ -88,7 +78,7 @@ def test_eval_forward_640_bs32(name):
 
 # ---- training step (config C2 per-GPU slice).  The fp16-activation policy perturbs a randomly initialised 110-layer
 # network chaotically less at batch 8 x 640^2 than at the toy sizes (every BatchNorm sees >= 3200 samples), so absolute
-# gates are possible.  measured on B200 (this file's printout):
+# gates are possible:
 def test_train_step_640_bs8():
     from utils import utils as my_utils
     name = "yolov4"
@@ -142,7 +132,7 @@ def test_train_step_640_bs8():
           "%.3g | running stats abs %.3g || vs fp16-policy oracle, every parameter: rel L2 error median %.3g worst %.3g"
           % (items_rel, yard_items, p_abs, np.median(norm_rel), norm_rel.max(), np.median(yard), yard.max(),
              max(elem), stat_err, np.median(pol), pol.max()))
-    # Gates = 2x the values measured on B200 (profiles/r02/parity_640.txt).  The element-wise figures are printed for
+    # The element-wise figures are printed for
     # the record only: the oracle pair (fp32 vs fp16 policy, CPU) itself is uncorrelated on this batch (relative L2
     # error 1.12 median, oracle/README note in DESIGN.md section 4), so they cannot be gated end to end -- the
     # element-wise gates for every parameter are in test_train_step_layerwise below.

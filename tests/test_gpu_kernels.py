@@ -97,7 +97,7 @@ def test_conv2d_tc(case):
 
 
 def test_conv2d_large_multiwave():
-    # more tiles than SMs -> exercises the persistent loop, the smem ring wrap and both TMEM stages
+    # more tiles than SMs -> exercises the persistent loop, the smem ring wrap and the accumulator staging reuse
     err, rms = conv_case(4, 80, 80, 128, 256, 3, 1, "leaky")
     assert err <= 6e-3 * max(rms, 1.0)
 
@@ -233,7 +233,7 @@ def test_conv_weight_stationary_many_tiles(cin, cout, k, stride, res):
     per CTA, the ring carries A only), 8 epilogue warps on alternate tiles, TMA-store epilogue with a partial last tile."""
     ops = _ops()
     g = torch.Generator().manual_seed(21)
-    B, H, W = 2, 110, 100                       # 22000 pixels = 171.9 tiles > 148 SMs
+    B, H, W = 2, 110, 100                       # 22000 pixels = 171.9 tiles > 132 SMs
     x = torch.randn(B, H, W, cin, generator=g).half()
     w = (torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5).half()
     b = torch.randn(cout, generator=g)

@@ -7,7 +7,7 @@ Semantics under test (reference train.py:219-221 = DistributedDataParallel; SURV
   * BatchNorm running buffers follow rank 0 (broadcast_buffers) on the next forward.
 The per-rank gradients are recomputed on rank 0 by the same engine WITHOUT the data-parallel wrapper (plain autograd
 .grad path), so the comparison isolates the exchange step; the engine's gradients themselves are gated against the
-oracle in tests/test_gpu_train_model.py.  Skipped when fewer than two GPUs are visible (run: gpurun --gpus 2)."""
+oracle in tests/test_gpu_train_model.py.  Skipped when fewer than two GPUs are visible."""
 import os
 import socket
 
@@ -92,7 +92,7 @@ def _worker(rank, world, port, out):
 
 def test_two_rank_nccl_training_step():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     world = 2
     mgr = mp.Manager()
     out = mgr.dict()

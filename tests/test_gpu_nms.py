@@ -19,7 +19,7 @@ from oracle import metrics_oracle as mo
 
 pytestmark = pytest.mark.gpu
 
-MERGE_RTOL = 1e-5       # measured on B200: see the printed maxima
+MERGE_RTOL = 1e-5       # the test prints the measured maxima
 
 
 def synth_predictions(B, R, nc, seed, n_obj=30, per_obj=12, bg_pass=0.02, small_boxes=0):

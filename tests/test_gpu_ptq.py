@@ -182,8 +182,7 @@ def test_ptq_native_calibration_matches_reference():
           [(j, round(e, 4)) for j, e in enumerate(bias_err) if e > 0.01][:8])
     print("[ptq calibration] %d weight scales (> 150k elements) taken from the fixture" % big)
     assert not bad
-    # measured on B200: 0 of 298 scales differ; 35 of 21 9xx bias codes off by exactly 1 LSB (corrected biases sitting on a
-    # rounding boundary); corrected float bias median 1.3e-4 LSB, worst 0.67 LSB
+    # bias codes may differ by one LSB where the corrected bias sits on a rounding boundary (the test prints the counts)
     assert worst_qb <= 1.0 and n_qb_off <= 70
     assert float(np.median(bias_err)) < 1e-3 and max(bias_err) < 1.4
     # the INT8 eval graph on the natively calibrated model == the reference's eval output
@@ -203,5 +202,5 @@ def test_ptq_native_calibration_matches_reference():
         frac_far = max(frac_far, float((d > 4.5).float().mean()))
     print("[ptq calibration -> INT8 eval] head codes differing from the reference's eval: %.4g of elements, beyond 4 LSB: %.4g"
           % (frac_off, frac_far))
-    # measured on B200: 56 % of the head codes move by 1-4 LSB (the 35 one-LSB bias codes upstream), none beyond 4 LSB
+    # the one-LSB bias codes upstream move head codes by a few LSB; the printed fractions are the measured values
     assert frac_off < 0.8 and frac_far < 0.01

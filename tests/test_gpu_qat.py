@@ -1,7 +1,7 @@
 """GPU: quantisation-aware-training graphs (quantized=1 google QAT with shortcut_way=1, quantized=2 TPSQ; SURVEY 8a rows a22 /
 a23) against fixtures produced by the reference itself (oracle/gen_golden_qat.py: ONE training step -- forward,
 compute_loss, backward -- of yolov3 at 64x64, batch 2, then an eval forward).  The QAT layers run as module forwards
-over NHWC tensors composed of the sm_100a kernels (b200yolo/qat.py)."""
+over NHWC tensors composed of the sm_90a kernels (b200yolo/qat.py)."""
 import numpy as np
 import pytest
 import torch
@@ -80,7 +80,7 @@ def test_qat_training_step_and_eval_match_reference(name, mode, tag):
     # every layer) amplifies a single flipped code chaotically: the first block agrees with the reference to 5e-7 in the
     # batch statistics and in all but 0.02 % of the output codes, 86 % of the codes differ by layer 36 (tools/debug_qat.py).
     # The end-to-end gates are therefore statistical; the exact gates are per layer on the reference's own tensors
-    # (test_qat_layers_teacher_forced below).  Measured on B200: loss items rel 0.039 / 0.025, grad norms median 0.11 / 0.25.
+    # (test_qat_layers_teacher_forced below).
     assert not missing
     assert items_rel < 0.1
     assert np.median(rel) < 0.5
@@ -133,8 +133,8 @@ def test_qat_layers_teacher_forced(mode, tag):
             if slot:
                 worst[slot] = max(worst[slot], err)
     print("\n[%s layers, teacher forced] %s" % (tag, " ".join("%s=%.3g" % kv for kv in worst.items())))
-    # measured on B200: y off by exactly 1 LSB on 2.4e-3 / 8.5e-4 of the codes (values on a rounding boundary), gx 2.0e-3
-    # (bf16 store of the data gradient), gw 3.8e-4, ggamma 3.5e-4, gbeta 5.5e-7, batch statistics 7.5e-6
+    # y codes may be off by one LSB where a value sits on a rounding boundary; gx carries the bf16 store of the data
+    # gradient (the printed maxima are the measured values)
     assert worst["y_frac_off"] < 5e-3 and worst["y_max_lsb"] <= 2.0
     assert worst["stats"] < 1e-4
     assert worst["gx"] < 5e-3 and worst["gw"] < 1e-3 and worst["ggamma"] < 1e-3 and worst["gbeta"] < 1e-5

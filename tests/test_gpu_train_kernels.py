@@ -1,4 +1,4 @@
-"""GPU parity of the training kernels (dgrad / wgrad tcgen05 GEMMs, BN+activation fwd/bwd, SGD) and the
+"""GPU parity of the training kernels (dgrad / wgrad wgmma GEMMs, BN+activation fwd/bwd, SGD) and the
 quantisation kernels against torch autograd / the oracle on identical fp16-rounded operands."""
 import math
 
@@ -68,9 +68,9 @@ GRAD_CASES = [
     (2, 16, 16, 32, 64, 3, 1),      # Cin=32 (64B swizzle atoms)
     (2, 16, 16, 16, 32, 3, 1),      # Cin=16
     (2, 10, 10, 512, 256, 1, 1),    # yolo head sized (Cout padded to 256 by the caller)
-    (2, 12, 12, 256, 512, 3, 1),    # 4 co tiles, N=256
+    (2, 12, 12, 256, 512, 3, 1),    # 4 co tiles, two N=128 tiles
     (4, 40, 40, 128, 128, 3, 1),    # many k-steps -> split-K > 1
-    # narrow-input 3x3 layers: the tap-transposed weight-gradient kernel (wgrad_taps_kernel)
+    # narrow-input 3x3 layers (Cin 32 / 64)
     (2, 24, 24, 32, 128, 3, 1),     # Cin 32, N = 128 tile
     (3, 20, 22, 32, 64, 3, 2),      # Cin 32, stride 2
     (4, 40, 40, 64, 64, 3, 1),      # Cin 64, 100 k-steps over many split-K slices
@@ -110,6 +110,31 @@ def test_dgrad_fp16_operands_bf16_output_with_device_scale():
     dw = ops.conv2d_bwd_weight(_nhwc(torch.randn(B, Cin, H, W, generator=g)), _nhwc(dz16.float()), k, stride, pad,
                                inv_scale=inv)
     assert torch.isfinite(dw).all()
+
+
+def test_wgrad_concurrent_streams_match_serial():
+    """Weight gradients issued on two streams at once (as the training engine does with its side stream) equal the same
+    gradients computed one after the other, bit for bit: the split-K partial sums of concurrent launches never mix."""
+    ops = _ops()
+    g = torch.Generator().manual_seed(7)
+    cases = [(4, 64, 64, 32, 64), (4, 32, 32, 64, 128), (2, 40, 40, 128, 64)]
+    data = [(_nhwc(torch.randn(B, Ci, H, W, generator=g)), _nhwc(torch.randn(B, Co, H, W, generator=g)))
+            for B, H, W, Ci, Co in cases]
+    serial = [ops.conv2d_bwd_weight(x, dy, 3, 1, 1) for x, dy in data]
+    torch.cuda.synchronize()
+    streams = [torch.cuda.Stream(), torch.cuda.Stream()]
+    main = torch.cuda.current_stream()
+    for s in streams:
+        s.wait_stream(main)
+    outs = [[None] * len(data) for _ in range(4)]
+    for rep in range(4):                     # interleave launches of both streams so that they overlap
+        for i, (x, dy) in enumerate(data):
+            with torch.cuda.stream(streams[(rep + i) % 2]):
+                outs[rep][i] = ops.conv2d_bwd_weight(x, dy, 3, 1, 1)
+    torch.cuda.synchronize()
+    for rep in range(4):
+        for i in range(len(data)):
+            assert torch.equal(outs[rep][i], serial[i]), (rep, cases[i])
 
 
 def test_mixed_f16_bf16_operands_are_rejected():
@@ -292,7 +317,7 @@ def test_fakequant_and_cos_search_match_reference():
 @pytest.mark.parametrize("case", [(2, 20, 20, 64, 128, 3, 1), (2, 20, 20, 128, 256, 1, 1), (1, 40, 40, 32, 64, 3, 2),
                                   (2, 13, 13, 512, 1024, 3, 1)])
 def test_int8_conv_bit_exact(case):
-    """INT8 tcgen05 conv (int32 accumulate) vs the reference's fp32 fake-quant arithmetic: requantised outputs equal."""
+    """INT8 wgmma conv (int32 accumulate) vs the reference's fp32 fake-quant arithmetic: requantised outputs equal."""
     ops = _ops()
     B, H, W, Cin, Cout, k, stride = case
     pad = (k - 1) // 2

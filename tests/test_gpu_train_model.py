@@ -1,4 +1,4 @@
-"""GPU: training step parity (forward with batch-stat BN, YOLO loss, full backward) of the B200 engine against the
+"""GPU: training step parity (forward with batch-stat BN, YOLO loss, full backward) of the H100 engine against the
 fixtures produced by the reference itself on CPU fp32 (tests/golden/*_64_train.npz)."""
 import numpy as np
 import pytest

@@ -12,9 +12,6 @@ import torch
 
 from helpers import GOLD, PKG, ROOT, cfg_path, module_defs, orc
 
-REF = "/root/reference"
-
-
 def _snapshot():
     with open(os.path.join(GOLD, "cfg_snapshot.json")) as f:
         return json.load(f)
@@ -159,22 +156,24 @@ def test_cpu_tensors_fail_loudly():
         my_utils.compute_loss([torch.zeros(1, 3, 2, 2, 85)], torch.zeros(0, 6), m)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present (GPU box)")
-@pytest.mark.parametrize("name,rel", [("yolov3", "cfg/yolov3/yolov3.cfg"), ("yolov3-tiny", "cfg/yolov3tiny/yolov3-tiny.cfg"),
-                                      ("yolov4", "cfg/yolov4/yolov4.cfg"),
-                                      ("yolov3-mobilenet", "cfg/yolov3-mobilenet/yolov3-mobilenet-coco.cfg")])
-def test_generated_cfg_equals_reference_cfg(name, rel):
-    from utils.parse_config import parse_model_cfg
+@pytest.mark.parametrize("name", ["yolov3", "yolov3-tiny", "yolov4", "yolov3-mobilenet"])
+def test_generated_cfg_equals_reference_cfg(name):
+    """the generated cfgs against the reference's own .cfg files, as parsed (tests/golden/ref_cfg_layers.json,
+    written by oracle/gen_golden_cfg.py)."""
+    with open(os.path.join(GOLD, "ref_cfg_layers.json")) as f:
+        ref = json.load(f)[name]
     ours = module_defs(name)
-    ref = parse_model_cfg(os.path.join(REF, rel))[1:]
     assert len(ours) == len(ref)
     keys = ('type', 'batch_normalize', 'filters', 'size', 'stride', 'pad', 'activation', 'layers', 'from', 'mask',
             'classes', 'num')
+
+    def plain(v):
+        return v.tolist() if hasattr(v, "tolist") else v
     for a, b in zip(ours, ref):
         for k in keys:
-            assert a.get(k) == b.get(k), (name, k, a, b)
+            assert plain(a.get(k)) == b.get(k), (name, k, a, b)
         if 'anchors' in b:
-            assert np.array_equal(a['anchors'], b['anchors'])
+            assert np.array_equal(np.asarray(a['anchors']), np.asarray(b['anchors']))
 
 
 def test_prepare_labels_matches_the_reference_expressions():

@@ -2,7 +2,7 @@
 """INT8 PTQ inference throughput (BASELINE configs[4]: yolov3.cfg, quantized=3) with the WHOLE flow on the device and no
 test infrastructure: PTQ.py's calibration (`q_model.train()` + forwards over calibration batches, b200yolo/qcalib.py:
 cosine votes, bias correction, shortcut / concat searches) on two small synthetic batches, then the INT8 eval graph
-(tcgen05 kind::i8 convolutions, power-of-two requantisation) at the benchmark size.
+(int8 wgmma convolutions, power-of-two requantisation) at the benchmark size.
 
     python tools/bench_ptq_native.py [--batch 32] [--size 640] [--steps 10]
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Training-step throughput of the B200 engine (BASELINE configs[2]: yolov4.cfg, 8 images / GPU, 640x640):
+"""Training-step throughput of the H100 engine (BASELINE configs[2]: yolov4.cfg, 8 images / GPU, 640x640):
 forward (batch-stat BN) + YOLO loss + backward + ONE gradient all-reduce + fused SGD-Nesterov.
 
     python tools/bench_train.py [--model yolov4] [--batch 8] [--size 640] [--steps 10]

@@ -4,7 +4,7 @@ parameter gradients).  Environment knobs are read once per process, so run one p
 
     B2Y_PDL=0 python tools/flake_probe.py 4
 
-Finding (gpurun_out/flake_probe.log of round 2, kept in profiles/r02c/): deviations of 1e-3..3e-2 appear on the leaky-ReLU
+Finding (an earlier run on another GPU generation; not re-measured on H100): deviations of 1e-3..3e-2 appear on the leaky-ReLU
 layers of the yolov4 neck in about a third of the iterations under EVERY configuration (PDL on / off, weight gradients on
 the side stream or not, TMA-store epilogue or not, eager or graph replay) and never on the Mish layers: they are elements
 with |u| below fp32 rounding, whose branch of the leaky-ReLU derivative differs between the engine's fma(z, scale, shift)

@@ -1,5 +1,5 @@
 """Debug driver (not a pytest file): run conv parity cases one process per case so that a trapped kernel
-(bounded mbarrier wait -> __trap) cannot poison the following cases.  Usage on the GPU box:
+(bounded mbarrier wait -> __trap) cannot poison the following cases.  Usage on a GPU machine:
     python tests/gpu_debug_conv.py            # all cases, one subprocess each
     python tests/gpu_debug_conv.py 3          # a single case in-process
 """

@@ -1,7 +1,7 @@
 """Run the bench's NMS + TP-matching block a few times (for an ncu launch list of csrc/nms.cu):
 
     ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none --csv \\
-        --log-file gpurun_out/launches_nms.csv python tools/nms_profile.py
+        --log-file launches_nms.csv python tools/nms_profile.py
 """
 import os
 import sys

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-launch timing of one step of the B200 engine (measurement tool, not part of the product path).
+"""Per-launch timing of one step of the H100 engine (measurement tool, not part of the product path).
 
     python tools/profile_calls.py --mode train|infer [--model yolov4] [--batch 8] [--size 640] [--out FILE.json]
 

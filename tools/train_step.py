@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """N eager (or graph-replayed) YOLOv4 training steps, 8 images, 640x640 -- the bench.py headline workload without the
-measurement scaffolding; the target of the ncu captures in profiles/capture_r02.sh.
+measurement scaffolding; a target for profiler captures.
 
     python tools/train_step.py [--steps 2] [--model yolov4] [--batch 8] [--graph]
 """

@@ -3,7 +3,7 @@
 The production path keeps activations and weights in fp16 (BASELINE configs[1]); every stored activation carries a
 2^-11 relative rounding, which is what separates its detections from the fp32 reference's by ~1e-3 in probability and
 keeps the held-batch mAP from matching to 1e-4 (a few candidates straddle the confidence threshold).  This mode exists
-for that gate (SURVEY.md section 7 "hard parts"): the same tcgen05 convolution kernels, but
+for that gate (SURVEY.md section 7 "hard parts"): the same wgmma convolution kernels, but
 
   * activations live in fp32 (NHWC) between layers and enter a conv as a two-term fp16 split x = x_hi + x_lo,
   * folded weights likewise w = w_hi + w_lo,

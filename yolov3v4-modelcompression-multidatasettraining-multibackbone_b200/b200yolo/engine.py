@@ -1,9 +1,9 @@
-"""Graph executor for Darknet models on sm_100a.
+"""Graph executor for Darknet models on sm_90a.
 
 Replaces the reference's per-module Python loop (models.py:508-561, ~250-520 ATen/cuDNN launches per forward)
 by a static plan over NHWC fp16 buffers:
 
-  * conv + folded BN + activation (+ the following Shortcut) = one tcgen05 implicit-GEMM launch,
+  * conv + folded BN + activation (+ the following Shortcut) = one wgmma implicit-GEMM launch,
   * route/concat is zero-copy: producers write straight into their channel slot of the concat buffer,
   * the stem reads the NCHW fp32 image directly, the head convs emit fp32 for the decode kernel,
   * the launch sequence is captured once into a CUDA graph per input shape and replayed.
@@ -146,7 +146,7 @@ class Plan:
             elif t in ('shortcut', 'yolo'):
                 pass
             else:
-                raise NotImplementedError("layer type '%s' is not supported by the sm_100a engine yet" % t)
+                raise NotImplementedError("layer type '%s' is not supported by the sm_90a engine yet" % t)
             prev = (C, H, W)
             shapes.append(prev)
 
@@ -238,7 +238,7 @@ class Plan:
             elif t == 'convolutional':
                 conv, bn, act, slope = _block_parts(m)
                 if conv.groups != 1:
-                    raise NotImplementedError("grouped convolution is not supported by the sm_100a engine yet")
+                    raise NotImplementedError("grouped convolution is not supported by the sm_90a engine yet")
                 out = alloc(tens[i])
                 res = None
                 if i + 1 < n and fused_into[i + 1] == i:
@@ -251,7 +251,7 @@ class Plan:
                     continue
                 frm = [i + l if l < 0 else l for l in d['from']]
                 if getattr(m, 'weight', False):
-                    raise NotImplementedError("weighted shortcut is not supported by the sm_100a engine yet")
+                    raise NotImplementedError("weighted shortcut is not supported by the sm_90a engine yet")
                 out = alloc(tens[i])
                 cur = tens[i - 1]
                 for s in frm:
@@ -494,7 +494,7 @@ class Plan:
     def profile_layers(self, x, reps=10):
         """Per-launch CUDA-event timing.  Each step is captured `reps` times back to back in its own CUDA graph and the
         replay is timed (best of 3), so the CPU launch cost of eager calls (tensor-map encodes, ctypes) is excluded;
-        consecutive launches of one layer re-use its tensors, so layers whose working set fits the 126 MB L2 are
+        consecutive launches of one layer re-use its tensors, so layers whose working set fits the 50 MB L2 are
         measured L2-warm (like in the real graph, where the producer layer just wrote them)."""
         x = x.contiguous()
         if self.param_version is None:
@@ -527,7 +527,7 @@ class Plan:
         return rows
 
     def time_tc_convs(self, x, iters=5):
-        """Time only the tcgen05 conv launches of one forward, back to back on the current stream.
+        """Time only the wgmma conv launches of one forward, back to back on the current stream.
         Returns (ms per forward-worth of conv launches, algorithmic FLOPs of those launches, n launches)."""
         x = x.contiguous().float()
         if self.param_version is None:
@@ -643,7 +643,7 @@ class Engine:
         if p is not None and p.device != x.device:
             raise RuntimeError(
                 "b200yolo: input on %s but the model's parameters are on %s. Single-process multi-GPU "
-                "(nn.DataParallel) is not supported by the sm_100a engine: run one process per GPU "
+                "(nn.DataParallel) is not supported by the sm_90a engine: run one process per GPU "
                 "(CUDA_VISIBLE_DEVICES / --device 0, or torchrun + FlatDataParallel)." % (x.device, p.device))
 
     def forward(self, x):

@@ -57,7 +57,7 @@ class QConvDesc(C.Structure):
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
-            "libb200yolo.so not built: run `python %s` (nvcc, sm_100a). There is no fallback path."
+            "libb200yolo.so not built: run `python %s` (nvcc, sm_90a). There is no fallback path."
             % os.path.join(_PKG, "build.py"))
     return C.CDLL(LIB_PATH)
 
@@ -190,7 +190,7 @@ def raw():
 
 
 # Launch recorder (measurement only, bench.py / tools): while RECORD is a list every C-ABI call is appended as
-# (name, args) so that a family of launches (e.g. all tcgen05 convolutions of one step) can be replayed back to back.
+# (name, args) so that a family of launches (e.g. all wgmma convolutions of one step) can be replayed back to back.
 RECORD = None
 KEEPALIVE = []      # tensors whose pointers were handed out while recording (temporaries must outlive the replay)
 

@@ -309,7 +309,7 @@ def conv2d_bwd_weight(x, dy, k, stride, pad, scale=1.0, dw=None, inv_scale=None)
     if dw is None:
         dw = torch.zeros((O, k, k, I), dtype=torch.float32, device=x.device)
     d = ConvDesc(B, H, W, I, _pitch(x), O, k, stride, pad, Ho, Wo, _pitch(dy), 0, 0.0, OUT_F16, 0)
-    assert x.dtype == dy.dtype, "tcgen05 kind::f16 needs both operands in the same 16-bit format"
+    assert x.dtype == dy.dtype, "wgmma needs both operands in the same 16-bit format"
     call("b2y_conv2d_bwd_weight", C.byref(d), ptr(x), ptr(dy), ptr(dw), float(scale), _gdt(dy), ptr(inv_scale),
          stream_ptr())
     return dw

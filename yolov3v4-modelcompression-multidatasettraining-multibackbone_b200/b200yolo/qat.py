@@ -1,11 +1,11 @@
-"""Quantisation-aware-training execution (quantized=1 google, quantized=2 TPSQ) on sm_100a.
+"""Quantisation-aware-training execution (quantized=1 google, quantized=2 TPSQ) on sm_90a.
 
 Reference: utils/quantized/quantized_google.py:235-836 / quantized_TPSQ.py:349-589.  A QAT layer is two convolutions per
 training step (a plain one for the BatchNorm batch statistics, one on the fake-quantised folded weights), fake-quant with
 straight-through gradients on weights / bias / activations, and a BN fold whose gradient flows through the batch
 statistics.  That chain is data dependent per step (range trackers, freeze steps), so it is not captured in a static plan:
 the module forwards of utils/quantized/*.py are executed one by one over NHWC fp32 tensors, composed from the autograd
-Functions below -- each of which runs the hand-written kernels (tcgen05 forward / data-gradient / weight-gradient convs,
+Functions below -- each of which runs the hand-written kernels (wgmma forward / data-gradient / weight-gradient convs,
 fake-quant forward / STE backward, activation forward / backward) -- while torch.autograd only chains them and handles the
 per-channel [C]-sized fold arithmetic.
 
@@ -26,8 +26,8 @@ def _pow2_scale(g):
 
 
 class ConvFn(torch.autograd.Function):
-    """y[, sum_c y, sum_c y^2] = conv2d(x NHWC fp32, w OIHW fp32) on the tcgen05 fp16 kernel with fp32 accumulation / output.
-    backward: weight gradient + data gradient on the tcgen05 backward kernels (dz as fp16 x 2^k, k chosen on the device).
+    """y[, sum_c y, sum_c y^2] = conv2d(x NHWC fp32, w OIHW fp32) on the wgmma fp16 kernel with fp32 accumulation / output.
+    backward: weight gradient + data gradient on the wgmma backward kernels (dz as fp16 x 2^k, k chosen on the device).
     The optional channel sums come out of the conv epilogue and are differentiable (their gradients are folded into dz)."""
 
     @staticmethod

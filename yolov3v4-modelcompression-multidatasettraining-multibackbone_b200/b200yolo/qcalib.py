@@ -1,4 +1,4 @@
-"""PTQ calibration forward (quantized=3, model.train()) on sm_100a -- what the reference's PTQ.py:76-88 calls before
+"""PTQ calibration forward (quantized=3, model.train()) on sm_90a -- what the reference's PTQ.py:76-88 calls before
 the INT8 eval graph (qengine.py) can run.  Reference: utils/quantized/quantized_ptq_cos.py
   conv      :193-296 (fold, quantise W / b once, quantised conv + "correct" conv, bias correction), :543-567 activation,
             :717-721 activation quantiser vote
@@ -8,7 +8,7 @@ the INT8 eval graph (qengine.py) can run.  Reference: utils/quantized/quantized_
 
 How it runs here.  In the reference every tensor of the quantised branch is an fp32 tensor whose values sit on a
 power-of-two grid (int8 code x 2^e) and every conv is F.conv2d on those floats.  Such values (and the fake-quantised
-weights) are exact in fp16 and their products / fp32 partial sums are exact, so the quantised conv runs on the tcgen05
+weights) are exact in fp16 and their products / fp32 partial sums are exact, so the quantised conv runs on the wgmma
 fp16 kernel with fp32 output and reproduces the reference's accumulators exactly (the int8 kernel cannot be used during
 calibration: a concat of tensors with different scales has no single int8 scale, and the reference does not requantise
 in training mode, :1533-1534).  The "correct" conv (quantised input x FLOAT folded weights, fp32 in the reference) uses a
@@ -46,7 +46,7 @@ class QCalibPlan:
         return ops.fakequant_range(x, scale, -3.0e38, 3.0e38)
 
     def _conv(self, x16, w_oihw_f32_vals, k, s, p):
-        """tcgen05 conv of fp16 NHWC values with weights given as fp32 OIHW whose values are exact in fp16 -> fp32"""
+        """wgmma conv of fp16 NHWC values with weights given as fp32 OIHW whose values are exact in fp16 -> fp32"""
         wp, _, _ = ops.pack_conv_weights(w_oihw_f32_vals.contiguous())
         return ops.conv2d(x16, wp, None, k, s, p, out_dtype=torch.float32)
 

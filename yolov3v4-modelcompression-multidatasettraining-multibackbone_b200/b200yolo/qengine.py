@@ -4,7 +4,7 @@ The reference *simulates* int8 in fp32: every tensor is a float on a power-of-tw
 floats (utils/quantized/quantized_ptq_cos.py:288-296).  Because all scales are powers of two the products are exact
 integers times a power of two, so the same arithmetic runs here on the real int8 codes:
 
-   conv      int8 x int8 -> int32 on tcgen05 kind::i8, epilogue  acc*(s_in*s_w) + q_bias -> act -> requant(s_act)
+   conv      int8 x int8 -> int32 on int8 wgmma, epilogue  acc*(s_in*s_w) + q_bias -> act -> requant(s_act)
    shortcut  folded into the epilogue of the conv that feeds it (b2y_qconv2d_shortcut_fwd) when nothing else reads that
              conv's output; otherwise b2y_qshortcut_i8 (both addends rounded onto scale_x / scale_a, sum requantised)
    concat    b2y_requant_i8 of every source onto the concat scale, written into its channel slot
@@ -170,7 +170,7 @@ class QPlan:
                     raise RuntimeError("layer %d is not calibrated (scale == 0): load a calibrated state_dict" % i)
                 bits_w, bits_a = conv.w_bits, conv.a_bits
                 if bits_w > 8 or bits_a > 8:
-                    raise NotImplementedError("the tcgen05 kind::i8 path covers <= 8 bit weights and activations")
+                    raise NotImplementedError("the int8 wgmma path covers <= 8 bit weights and activations")
                 act = _ACT_NAME[conv.activate]
                 slope = 0.25 if conv.maxabsscaler else 0.1
                 if src is None:
@@ -187,7 +187,7 @@ class QPlan:
                 if s_w <= 0 or s_a <= 0:
                     raise RuntimeError("layer %d is not calibrated (scale == 0): load a calibrated state_dict" % i)
                 if conv.w_bits > 8 or conv.a_bits > 8:
-                    raise NotImplementedError("the tcgen05 kind::i8 path covers <= 8 bit weights and activations")
+                    raise NotImplementedError("the int8 wgmma path covers <= 8 bit weights and activations")
                 w8, bq, mode = self._pack_qconv(src, conv, s_w)
                 self.packed[i] = (w8, bq, scale_of[id(src)] * s_w, s_a, _ACT_NAME[conv.activate],
                                   0.25 if conv.maxabsscaler else 0.1, conv.a_bits, mode)

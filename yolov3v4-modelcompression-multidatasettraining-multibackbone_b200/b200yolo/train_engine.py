@@ -1,16 +1,16 @@
-"""Training-mode executor: forward with batch-statistics BatchNorm and the full backward pass on sm_100a.
+"""Training-mode executor: forward with batch-statistics BatchNorm and the full backward pass on sm_90a.
 
 Replaces autograd over ~500 ATen/cuDNN calls (reference train.py:380-441 -> models.py:508-551) by a static plan:
 
-  forward   conv (tcgen05, per-channel sum / sum^2 from the epilogue) -> bn_finalize -> bn+act(+shortcut) apply
-  backward  yolo permute^T -> [bn+act backward reduce / apply -> wgrad (tcgen05, pixel-K GEMM) -> dgrad (tcgen05)]
+  forward   conv (wgmma, per-channel sum / sum^2 from the epilogue) -> bn_finalize -> bn+act(+shortcut) apply
+  backward  yolo permute^T -> [bn+act backward reduce / apply -> wgrad (wgmma, pixel-K GEMM) -> dgrad (wgmma)]
 
 Activations z (raw conv output) and y (post activation) are kept in NHWC fp16 (accurate forward).  Gradients w.r.t.
 activations (dY) are stored in **bf16** (fp32 range: their magnitude drifts by orders of magnitude across ~100
 BatchNorm layers, which fp16 cannot hold with one loss scale).  The conv data gradient dZ, which is an operand of the
 two tensor-core GEMMs (dgrad with the fp16 weights, wgrad with the fp16 activations), is written in fp16 times a
-per-layer power-of-two scale chosen inside the BN-backward kernel from a bound on max|dZ| (tcgen05 kind::f16 faults on
-mixed f16/bf16 operands); the GEMM epilogues read 1/scale from device memory, so there is no host synchronisation.
+per-layer power-of-two scale chosen inside the BN-backward kernel from a bound on max|dZ| (wgmma takes one 16-bit format for
+both operands); the GEMM epilogues read 1/scale from device memory, so there is no host synchronisation.
 Weight / BN gradients are accumulated and stored in fp32.
 The plan plugs into autograd as ONE torch.autograd.Function whose inputs are the model parameters, so
 loss.backward(), DistributedDataParallel hooks and torch optimisers work unchanged.
@@ -94,7 +94,7 @@ class TrainPlan:
             elif t in ('shortcut', 'yolo'):
                 pass
             else:
-                raise NotImplementedError("layer type '%s' is not supported by the sm_100a training engine yet" % t)
+                raise NotImplementedError("layer type '%s' is not supported by the sm_90a training engine yet" % t)
             prev = (Cc, H, W)
             shapes.append(prev)
 
@@ -206,7 +206,7 @@ class TrainPlan:
                     if conv.groups != conv.in_channels or conv.out_channels != conv.in_channels or bn is None or i == 0:
                         raise NotImplementedError("depthwise block: channel multiplier 1 with BatchNorm expected")
                 elif conv.groups != 1:
-                    raise NotImplementedError("grouped convolution is not supported by the sm_100a engine yet")
+                    raise NotImplementedError("grouped convolution is not supported by the sm_90a engine yet")
                 r.i, r.conv, r.bn, r.act, r.slope = i, conv, bn, act, slope
                 r.k, r.s, r.p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
                 r.head, r.stem = is_head[i], (i == 0)
@@ -357,7 +357,7 @@ class TrainPlan:
 
     def _pack(self):
         """fp32 master weights -> fp16 operand layouts (forward [O][k][k][I], per-phase data-gradient slabs): ONE
-        table-driven launch over all tcgen05 convolutions (csrc/multi.cu) + the stem's own tiny pack."""
+        table-driven launch over all wgmma convolutions (csrc/multi.cu) + the stem's own tiny pack."""
         from .lib import PackItem, raw
         body = [r for r in self.convs if not r.stem and not r.depthwise]
         key = tuple(r.conv.weight.data_ptr() for r in body)
@@ -480,7 +480,7 @@ class TrainPlan:
         return d
 
     def _unpack_all(self):
-        """packed fp32 weight gradients [O][k][k][I] of all tcgen05 convolutions -> OIHW destinations, ONE launch."""
+        """packed fp32 weight gradients [O][k][k][I] of all wgmma convolutions -> OIHW destinations, ONE launch."""
         from .lib import UnpackItem, raw
         body = [r for r in self.convs if not r.stem and not r.depthwise]
         dsts = [self._grad_dst(r.conv.weight) for r in body]

@@ -1,4 +1,4 @@
-"""Build libb200yolo.so (sm_100a only) in-tree with nvcc.
+"""Build libb200yolo.so (sm_90a only) in-tree with nvcc.
 
     python build.py            # incremental: rebuilds only when a source is newer than the .so
     python build.py --force
@@ -19,7 +19,7 @@ OBJ_DIR = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-O3", "-std=c++17", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr", "--extended-lambda",
     "-I", INCLUDE, "-I", CSRC,
@@ -60,7 +60,7 @@ def build(force=False, verbose=False):
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(lambda s: _compile(s, verbose), srcs))
     if (not os.path.exists(OUT)) or any(os.path.getmtime(o) > os.path.getmtime(OUT) for o in objs):
-        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

@@ -11,7 +11,7 @@
 // Layout: NHWC, C % 8 == 0.  A thread owns ONE 8-channel vector for the whole kernel (its per-channel coefficients
 // live in registers) and walks pixels with a fixed stride; U independent 16-byte loads per operand are issued before
 // any arithmetic so that enough bytes are in flight per SM to cover HBM latency (the round-1 kernels issued one load
-// per operand per iteration and ran at 0.8-1.5 TB/s).  Block = CV * (256 / CV) threads (CV = C/8 <= 256), grid = one
+// per operand per iteration and were latency bound).  Block = CV * (256 / CV) threads (CV = C/8 <= 256), grid = one
 // wave of 2 CTAs per SM.
 #include "b200yolo.h"
 #include "common.cuh"
@@ -52,8 +52,8 @@ inline int wave_grid(long long pixels, int ppb, int ctas_per_sm) {
     int dev = 0;
     cudaGetDevice(&dev);
     int& sms = sm_count[dev & 63];
-    if (sms <= 0 && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
-    if (sms <= 0) sms = 148;
+    if (sms <= 0 && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
+    if (sms <= 0) sms = 132;
     long long g = (pixels + ppb - 1) / ppb;
     const long long cap = (long long)sms * ctas_per_sm;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
@@ -141,7 +141,7 @@ bn_train_fwd_kernel(const __half* __restrict__ z, long long zp, const float* __r
 template <typename GT, int ACT, int U>
 __global__ void __launch_bounds__(256, 2)
 bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT* __restrict__ dy, long long dp,
-                           const float* __restrict__ save, float* __restrict__ sums, float* __restrict__ du_absmax,
+                           const float* __restrict__ save, double* __restrict__ sums, float* __restrict__ du_absmax,
                            long long pixels, int CV, int PPB, int act_rt, float slope, int pf) {
     __shared__ float red[256][17];
     pdl_wait();
@@ -212,9 +212,9 @@ bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT*
         float sum = 0.f;
         for (int k = 0; k < PPB; ++k) sum += red[v + k * CV][comp];
         if (comp < 8)
-            atomicAdd(sums + v * 8 + comp, sum);
-        else
-            atomicAdd(sums + C + v * 8 + comp - 8, sum * __ldg(save + C + v * 8 + comp - 8));   // * invstd -> sum du*xhat
+            atomicAdd(sums + v * 8 + comp, (double)sum);
+        else   // * invstd -> sum du*xhat
+            atomicAdd(sums + C + v * 8 + comp - 8, (double)(sum * __ldg(save + C + v * 8 + comp - 8)));
     }
 }
 
@@ -369,19 +369,21 @@ extern "C" int b2y_bn_train_bwd_reduce(const void* z, long long z_pitch, const v
     const Geo g = geo_for(c);
     const int grid = wave_grid(pixels, g.PPB, 2);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* acc = stream_acc(st, 2LL * c);     // [0, C) sum du, [C, 2C) sum du*xhat
+    if (acc == nullptr) return B2Y_ERR_CUDA;
     dispatch_act(act, [&](auto A) {
         constexpr int ACT = decltype(A)::value;
         if (grad_dtype == B2Y_DT_BF16)
             launch_pdl(bn_train_bwd_reduce_kernel<__nv_bfloat16, ACT, 4>, dim3(grid), dim3(256), 0, st, 
                 reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, save,
-                sums, du_absmax, pixels, g.CV, g.PPB, act, slope, bn_prefetch());
+                acc, du_absmax, pixels, g.CV, g.PPB, act, slope, bn_prefetch());
         else
             launch_pdl(bn_train_bwd_reduce_kernel<__half, ACT, 4>, dim3(grid), dim3(256), 0, st, 
-                reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, save, sums,
+                reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, save, acc,
                 du_absmax, pixels, g.CV, g.PPB, act, slope, bn_prefetch());
     });
     B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
+    return acc_finalize(acc, sums, 2LL * c, st);
 }
 
 extern "C" int b2y_bn_train_bwd_apply(const void* z, long long z_pitch, const void* dy, long long dy_pitch,

@@ -1,5 +1,5 @@
-// Shared device helpers for the b200yolo kernels (sm_100a only).
-// Thin inline-PTX wrappers around mbarrier / TMA / tcgen05 / TMEM.
+// Shared device helpers for the b200yolo kernels (sm_90a).
+// Thin inline-PTX wrappers around mbarrier / TMA / clusters / wgmma operands.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -8,6 +8,7 @@
 #include <stdint.h>
 
 #include "b200yolo.h"  // status codes + activation ids (single source of truth)
+#include "wgmma.cuh"
 
 namespace b2y {
 
@@ -202,176 +203,68 @@ __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.w
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_cta() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- CTA-pair (cta_group::2) variants: both CTAs of the pair issue their own loads, all of them complete on the
-// mbarrier of the leader CTA (rank 0), addressed through the shared::cluster window (mapa).
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t cta_rank) {
     uint32_t r;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(cta_rank));
     return r;
 }
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
 }
-__device__ __forceinline__ void tma2_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma2_load_im2col_4d(uint32_t dst, const CUtensorMap* m, uint32_t leader_bar, int c, int w,
-                                                    int h, int n, uint16_t off_w, uint16_t off_h) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w),
-        "h"(off_h)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// arrives on the barrier at this smem offset in every CTA of `mask` once all prior cta_group::2 MMAs retire
-__device__ __forceinline__ void tc_commit2_multicast_s(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"(mask)
-                 : "memory");
-}
-// D[tmem of both CTAs, 256 rows] (+)= A[smem of both CTAs] * B[N/2 rows in each CTA's smem]
-__device__ __forceinline__ void mma2_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma2_i8_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// named barrier over `nthreads` threads (a multiple of 32); id 0 is __syncthreads()
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// tcgen05.commit: arrive on an mbarrier when all prior MMAs issued by this thread retire.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-__device__ __forceinline__ void tc_commit_s(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit_multicast_s(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"(mask)
-                 : "memory");
-}
-
-// commit that arrives on the barrier at the same smem offset in every CTA of `mask` (cluster multicast)
-__device__ __forceinline__ void tc_commit_multicast(uint64_t* bar, uint16_t mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(mask)
-        : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc];  kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// kind::i8 (int8 in, int32 accumulate)
-__device__ __forceinline__ void mma_i8_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread = TMEM lane).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-
-// Shared-memory matrix descriptor (tcgen05), swizzled canonical layouts.
-//   K-major : rows of `row_bytes` (32/64/128 = swizzle span), 8-row groups SBO apart.
-//   bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout type
+// ---------------------------------------------------------------- wgmma operands / accumulators
+// Shared-memory matrix descriptor (wgmma), swizzled canonical layouts.
+//   bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) swizzle: 1 = 128B, 2 = 64B, 3 = 32B
+//   K-major: rows of `row_bytes` (= the swizzle span), 8-row groups SBO apart.  Tiles start 1024-byte aligned.
 __host__ __device__ __forceinline__ uint64_t smem_desc_base(uint32_t lbo_bytes, uint32_t sbo_bytes,
                                                             uint32_t layout_type) {
     uint64_t d = 0;
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout_type & 7) << 61;
+    d |= (uint64_t)(layout_type & 3) << 62;
     return d;
 }
 __device__ __forceinline__ uint64_t smem_desc_at(uint64_t base, uint32_t smem_addr) {
     return base | (uint64_t)((smem_addr >> 4) & 0x3FFF);
 }
 __host__ __device__ constexpr uint32_t swizzle_layout_type(int row_bytes) {
-    return row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : (row_bytes == 32 ? 6u : 0u));
+    return row_bytes == 128 ? 1u : (row_bytes == 64 ? 2u : (row_bytes == 32 ? 3u : 0u));
 }
 
-// Instruction descriptor (upper 32 bits of the idesc operand).
-//   c_format [4,6): 1=F32 2=S32 | a_format [7,10) | b_format [10,13) | a_major 15 | b_major 16
-//   n_dim [17,23) = N>>3 | m_dim [24,29) = M>>4
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t c_fmt, uint32_t a_fmt, uint32_t b_fmt, uint32_t a_mn_major,
-                                                  uint32_t b_mn_major, uint32_t M, uint32_t N) {
-    return (c_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-           ((M >> 4) << 24);
+// fp32 accumulator staging tile [rows][N] in smem, 16-byte granules XOR-swizzled by (row & 7): conflict-free row reads
+// (thread = row) and at most two-way conflicts on the fragment stores.  N >= 32.
+template <int N>
+__device__ __forceinline__ uint32_t stage_off(int row, int col) {   // byte offset of (row, col), col % 2 == 0
+    return (uint32_t)(row * N * 4) + ((uint32_t)(((col >> 2) ^ (row & 7))) << 4) + (uint32_t)((col & 3) * 4);
+}
+// the wgmma accumulator fragment of this thread (64 x N block of a warpgroup, rows row0 .. row0 + 63) -> staging tile
+template <int N, typename T>
+__device__ __forceinline__ void frag_to_stage(const T (&d)[N / 2], uint8_t* stage, int row0, int tid_in_wg) {
+    const int r = row0 + 16 * (tid_in_wg >> 5) + ((tid_in_wg & 31) >> 2);
+    const int c = 2 * (tid_in_wg & 3);
+#pragma unroll
+    for (int i = 0; i < N / 8; ++i) {
+        *reinterpret_cast<uint2*>(stage + stage_off<N>(r, 8 * i + c)) =
+            make_uint2(reinterpret_cast<const uint32_t&>(d[4 * i]), reinterpret_cast<const uint32_t&>(d[4 * i + 1]));
+        *reinterpret_cast<uint2*>(stage + stage_off<N>(r + 8, 8 * i + c)) =
+            make_uint2(reinterpret_cast<const uint32_t&>(d[4 * i + 2]), reinterpret_cast<const uint32_t&>(d[4 * i + 3]));
+    }
+}
+// 32 consecutive 32-bit accumulators of one row (columns c0 .. c0 + 31) from the staging tile
+template <int N>
+__device__ __forceinline__ void stage_row32(const uint8_t* stage, int row, int c0, uint32_t (&r)[32]) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+        const uint4 u = *reinterpret_cast<const uint4*>(stage + stage_off<N>(row, c0 + 4 * q));
+        r[4 * q] = u.x;
+        r[4 * q + 1] = u.y;
+        r[4 * q + 2] = u.z;
+        r[4 * q + 3] = u.w;
+    }
 }
 
 // ---------------------------------------------------------------- activations (fp32)
@@ -525,3 +418,30 @@ static inline bool b2y_first_use_on_device(unsigned long long& mask) {
     } while (0)
 
 extern "C" void b2y_set_last_cuda_error(int e);
+
+// Order-independent reductions: a kernel whose CTAs add partial sums into one fp32 result adds them into a double
+// accumulator instead, and acc_finalize then adds the rounded total into the fp32 destination and clears the
+// accumulator.  A double sum of fp32 terms is exact unless the terms span more than 29 binades, so in practice the result
+// no longer depends on the order of the atomics: batch-statistics BatchNorm over fp16 activations magnifies last-bit
+// differences step after step, and without this two runs of the same training diverge within a few steps, which would
+// make the outputs of two builds impossible to compare.
+//
+// stream_acc(st, n) returns the zero-filled accumulator (>= n doubles) owned by the current device and stream `st`:
+// launches on one stream are ordered and each finalizes (clears) what it used before the next one starts, and launches
+// on different streams never share an accumulator.
+double* stream_acc(cudaStream_t st, long long n);
+
+template <int UNUSED = 0>
+__global__ void acc_finalize_kernel(double* __restrict__ acc, float* __restrict__ dst, long long n) {
+    b2y::pdl_wait();
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        dst[i] += (float)acc[i];
+        acc[i] = 0.0;
+    }
+}
+static inline int acc_finalize(double* acc, float* dst, long long n, cudaStream_t st) {
+    long long grid = (n + 255) / 256;
+    if (grid > 132 * 16) grid = 132 * 16;
+    B2Y_CUDA_CHECK(b2y::launch_pdl(acc_finalize_kernel<0>, dim3((unsigned)grid), dim3(256), 0, st, acc, dst, n));
+    return B2Y_OK;
+}

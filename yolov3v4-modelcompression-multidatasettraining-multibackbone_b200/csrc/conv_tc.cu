@@ -1,4 +1,4 @@
-// Host side of the tcgen05 implicit-GEMM convolution: TMA tensor-map encoding, tile-shape dispatch,
+// Host side of the wgmma implicit-GEMM convolution: TMA tensor-map encoding, tile-shape dispatch,
 // C-ABI entry points (include/b200yolo.h).
 #include "conv_tc.cuh"
 
@@ -37,7 +37,7 @@ static void resolve_driver() {
     cudaDriverGetVersion(&g_driver_version);
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
 }
 
 static CUtensorMapSwizzle swizzle_enum(int kbytes) {
@@ -92,11 +92,23 @@ static int make_map_im2col(CUtensorMap* m, const void* base, int esize, int N, i
     return B2Y_OK;
 }
 
-template <int BLOCK_N, int KBYTES, int KIND, int CLUSTER, int PAIR = 0>
+// Adds the batch statistics accumulated in double (stream_acc: [0, CONV_STAT_MAX) sums, [CONV_STAT_MAX, ...) squares)
+// into the caller's fp32 buffers and clears the accumulator; a programmatic dependent of the convolution.
+__global__ void stats_finalize_kernel(double* __restrict__ acc, int C, float* __restrict__ sum, float* __restrict__ sqsum) {
+    pdl_wait();
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    sum[c] += (float)acc[c];
+    sqsum[c] += (float)acc[CONV_STAT_MAX + c];
+    acc[c] = 0.0;
+    acc[CONV_STAT_MAX + c] = 0.0;
+}
+
+template <int BLOCK_N, int KBYTES, int KIND, int CLUSTER>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const ConvTcParams& p,
                       cudaStream_t st) {
     using Cfg = ConvTcCfg<BLOCK_N, KBYTES>;
-    auto kern = conv_tc_kernel<BLOCK_N, KBYTES, KIND, CLUSTER, PAIR>;
+    auto kern = conv_tc_kernel<BLOCK_N, KBYTES, KIND, CLUSTER>;
     static unsigned long long attr_set = 0;      // one bit per device: the attribute is per (function, device)
     if (b2y_first_use_on_device(attr_set)) {
         B2Y_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -111,7 +123,7 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
     }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(clusters * CLUSTER);
-    cfg.blockDim = dim3(ConvTcEpi<BLOCK_N>::THREADS);
+    cfg.blockDim = dim3(ConvTcEpi::THREADS);
     cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
@@ -145,34 +157,23 @@ static int dispatch(int block_n, int kbytes, int cluster, const CUtensorMap& a, 
     B2Y_CASE(32, 32) B2Y_CASE(32, 64) B2Y_CASE(32, 128)
     B2Y_CASE(64, 32) B2Y_CASE(64, 64) B2Y_CASE(64, 128)
     B2Y_CASE(128, 32) B2Y_CASE(128, 64) B2Y_CASE(128, 128)
-    B2Y_CASE(256, 32) B2Y_CASE(256, 64) B2Y_CASE(256, 128)
 #undef B2Y_CASE
     // weight-multicast clusters exist for the wide, deep tiles only (KBYTES = 128)
-    if (p.pair) {
-        if (kbytes == 128 && block_n == 128 && cluster == 2) return launch_cfg<128, 128, KIND, 2, 1>(a, b, c, p, st);
-        if (kbytes == 128 && block_n == 256 && cluster == 2) return launch_cfg<256, 128, KIND, 2, 1>(a, b, c, p, st);
-        return B2Y_ERR_UNSUPPORTED;
-    }
     if (kbytes == 128 && block_n == 128 && cluster == 2) return launch_cfg<128, 128, KIND, 2>(a, b, c, p, st);
-    if (kbytes == 128 && block_n == 256 && cluster == 2) return launch_cfg<256, 128, KIND, 2>(a, b, c, p, st);
-    if (kbytes == 128 && block_n == 256 && cluster == 4) return launch_cfg<256, 128, KIND, 4>(a, b, c, p, st);
     return B2Y_ERR_UNSUPPORTED;
 }
 
-// cluster size for a launch: B2Y_CLUSTER env (1 = off, 2 default, 4) when the tile shape supports multicast and
-// there is more than one M tile per cluster to share the weights across
+// cluster size for a launch: B2Y_CLUSTER env (1 = off, 2 default) when the tile shape supports multicast and there is
+// more than one M tile per cluster to share the weights across
 static int pick_cluster(int block_n, int kbytes, int num_m_tiles) {
     static int want = -1;
     if (want < 0) {
         const char* e = getenv("B2Y_CLUSTER");
-        want = e ? atoi(e) : 2;
-        if (want != 1 && want != 2 && want != 4) want = 2;
+        want = (e && atoi(e) == 1) ? 1 : 2;
     }
     if (kbytes != 128 || block_n < 128) return 1;
-    int c = want;
-    if (c == 4 && block_n != 256) c = 2;
-    if (num_m_tiles < 2 * c) return 1;
-    return c;
+    if (num_m_tiles < 2 * want) return 1;
+    return want;
 }
 
 struct EpilogueArgs {
@@ -211,7 +212,7 @@ struct GemmConvSpec {
     int ntaps = 1;
     unsigned char tap_ow[16] = {0}, tap_oh[16] = {0};
     bool pointwise = false;      // plain GEMM over [N*H*W][C] (2-D tiled TMA)
-    bool a_bf16 = false, b_bf16 = false;   // 16-bit operand formats of the kind::f16 MMA
+    bool a_bf16 = false, b_bf16 = false;   // 16-bit operand formats (wgmma: both the same)
     const void* w = nullptr;
     int Nout = 0;
     int out_identity = 1, out_OH = 0, out_OW = 0, out_ys = 1, out_xs = 1, out_y0 = 0, out_x0 = 0;
@@ -229,7 +230,10 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
     if ((reinterpret_cast<uintptr_t>(g.a) & 15) || (reinterpret_cast<uintptr_t>(g.w) & 15)) return B2Y_ERR_INVALID;
     const long long M = (long long)g.N * g.MH * g.MW;
     if (M <= 0 || M > 0x7fffff00LL) return B2Y_ERR_UNSUPPORTED;
-    const int block_n = g.Nout <= 32 ? 32 : (g.Nout <= 64 ? 64 : (g.Nout <= 128 ? 128 : 256));
+    if (g.kind == CONV_KIND_F16 && g.a_bf16 != g.b_bf16) return B2Y_ERR_UNSUPPORTED;
+    // N tiles of at most 128 columns: a 128 x 128 fp32 accumulator is 64 registers per thread of the two consumer
+    // warpgroups and 64 KB of epilogue staging, which leaves room for a 4-deep ring of 32 KB k-step stages
+    const int block_n = g.Nout <= 32 ? 32 : (g.Nout <= 64 ? 64 : 128);
     const int block_k = kbytes / esize;
 
     ConvTcParams p{};
@@ -265,7 +269,7 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
     p.slope = e.slope;
     p.acc_scale = e.acc_scale;
     p.acc_scale_ptr = e.acc_scale_ptr;
-    p.idesc_ab = (g.a_bf16 ? (1u << 7) : 0u) | (g.b_bf16 ? (1u << 10) : 0u);
+    p.ab_bf16 = g.a_bf16 ? 1 : 0;
     p.res_bf16 = e.res_bf16;
     p.res = reinterpret_cast<const __half*>(e.res);
     p.res_pitch = e.res_pitch;
@@ -277,8 +281,12 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
     p.out_fakequant = e.out_fakequant;
     p.q_lo = e.q_lo;
     p.q_hi = e.q_hi;
-    p.stat_sum = e.stat_sum;
-    p.stat_sqsum = e.stat_sqsum;
+    p.stat_acc = nullptr;
+    if (e.stat_sum != nullptr) {
+        if (e.stat_sqsum == nullptr || g.Nout > CONV_STAT_MAX) return B2Y_ERR_UNSUPPORTED;
+        p.stat_acc = stream_acc(st, 2 * CONV_STAT_MAX);
+        if (p.stat_acc == nullptr) return B2Y_ERR_CUDA;
+    }
     static int tma_on = -1;      // B2Y_EPI_TMA=0: direct 16-byte stores from registers instead of smem + TMA
     if (tma_on < 0) {
         const char* ev = getenv("B2Y_EPI_TMA");
@@ -374,17 +382,11 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
             const char* m = getenv("B2Y_BRES_MIN_STAGES");
             if (m && atoi(m) >= 2) bres_min = atoi(m);
         }
-        const long long max_smem = 192 * 1024;
+        const long long max_smem = conv_max_stage_smem(block_n);
         const long long a_bytes = 128LL * kbytes, b_bytes = (long long)block_n * kbytes;
         const long long res_bytes = (long long)p.ntaps * p.k_chunks * b_bytes;
-        static int pair_on = -1;     // B2Y_PAIR=0: clusters of two use weight multicast instead of cta_group::2 MMA
-        if (pair_on < 0) {
-            const char* e = getenv("B2Y_PAIR");
-            pair_on = (e && atoi(e) == 0) ? 0 : 1;
-        }
-        p.pair = (cluster == 2 && pair_on) ? 1 : 0;
         p.b_resident = 0;
-        long long ns = max_smem / (a_bytes + (p.pair ? b_bytes / 2 : b_bytes));
+        long long ns = max_smem / (a_bytes + b_bytes);
         if (bres_on && cluster == 1 && p.num_n_tiles == 1 && p.num_m_tiles > g_num_sms &&
             res_bytes + bres_min * a_bytes <= max_smem) {
             p.b_resident = 1;
@@ -402,8 +404,12 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
         if (rc != B2Y_OK) return rc;
         p.epi_tma = 1;
     }
-    if (g.kind == CONV_KIND_F16) return dispatch<CONV_KIND_F16>(block_n, kbytes, cluster, tmA, tmB, tmC, p, st);
-    return dispatch<CONV_KIND_I8>(block_n, kbytes, cluster, tmA, tmB, tmC, p, st);
+    rc = g.kind == CONV_KIND_F16 ? dispatch<CONV_KIND_F16>(block_n, kbytes, cluster, tmA, tmB, tmC, p, st)
+                                 : dispatch<CONV_KIND_I8>(block_n, kbytes, cluster, tmA, tmB, tmC, p, st);
+    if (rc != B2Y_OK || p.stat_acc == nullptr) return rc;
+    B2Y_CUDA_CHECK(launch_pdl(stats_finalize_kernel, dim3((g.Nout + 255) / 256), dim3(256), 0, st, p.stat_acc, g.Nout,
+                              e.stat_sum, e.stat_sqsum));
+    return B2Y_OK;
 }
 
 // Forward convolution: x NHWC (fp16 or int8), w [Cout][R][S][Cin].
@@ -553,7 +559,7 @@ extern "C" int b2y_pack_dgrad_weights(const b2y_conv_desc* d, const float* w_oih
         if (P.nh * P.nw == 0) continue;
         const long long total = (long long)d->in_c * P.nh * P.nw * d->out_c;
         int grid = (int)((total + 255) / 256);
-        if (grid > 148 * 16) grid = 148 * 16;
+        if (grid > 132 * 16) grid = 132 * 16;
         if (grad_dtype == B2Y_DT_BF16)
             pack_dgrad_kernel<__nv_bfloat16><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
                 w_oihw, reinterpret_cast<__nv_bfloat16*>(w_packed_t) + P.w_offset, d->out_c, d->in_c, d->ksize, P.nh,
@@ -570,8 +576,8 @@ extern "C" int b2y_pack_dgrad_weights(const b2y_conv_desc* d, const float* w_oih
 extern "C" int b2y_conv2d_bwd_data(const b2y_conv_desc* d, const void* dy, const void* w_packed_t, void* dx,
                                    int accumulate, int operand_dtype, int out_dtype, const float* inv_scale_ptr,
                                    void* stream) {
-    const bool gbf = operand_dtype == B2Y_DT_BF16;     // dY and the packed weights (must match: tcgen05 kind::f16
-                                                       // raises an illegal-instruction fault for mixed f16/bf16)
+    const bool gbf = operand_dtype == B2Y_DT_BF16;     // dY and the packed weights (must match: wgmma takes one
+                                                       // 16-bit format for both operands)
     const bool obf = out_dtype == B2Y_DT_BF16;         // dX (and the accumulate source)
     if (!d || !dy || !w_packed_t || !dx) return B2Y_ERR_INVALID;
     if (d->stride > 4) return B2Y_ERR_UNSUPPORTED;
@@ -638,7 +644,7 @@ extern "C" int b2y_conv2d_bwd_data(const b2y_conv_desc* d, const void* dy, const
 // ---- tensor-core stem ------------------------------------------------------------------------------------------
 // The image (NCHW fp32, Cin <= 4) is first re-laid as NHWC fp16 with the kw taps unrolled into the channel dim:
 //   packed[n][y][x][kw*Cin + c] = x[n][c][y][x + kw - pad]   (16 "channels", zero padded)
-// so that the conv becomes a k x 1 implicit GEMM with K = 16 per tap row on the same tcgen05 kernel.
+// so that the conv becomes a k x 1 implicit GEMM with K = 16 per tap row on the same wgmma kernel.
 template <int CIN, int K>
 __global__ void stem_pack_kernel(const float* __restrict__ x, __half* __restrict__ out, int B, int H, int W,
                                  int pad) {
@@ -783,7 +789,7 @@ extern "C" int b2y_stem_conv_fwd_tc(const b2y_conv_desc* d, const float* x_nchw,
     if (stem_is_full(d->in_c, d->ksize)) {
         const long long opix = (long long)d->batch * Ho * Wo;
         int fgrid = (int)((opix + 127) / 128);
-        if (fgrid > 148 * 64) fgrid = 148 * 64;
+        if (fgrid > 132 * 64) fgrid = 132 * 64;
         __half* fws = reinterpret_cast<__half*>(workspace);
 #define B2Y_STEM_FULL(CI, KK)                                                                                       \
     if (d->in_c == CI && d->ksize == KK) {                                                                          \
@@ -822,7 +828,7 @@ extern "C" int b2y_stem_conv_fwd_tc(const b2y_conv_desc* d, const float* x_nchw,
     if (d->in_c * d->ksize > 16 || d->ksize > 16) return B2Y_ERR_UNSUPPORTED;
     const long long pixels = (long long)d->batch * d->in_h * d->in_w;
     int grid = (int)((pixels + 255) / 256);
-    if (grid > 148 * 32) grid = 148 * 32;
+    if (grid > 132 * 32) grid = 132 * 32;
     __half* ws = reinterpret_cast<__half*>(workspace);
 #define B2Y_STEM_PACK(CI, KK)                                                                             \
     if (d->in_c == CI && d->ksize == KK) {                                                                \

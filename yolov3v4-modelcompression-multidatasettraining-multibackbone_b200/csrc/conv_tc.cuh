@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution, sm_100a.
+// wgmma implicit-GEMM convolution, sm_90a.
 //
 //   D[M = B*Ho*Wo pixels][N = Cout] = sum_{tap (r,s)} sum_{c} A_tap[M][c] * W[N][(r,s,c)]
 //
@@ -6,11 +6,13 @@
 //   (tap, 64-channel) slab straight from the NHWC tensor in im2col mode (zero fill for the
 //   padding halo, traversal stride = conv stride) into a 128B-swizzled K-major smem tile.
 // * B (weights, [Cout][R][S][Cin]) comes in through a tiled 2-D TMA map.
-// * One elected thread issues tcgen05.mma (M=128, N=BLOCK_N, K=32 bytes) with the fp32/int32
-//   accumulator in TMEM, double-buffered so the epilogue of tile i overlaps the MMAs of tile i+1.
-// * Persistent grid (<= #SMs CTAs), warp-specialised: warp0 = TMA producer, warp1 = MMA issuer,
-//   warp2 = TMEM allocator, warps 4-11 = epilogue (TMEM -> regs -> bias/act/residual -> global).
+// * Two consumer warpgroups issue wgmma.mma_async (M=64 rows each, N=BLOCK_N, K=32 bytes) with the fp32/int32
+//   accumulator in registers, then stage it through shared memory for the row-per-thread epilogue.
+// * Persistent grid (<= #SMs CTAs), warp-specialised: warp0 = TMA producer (runs up to num_stages k-steps ahead,
+//   across tile boundaries), warps 4-11 = MMA + epilogue (bias/act/residual/statistics -> global).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b2y {
@@ -18,6 +20,7 @@ namespace b2y {
 enum { CONV_KIND_F16 = 0, CONV_KIND_I8 = 1 };
 enum { A_MODE_IM2COL = 0, A_MODE_TILED2D = 1 };
 enum { OUT_F16 = 0, OUT_F32 = 1, OUT_I8 = 2, OUT_BF16 = 3 };
+constexpr int CONV_STAT_MAX = 4096;   // channels of a convolution that accumulates batch statistics
 
 struct ConvTcParams {
     int M_total;      // B*Ho*Wo
@@ -44,7 +47,7 @@ struct ConvTcParams {
     float slope;
     float acc_scale;        // multiplies the accumulator (1 for fp16; s_a*s_w for int8)
     const float* acc_scale_ptr;  // optional device scalar multiplied in as well (per-layer gradient un-scaling)
-    unsigned idesc_ab;      // a_format<<7 | b_format<<10 for kind::f16 (0 = f16, 1 = bf16 per operand)
+    int ab_bf16;            // 16-bit operands are bf16 (both: wgmma takes one format for A and B)
     int res_bf16;           // residual / accumulate tensor is bf16 instead of fp16
     const __half* res;      // optional residual (16-bit, NHWC) added after the activation
     long long res_pitch;    // elements per pixel row
@@ -55,12 +58,13 @@ struct ConvTcParams {
     float out_scale;        //              (and v_dequant = q * out_scale when out is fp16/fp32 fake-quant)
     int out_fakequant;      // 1: write the dequantised value q*out_scale in out_dtype (fp16/fp32)
     float q_lo, q_hi;       // clamp range, e.g. -128, 127
-    // training extras: per-channel sum / sum of squares of the raw (pre-bias) output, fp32 atomics
-    float* stat_sum;
-    float* stat_sqsum;
+    // training extras: per-channel sum / sum of squares of the raw (pre-bias) output, accumulated in double
+    // ([0, CONV_STAT_MAX) sums, [CONV_STAT_MAX, 2 CONV_STAT_MAX) squares) so that the result does not depend on the order
+    // of the atomics: the variance is E[z^2] - E[z]^2, and that cancellation magnifies fp32 ordering noise, which
+    // batch-statistics BatchNorm then carries through every later layer
+    double* stat_acc;
     int b_resident;         // 1: the whole weight panel of the (single) N tile stays in smem, loaded once per CTA
     int num_stages;         // smem ring depth for this launch (<= 32)
-    int pair;               // host: launch the cta_group::2 variant (cluster of two)
     int epi_tma;            // the short epilogue stores through smem + TMA (tmC valid); rows / columns clipped by the map
     int epi_fast;           // host-checked: 16-bit out, whole channel tiles, 16-byte aligned bias/residual/output
     // int8 graph: quantised shortcut folded into the epilogue (COSPTQuantizedShortcut eval, ptq_cos.py:876-884 / 931-933):
@@ -73,24 +77,24 @@ struct ConvTcParams {
     float qs_cx, qs_ca;     // out_scale / scale_sum, a_in / scale_sum
 };
 
+// Opt-in shared memory per block on sm_90 (227 KB); the ring of k-step stages takes what the epilogue leaves.
+constexpr int CONV_SMEM_LIMIT = 227 * 1024;
+constexpr int conv_max_stage_smem(int block_n) {
+    return ((CONV_SMEM_LIMIT - 1024 - 1024 - 8 * 4096 - 128 * block_n * 4) / 1024) * 1024;
+}
+
 template <int BLOCK_N, int KBYTES>
 struct ConvTcCfg {
     static constexpr int BLOCK_M = 128;
     static constexpr int A_BYTES = BLOCK_M * KBYTES;
     static constexpr int B_BYTES = BLOCK_N * KBYTES;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // always a multiple of 1024
-    static constexpr int MAX_STAGE_SMEM = 192 * 1024;
-    static constexpr int NUM_STAGES_RAW = MAX_STAGE_SMEM / STAGE_BYTES;
-    // small-K layers have small stages: keep up to 32 of them in flight so that enough bytes are outstanding per SM
-    // to cover HBM latency (Little's law: 148 SMs x ~190 KB / ~2 us)
-    static constexpr int NUM_STAGES = NUM_STAGES_RAW > 32 ? 32 : NUM_STAGES_RAW;
-    // accumulator ring in TMEM: narrow tiles get a deeper ring so the MMA warp can run several tiles ahead of
-    // the (latency-bound) epilogue; 256-wide tiles use the whole 512-column TMEM with 2 stages
-    static constexpr int ACC_STAGES = BLOCK_N >= 256 ? 2 : (BLOCK_N == 128 ? 4 : 8);
-    static constexpr int TMEM_COLS = ACC_STAGES * BLOCK_N;   // 512, 512, 512, 256 columns
-    static constexpr int AUX_BYTES = 1024;  // barriers + tmem ptr, at a fixed offset behind the tile area
+    static constexpr int MAX_STAGE_SMEM = conv_max_stage_smem(BLOCK_N);
+    static constexpr int AUX_BYTES = 1024;  // barriers, at a fixed offset behind the tile area
     static constexpr int EPI_STAGE_BYTES = 8 * 4096;   // per epilogue warp: 2 x 2 KB output staging for TMA stores
-    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + MAX_STAGE_SMEM + AUX_BYTES + EPI_STAGE_BYTES;
+    static constexpr int ACC_BYTES = BLOCK_M * BLOCK_N * 4;   // fp32 / int32 accumulator tile between MMA and epilogue
+    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + MAX_STAGE_SMEM + AUX_BYTES + EPI_STAGE_BYTES + ACC_BYTES;
+    static_assert(SMEM_BYTES <= CONV_SMEM_LIMIT, "shared memory");
 };
 
 __device__ __noinline__ float mish_noinline(float x) { return mish_f(x); }
@@ -114,14 +118,10 @@ __device__ __forceinline__ uint32_t pack_i8x4(float a, float b, float c, float d
     return __byte_perm(__byte_perm(ua, ub, 0x0040), __byte_perm(uc, ud, 0x0040), 0x5410);
 }
 
-template <int BLOCK_N>
 struct ConvTcEpi {
-    // 8 epilogue warps (two groups of 4, one warp per TMEM lane quarter each):
-    //   wide tiles  (BLOCK_N >= 128): both groups work on the same tile, half of the columns each;
-    //   narrow tiles (BLOCK_N < 128): the groups take alternate tiles, so two accumulators drain concurrently.
+    // two consumer warpgroups (warps 4-11): each issues the MMAs of 64 of the 128 tile rows; in the epilogue warp w
+    // takes rows 32 (w % 4) .. + 31 (thread = row) and every other 32-column chunk (w / 4 = chunk parity)
     static constexpr int WARPS = 8;
-    static constexpr bool SPLIT_TILES = BLOCK_N < 128;
-    static constexpr int ARRIVALS = SPLIT_TILES ? 4 : 8;    // epilogue warps that release one accumulator stage
     static constexpr int THREADS = 128 + 32 * WARPS;
 };
 
@@ -132,7 +132,7 @@ __device__ __forceinline__ void epi_chunk_general(float (&v)[32], const ConvTcPa
                                                bool row_ok, int lane, uint8_t* stage, bool defer_stats, float& ds1,
                                                float& ds2) {
     ds1 = ds2 = 0.f;
-    if (p.stat_sum != nullptr) {
+    if (p.stat_acc != nullptr) {
         // per-channel batch statistics of the raw conv output (training BN): the warp's 32x32 chunk goes through its smem
         // staging tile (rotated columns: conflict-free both ways), then lane j sums column j -- 32 STS + 32 LDS instead of
         // 640 shuffles per chunk
@@ -152,8 +152,8 @@ __device__ __forceinline__ void epi_chunk_general(float (&v)[32], const ConvTcPa
             ds1 = s1;
             ds2 = s2;
         } else if (n0c0 + lane < p.Cout) {
-            atomicAdd(p.stat_sum + n0c0 + lane, s1);
-            atomicAdd(p.stat_sqsum + n0c0 + lane, s2);
+            atomicAdd(p.stat_acc + n0c0 + lane, (double)s1);
+            atomicAdd(p.stat_acc + CONV_STAT_MAX + n0c0 + lane, (double)s2);
         }
     }
     const int nvalid = min(32, p.Cout - n0c0);
@@ -273,43 +273,31 @@ __device__ __forceinline__ void epi_chunk_general(float (&v)[32], const ConvTcPa
 }
 
 // CLUSTER > 1: the CTAs of a cluster work on CLUSTER consecutive M tiles of the same N tile; each loads 1/CLUSTER of
-// the weight tile and TMA-multicasts it to all of them, so the weight re-reads from L2 drop by CLUSTER x.
-//
-// PAIR (CLUSTER == 2): the two CTAs of the cluster are one cta_group::2 MMA pair.  Each CTA loads its own 128-row A tile
-// and HALF of the weight tile; the leader CTA issues one M=256 tcgen05.mma per k-slice that reads both halves, each
-// CTA's TMEM receives its own 128 accumulator rows.  Per CTA the smem fill per k-step drops from A + B to A + B/2,
-// which is what bounds the wide layers (L2 -> SM bandwidth), with no extra instructions on the critical loops.
-template <int BLOCK_N, int KBYTES, int KIND, int CLUSTER, int PAIR = 0>
-__global__ void __launch_bounds__(ConvTcEpi<BLOCK_N>::THREADS, 1)
+// the weight tile and TMA-multicasts it to all of them, so the weight re-reads from L2 drop by CLUSTER x.  A stage is
+// free again once the consumer warps of every CTA of the cluster have released it.
+template <int BLOCK_N, int KBYTES, int KIND, int CLUSTER>
+__global__ void __launch_bounds__(ConvTcEpi::THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ ConvTcParams p) {
     using Cfg = ConvTcCfg<BLOCK_N, KBYTES>;
-    using Epi = ConvTcEpi<BLOCK_N>;
     constexpr int MAX_NS = 32;
     constexpr int ESIZE = (KIND == CONV_KIND_F16) ? 2 : 1;
     constexpr int BLOCK_K = KBYTES / ESIZE;  // elements per k-chunk
     constexpr uint32_t LAYOUT = swizzle_layout_type(KBYTES);
-    constexpr uint32_t IDESC = (KIND == CONV_KIND_F16)
-                                   ? make_idesc(/*c=F32*/ 1, /*a=F16*/ 0, /*b=F16*/ 0, 0, 0, PAIR ? 256 : 128, BLOCK_N)
-                                   : make_idesc(/*c=S32*/ 2, /*a=S8*/ 1, /*b=S8*/ 1, 0, 0, PAIR ? 256 : 128, BLOCK_N);
-    static_assert(!PAIR || CLUSTER == 2, "a CTA pair is a cluster of two");
+    using AccT = typename std::conditional<KIND == CONV_KIND_F16, float, uint32_t>::type;
 
-    // smem: [ns stages of A (+B)] [resident weight panel, if any] ... [aux at a fixed offset]
+    // smem: [ns stages of A (+B)] [resident weight panel, if any] ... [aux] [epilogue staging] [accumulator tile]
     const bool b_res = CLUSTER == 1 && p.b_resident != 0;
     const int ns = p.num_stages;
-    const uint32_t stage_bytes = b_res ? (uint32_t)Cfg::A_BYTES
-                                       : (PAIR ? (uint32_t)(Cfg::A_BYTES + Cfg::B_BYTES / 2) : (uint32_t)Cfg::STAGE_BYTES);
+    const uint32_t stage_bytes = b_res ? (uint32_t)Cfg::A_BYTES : (uint32_t)Cfg::STAGE_BYTES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* aux = smem + Cfg::MAX_STAGE_SMEM;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);           // [MAX_NS]
     uint64_t* empty_bar = full_bar + MAX_NS;                         // [MAX_NS]
-    constexpr int AS = Cfg::ACC_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + MAX_NS;                    // [AS]
-    uint64_t* tmem_empty_bar = tmem_full_bar + AS;                   // [AS]
-    uint64_t* bres_bar = tmem_empty_bar + AS;                        // [1] resident weight panel landed
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bres_bar + 1);
+    uint64_t* bres_bar = empty_bar + MAX_NS;                         // [1] resident weight panel landed
     uint8_t* epi_stage = aux + Cfg::AUX_BYTES;                       // [8 warps][4096] output staging for TMA stores
+    uint8_t* acc_stage = epi_stage + Cfg::EPI_STAGE_BYTES;           // [128][BLOCK_N] accumulators
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -322,29 +310,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (warp == 1 && lane == 0) {
         for (int i = 0; i < ns; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], PAIR ? 1 : CLUSTER);   // multicast: every CTA that writes this stage releases it
+            mbar_init(&empty_bar[i], ConvTcEpi::WARPS * CLUSTER);   // every consumer warp of every CTA that reads it
         }
         mbar_init(bres_bar, 1);
-        for (int i = 0; i < AS; ++i) {
-            mbar_init(&tmem_full_bar[i], 1);
-            mbar_init(&tmem_empty_bar[i], PAIR ? 2 * Epi::ARRIVALS : Epi::ARRIVALS);   // pair: both CTAs' epilogues
-        }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        if (PAIR) {
-            tmem_alloc2(tmem_ptr_smem, Cfg::TMEM_COLS);
-            tmem_relinquish2();
-        } else {
-            tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-            tmem_relinquish();
-        }
-    }
-    tc_fence_before();
     __syncthreads();
     if (CLUSTER > 1) cluster_sync_all();   // barriers of every CTA are initialised before any remote arrive / multicast
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
     // work items: (group of CLUSTER consecutive M tiles, N tile); this CTA takes M tile group*CLUSTER + rank.
     // A "ghost" M tile past the end still runs the pipeline (TMA zero fill) but stores nothing.
@@ -362,10 +334,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t empty_base = smem_u32(empty_bar);
     const uint32_t bres_base = smem_base + (uint32_t)ns * stage_bytes;     // resident weight panel (k_steps x B tile)
 
-    // The two issue loops below are executed by the whole (converged) warp with one elected lane doing the issue:
-    // all loop state is then warp-uniform and lives in the uniform datapath.  (Run by a single divergent lane, each
-    // TMA / MMA issue cost ~10 extra R2UR/ELECT instructions and the loops, at ~8 cycles per dependent instruction,
-    // became the bottleneck of every layer whose k-step is shorter than ~800 cycles.)
+    // The issue loop is executed by the whole (converged) warp with one elected lane doing the issue: all loop state is
+    // then warp-uniform and lives in the uniform datapath.
     if (warp == 0) {
         // ===================== TMA producer =====================
         uint32_t stage = 0, phase = 0;
@@ -382,7 +352,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 tma_load_2d_s(bres_base + ks * Cfg::B_BYTES, &tmB, smem_u32(bres_bar), ks * BLOCK_K, 0);
         }
         __syncwarp();
-        // everything above (barriers, TMEM, the static weights) may overlap the tail of the previous layer's kernel;
+        // everything above (barriers, the static weights) may overlap the tail of the previous layer's kernel;
         // activations must not be touched before it has completed (programmatic dependent launch)
         pdl_wait();
         pdl_launch_dependents();
@@ -410,16 +380,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         const uint32_t a_dst = smem_base + stage * stage_bytes;
                         const uint32_t b_dst = a_dst + Cfg::A_BYTES;
                         const uint32_t fb = full_base + stage * 8;
-                        if (PAIR) {
-                            // all four loads of the pair complete on the leader's barrier, which expects both CTAs' bytes
-                            if (cta_rank == 0) mbar_expect_tx_s(fb, 2 * stage_bytes);
-                            const uint32_t lb = mapa_u32(fb, 0);
-                            if (im2col)
-                                tma2_load_im2col_4d(a_dst, &tmA, lb, a_c, base_w, base_h, img, s, r);
-                            else
-                                tma2_load_2d(a_dst, &tmA, lb, a_c, m0);
-                            tma2_load_2d(b_dst, &tmB, lb, b_k, b_row);
-                        } else {
                         mbar_expect_tx_s(fb, stage_bytes);
                         if (im2col)
                             tma_load_im2col_4d_s(a_dst, &tmA, fb, a_c, base_w, base_h, img, s, r);
@@ -430,7 +390,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                                                     MC_MASK);
                         else if (!b_res)
                             tma_load_2d_s(b_dst, &tmB, fb, b_k, b_row);
-                        }
                     }
                     a_c += BLOCK_K;
                     b_k += BLOCK_K;
@@ -442,100 +401,93 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 b_k += Cin - k_chunks * BLOCK_K;   // == 0 (Cin is a whole number of chunks); keeps the intent explicit
             }
         }
-    } else if (warp == 1 && (!PAIR || cta_rank == 0)) {
-        // ===================== MMA issuer (pair: the leader CTA issues for both) =====================
-        uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
+    } else if (warp >= 4) {
+        // ===================== MMA (two warpgroups, 64 rows each) + epilogue =====================
+        const int wg = (warp - 4) >> 2;
+        const int tid_wg = (int)threadIdx.x & 127;
         const int k_steps = taps * k_chunks;
-        const uint32_t idesc = IDESC | (KIND == CONV_KIND_F16 ? p.idesc_ab : 0u);
         const uint64_t desc_base = smem_desc_base(16, 8 * KBYTES, LAYOUT);
-        const uint32_t tfull_base = smem_u32(tmem_full_bar), tempty_base = smem_u32(tmem_empty_bar);
-        if (b_res) {
-            mbar_wait_s(smem_u32(bres_bar), 0);
-            tc_fence_after();
-        }
+        const bool ab_bf16 = p.ab_bf16 != 0;
+        uint32_t stage = 0, phase = 0;
+        pdl_wait();
+        const float acc_mul = p.acc_scale * (p.acc_scale_ptr != nullptr ? __ldg(p.acc_scale_ptr) : 1.f);
+        const int ew = (warp - 4) & 3;          // row quarter of the tile
+        const int cg = (warp - 4) >> 2;         // chunk parity
+        const bool fast = p.epi_fast != 0;
+        const int act = p.act;
+        const float slope = p.slope;
+        const int hw = p.MH * p.MW;
+        const bool epi_tma = p.epi_tma != 0;
+        uint8_t* my_stage = epi_stage + (warp - 4) * 4096;
+        const int trow = ew * 32 + lane;        // this thread's row of the tile in the epilogue
+        int sbuf = 0;
+        // training BN statistics: with a single N tile every tile of this warp covers the same columns, so the channel
+        // sums are kept in registers (lane j = column j of chunk q) and flushed with ONE atomic per column per warp at the
+        // end -- instead of one per column per 32-row chunk (millions of same-address L2 atomics on the large early layers)
+        const bool defer_stats = p.stat_acc != nullptr && num_n_tiles == 1;
+        float st1[2] = {0.f, 0.f}, st2[2] = {0.f, 0.f};
+        if (b_res) mbar_wait_s(smem_u32(bres_bar), 0);
         for (int item = cluster_id; item < num_items; item += num_clusters) {
-            mbar_wait_s(tempty_base + acc * 8, acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-            uint32_t accum = 0;
+            const int mgroup = item / num_n_tiles;
+            const int n_tile = item - mgroup * num_n_tiles;
+            const int m_tile = mgroup * CLUSTER + cta_rank;
+            const int n0 = n_tile * BLOCK_N;
+
+            AccT acc[BLOCK_N / 2];
+            uint32_t prev = 0;
             for (int ks = 0; ks < k_steps; ++ks) {
                 mbar_wait_s(full_base + stage * 8, phase);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t a_addr = smem_base + stage * stage_bytes;
-                    const uint32_t b_addr = b_res ? bres_base + ks * Cfg::B_BYTES : a_addr + Cfg::A_BYTES;
-                    const uint64_t adesc = desc_base | (uint64_t)((a_addr >> 4) & 0x3FFF);
-                    const uint64_t bdesc = desc_base | (uint64_t)((b_addr >> 4) & 0x3FFF);
+                const uint32_t a_tile = smem_base + stage * stage_bytes;
+                const uint32_t a_addr = a_tile + (uint32_t)(wg * 64 * KBYTES);
+                const uint32_t b_addr = b_res ? bres_base + ks * Cfg::B_BYTES : a_tile + Cfg::A_BYTES;
+                const uint64_t adesc = desc_base | (uint64_t)((a_addr >> 4) & 0x3FFF);
+                const uint64_t bdesc = desc_base | (uint64_t)((b_addr >> 4) & 0x3FFF);
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < KBYTES / 32; ++k) {
-                        if (PAIR) {
-                            if (KIND == CONV_KIND_F16)
-                                mma2_f16_ss(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc,
-                                            k > 0 ? 1u : accum);
-                            else
-                                mma2_i8_ss(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc,
-                                           k > 0 ? 1u : accum);
-                        } else if (KIND == CONV_KIND_F16)
-                            mma_f16_ss(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc,
-                                       k > 0 ? 1u : accum);
-                        else
-                            mma_i8_ss(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc,
-                                      k > 0 ? 1u : accum);
-                    }
-                    if (PAIR)
-                        tc_commit2_multicast_s(empty_base + stage * 8, MC_MASK);   // frees the slot in both CTAs
-                    else if (CLUSTER > 1)
-                        tc_commit_multicast_s(empty_base + stage * 8, MC_MASK);  // release the slot in every CTA
+                for (int k = 0; k < KBYTES / 32; ++k) {
+                    const uint32_t sc = (ks > 0 || k > 0) ? 1u : 0u;
+                    if constexpr (KIND == CONV_KIND_I8)
+                        wgmma_ss<BLOCK_N, 2, 0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), sc);
+                    else if (ab_bf16)
+                        wgmma_ss<BLOCK_N, 1, 0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), sc);
                     else
-                        tc_commit_s(empty_base + stage * 8);  // frees the smem slot when these MMAs retire
+                        wgmma_ss<BLOCK_N, 0, 0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), sc);
                 }
-                accum = 1;
+                wgmma_commit();
+                if (ks > 0) {
+                    // the MMAs of the previous k-step have retired: its smem slot goes back to the producer(s)
+                    wgmma_wait<1>();
+                    if (lane == 0) {
+                        if (CLUSTER == 1) {
+                            mbar_arrive(&empty_bar[prev]);
+                        } else {
+#pragma unroll
+                            for (int r = 0; r < CLUSTER; ++r) mbar_arrive_cluster(mapa_u32(empty_base + prev * 8, r));
+                        }
+                    }
+                }
+                prev = stage;
                 if (++stage == (uint32_t)ns) {
                     stage = 0;
                     phase ^= 1;
                 }
             }
-            if (elect_one()) {   // accumulator complete -> epilogue (of both CTAs for a pair)
-                if (PAIR)
-                    tc_commit2_multicast_s(tfull_base + acc * 8, MC_MASK);
-                else
-                    tc_commit_s(tfull_base + acc * 8);
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            if (lane == 0) {
+                if (CLUSTER == 1) {
+                    mbar_arrive(&empty_bar[prev]);
+                } else {
+#pragma unroll
+                    for (int r = 0; r < CLUSTER; ++r) mbar_arrive_cluster(mapa_u32(empty_base + prev * 8, r));
+                }
             }
-            if (++acc == AS) {
-                acc = 0;
-                acc_phase ^= 1;
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        constexpr int COLS_PER_GROUP = Epi::SPLIT_TILES ? BLOCK_N : BLOCK_N / 2;
-        pdl_wait();
-        const float acc_mul = p.acc_scale * (p.acc_scale_ptr != nullptr ? __ldg(p.acc_scale_ptr) : 1.f);
-        const int ew = (warp - 4) & 3;          // TMEM lane quarter == warp_id % 4
-        const int cg = (warp - 4) >> 2;         // group
-        const bool fast = p.epi_fast != 0;
-        const int act = p.act;
-        const float slope = p.slope;
-        const int c_begin = Epi::SPLIT_TILES ? 0 : cg * COLS_PER_GROUP;
-        const int hw = p.MH * p.MW;
-        const bool epi_tma = p.epi_tma != 0;
-        uint8_t* my_stage = epi_stage + (warp - 4) * 4096;
-        int sbuf = 0;
-        int it = 0;
-        // training BN statistics: with a single N tile every tile of this warp covers the same columns, so the channel
-        // sums are kept in registers (lane j = column j of chunk q) and flushed with ONE atomic per column per warp at the
-        // end -- instead of one per column per 32-row chunk (millions of same-address L2 atomics on the large early layers)
-        const bool defer_stats = p.stat_sum != nullptr && num_n_tiles == 1;
-        float st1[4] = {0.f, 0.f, 0.f, 0.f}, st2[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int item = cluster_id; item < num_items; item += num_clusters, ++it) {
-            if (Epi::SPLIT_TILES && (it & 1) != cg) continue;
-            const int acc = it % AS;
-            const uint32_t acc_phase = (uint32_t)(it / AS) & 1u;
-            const int mgroup = item / num_n_tiles;
-            const int n_tile = item - mgroup * num_n_tiles;
-            const int m_tile = mgroup * CLUSTER + cta_rank;
-            const int n0 = n_tile * BLOCK_N;
-            const long long grow = (long long)m_tile * 128 + ew * 32 + lane;   // GEMM row
+            // accumulators -> smem (after every epilogue thread is done with the previous tile's)
+            named_bar_sync(1, 256);
+            frag_to_stage<BLOCK_N>(acc, acc_stage, wg * 64, tid_wg);
+            named_bar_sync(1, 256);
+
+            const long long grow = (long long)m_tile * 128 + trow;              // GEMM row
             const bool row_ok = grow < p.M_total;
             long long row = grow;                                              // output pixel index
             if (!p.out_identity && row_ok) {
@@ -545,56 +497,29 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 row = ((long long)n_ * p.out_OH + (long long)p_ * p.out_ys + p.out_y0) * p.out_OW +
                       (long long)q_ * p.out_xs + p.out_x0;
             }
-            const uint32_t taddr_row = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * BLOCK_N);
 
-            if (fast) {
-                // short path: 16-bit output (or fp32 through TMA), vector-aligned bias / residual / output (checked on the host);
-                // a clipped last N tile is allowed on TMA-store launches
-                const float* bias_p = p.bias != nullptr ? p.bias + n0 + c_begin : nullptr;
-                const uint4* res_p = (p.res != nullptr && row_ok)
-                                         ? reinterpret_cast<const uint4*>(p.res + row * p.res_pitch + n0 + c_begin)
-                                         : nullptr;
-                uint4* out_p = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.out) + row * p.out_pitch + n0 + c_begin);
-                uint4 rnext[4];
-                if (res_p != nullptr) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) rnext[q] = __ldg(res_p + q);
-                }
-                if (p.res != nullptr) {
-                    // pull the residual rows of this warp's NEXT tile into L2 now: by the time its accumulator is ready
-                    // the loads above hit L2 instead of paying HBM latency inside the epilogue
-                    const int nitem = item + (Epi::SPLIT_TILES ? 2 : 1) * num_clusters;
-                    if (nitem < num_items) {
-                        const int nmg = nitem / num_n_tiles;
-                        const int nnt = nitem - nmg * num_n_tiles;
-                        const long long ngrow = (long long)(nmg * CLUSTER + cta_rank) * 128 + ew * 32 + lane;
-                        if (ngrow < p.M_total && p.out_identity) {
-                            const char* np_ = reinterpret_cast<const char*>(p.res + ngrow * p.res_pitch + nnt * BLOCK_N + c_begin);
-#pragma unroll
-                            for (int b = 0; b < COLS_PER_GROUP * 2; b += 128)
-                                asm volatile("prefetch.global.L2 [%0];" ::"l"(np_ + b));
-                        }
-                    }
-                }
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tc_fence_after();
 #pragma unroll 1
-                for (int c = 0; c < COLS_PER_GROUP; c += 32) {
-                    const int cvalid = p.Cout - (n0 + c_begin + c);     // < 32 only in the last chunk of a clipped N tile
+            for (int J = cg; J < BLOCK_N / 32; J += 2) {
+                const int cc = J * 32;                                   // column offset of the chunk in the tile
+                if (fast) {
+                    // short path: 16-bit output (or fp32 through TMA), vector-aligned bias / residual / output (checked on
+                    // the host); a clipped last N tile is allowed on TMA-store launches
+                    const int cvalid = p.Cout - (n0 + cc);               // < 32 only in the last chunk of a clipped tile
                     if (cvalid <= 0) break;                              // (TMA-store launches only; warp-uniform)
                     uint32_t raw[32];
-                    tmem_ld_32x32(taddr_row + (uint32_t)(c_begin + c), raw);
+                    stage_row32<BLOCK_N>(acc_stage, trow, cc, raw);
+                    const float* bias_p = p.bias != nullptr ? p.bias + n0 + cc : nullptr;
                     float4 bv[8];
                     if (bias_p != nullptr && cvalid >= 32) {
 #pragma unroll
-                        for (int q = 0; q < 8; ++q) bv[q] = __ldg(reinterpret_cast<const float4*>(bias_p + c) + q);
+                        for (int q = 0; q < 8; ++q) bv[q] = __ldg(reinterpret_cast<const float4*>(bias_p) + q);
                     } else if (bias_p != nullptr) {
 #pragma unroll
                         for (int q = 0; q < 8; ++q) {
-                            bv[q].x = 4 * q < cvalid ? __ldg(bias_p + c + 4 * q) : 0.f;
-                            bv[q].y = 4 * q + 1 < cvalid ? __ldg(bias_p + c + 4 * q + 1) : 0.f;
-                            bv[q].z = 4 * q + 2 < cvalid ? __ldg(bias_p + c + 4 * q + 2) : 0.f;
-                            bv[q].w = 4 * q + 3 < cvalid ? __ldg(bias_p + c + 4 * q + 3) : 0.f;
+                            bv[q].x = 4 * q < cvalid ? __ldg(bias_p + 4 * q) : 0.f;
+                            bv[q].y = 4 * q + 1 < cvalid ? __ldg(bias_p + 4 * q + 1) : 0.f;
+                            bv[q].z = 4 * q + 2 < cvalid ? __ldg(bias_p + 4 * q + 2) : 0.f;
+                            bv[q].w = 4 * q + 3 < cvalid ? __ldg(bias_p + 4 * q + 3) : 0.f;
                         }
                     } else {
 #pragma unroll
@@ -602,18 +527,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     }
                     uint4 qa[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
                     if (KIND == CONV_KIND_I8 && p.qres != nullptr && row_ok) {
-                        const uint4* ap = reinterpret_cast<const uint4*>(p.qres + row * p.qres_pitch + n0 + c_begin + c);
+                        const uint4* ap = reinterpret_cast<const uint4*>(p.qres + row * p.qres_pitch + n0 + cc);
                         qa[0] = __ldg(ap);
                         qa[1] = __ldg(ap + 1);
                     }
                     uint4 rcur[4];
+                    const bool has_res = p.res != nullptr && row_ok;
+                    if (has_res) {
+                        const uint4* res_p = reinterpret_cast<const uint4*>(p.res + row * p.res_pitch + n0 + cc);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) rcur[q] = rnext[q];
-                    if (res_p != nullptr && c + 32 < COLS_PER_GROUP) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) rnext[q] = __ldg(res_p + (c + 32) / 8 + q);
+                        for (int q = 0; q < 4; ++q) rcur[q] = __ldg(res_p + q);
                     }
-                    tc_wait_ld();
                     float v[32];
 #pragma unroll
                     for (int q = 0; q < 8; ++q) {
@@ -626,7 +550,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         v[4 * q + 2] = fmaf(a2, acc_mul, bv[q].z);
                         v[4 * q + 3] = fmaf(a3, acc_mul, bv[q].w);
                     }
-                    if (KIND == CONV_KIND_F16 && p.stat_sum != nullptr) {
+                    if (KIND == CONV_KIND_F16 && p.stat_acc != nullptr) {
                         // training BN statistics on the short path (host: TMA store, no bias, no residual): column sums of
                         // the warp's 32 x 32 chunk through the 2 KB staging buffer the NEXT TMA store will use, 16 columns
                         // at a time (rotated columns; lane L sums column L & 15 over rows 16 (L >> 4) .. + 15)
@@ -657,14 +581,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         }
                         if (defer_stats) {
 #pragma unroll
-                            for (int q = 0; q < 4; ++q)
-                                if (c == q * 32) {
+                            for (int q = 0; q < 2; ++q)
+                                if ((J >> 1) == q) {
                                     st1[q] += s1;
                                     st2[q] += s2;
                                 }
-                        } else if (n0 + c_begin + c + lane < p.Cout) {
-                            atomicAdd(p.stat_sum + n0 + c_begin + c + lane, s1);
-                            atomicAdd(p.stat_sqsum + n0 + c_begin + c + lane, s2);
+                        } else if (n0 + cc + lane < p.Cout) {
+                            atomicAdd(p.stat_acc + n0 + cc + lane, (double)s1);
+                            atomicAdd(p.stat_acc + CONV_STAT_MAX + n0 + cc + lane, (double)s2);
                         }
                     }
                     if (act == B2Y_ACT_LEAKY) {       // 0 <= slope <= 1 on this path: max(v, slope*v)
@@ -672,12 +596,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], v[j] * slope);
                     } else if (act == B2Y_ACT_MISH) {
                         // inlined closed form (one ex2, one rcp per element): 32 independent dependency chains the
-                        // scheduler can interleave -- as a call per element the epilogue was bound by the serial
-                        // MUFU latency of each chain (yolov4's Mish layers ran 2-6x slower than their leaky twins)
+                        // scheduler can interleave
 #pragma unroll
                         for (int j = 0; j < 32; ++j) v[j] = mish_f(v[j]);
                     }
-                    if (row_ok && res_p != nullptr) {
+                    if (has_res) {
 #pragma unroll
                         for (int q = 0; q < 4; ++q) {
                             const uint4 u = rcur[q];
@@ -752,13 +675,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             fence_proxy_async_cta();
                             __syncwarp();
                             if (lane == 0) {
-                                tma_store_2d(&tmC, smem_u32(buf), n0 + c_begin + c, m_tile * 128 + ew * 32);
+                                tma_store_2d(&tmC, smem_u32(buf), n0 + cc, m_tile * 128 + ew * 32);
                                 bulk_commit();
                             }
                             sbuf ^= 1;
                         } else if (row_ok) {
-                            uint4* op8 = reinterpret_cast<uint4*>(reinterpret_cast<int8_t*>(p.out) + row * p.out_pitch + n0 +
-                                                                  c_begin + c);
+                            uint4* op8 = reinterpret_cast<uint4*>(reinterpret_cast<int8_t*>(p.out) + row * p.out_pitch + n0 + cc);
                             op8[0] = make_uint4(w[0], w[1], w[2], w[3]);
                             op8[1] = make_uint4(w[4], w[5], w[6], w[7]);
                         }
@@ -776,7 +698,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         fence_proxy_async_cta();
                         __syncwarp();
                         if (lane == 0) {
-                            tma_store_2d(&tmC, smem_u32(buf), n0 + c_begin + c, m_tile * 128 + ew * 32);
+                            tma_store_2d(&tmC, smem_u32(buf), n0 + cc, m_tile * 128 + ew * 32);
                             bulk_commit();
                         }
                         continue;
@@ -809,72 +731,49 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         fence_proxy_async_cta();
                         __syncwarp();
                         if (lane == 0) {
-                            tma_store_2d(&tmC, smem_u32(buf), n0 + c_begin + c, m_tile * 128 + ew * 32);
+                            tma_store_2d(&tmC, smem_u32(buf), n0 + cc, m_tile * 128 + ew * 32);
                             bulk_commit();
                         }
                         sbuf ^= 1;
                     } else if (row_ok) {
+                        uint4* out_p = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.out) + row * p.out_pitch + n0 + cc);
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) out_p[c / 8 + q] = ou[q];
+                        for (int q = 0; q < 4; ++q) out_p[q] = ou[q];
                     }
-                }
-            } else {
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tc_fence_after();
-#pragma unroll 1
-                for (int c = 0; c < COLS_PER_GROUP; c += 32) {
-                    const int c0 = c_begin + c;
+                } else {
+                    if (n0 + cc >= p.Cout) continue;  // warp-uniform
                     uint32_t raw[32];
-                    tmem_ld_32x32(taddr_row + (uint32_t)c0, raw);
-                    tc_wait_ld();
-                    if (n0 + c0 >= p.Cout) continue;  // warp-uniform
+                    stage_row32<BLOCK_N>(acc_stage, trow, cc, raw);
                     float v[32];
 #pragma unroll
                     for (int j = 0; j < 32; ++j)
                         v[j] = ((KIND == CONV_KIND_F16) ? __uint_as_float(raw[j]) : (float)(int)raw[j]) * acc_mul;
                     float ds1, ds2;
-                    epi_chunk_general<KIND>(v, p, n0 + c0, row, row_ok, lane, my_stage, defer_stats, ds1, ds2);
+                    epi_chunk_general<KIND>(v, p, n0 + cc, row, row_ok, lane, my_stage, defer_stats, ds1, ds2);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        if (c == q * 32) {
+                    for (int q = 0; q < 2; ++q)
+                        if ((J >> 1) == q) {
                             st1[q] += ds1;
                             st2[q] += ds2;
                         }
                 }
             }
-            // release this accumulator stage back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (PAIR)
-                    mbar_arrive_cluster(mapa_u32(smem_u32(&tmem_empty_bar[acc]), 0));   // the leader's MMA warp waits on it
-                else
-                    mbar_arrive(&tmem_empty_bar[acc]);
-            }
         }
         if (defer_stats) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const int col = c_begin + q * 32 + lane;
-                if (q * 32 < COLS_PER_GROUP && col < p.Cout && (st1[q] != 0.f || st2[q] != 0.f)) {
-                    atomicAdd(p.stat_sum + col, st1[q]);
-                    atomicAdd(p.stat_sqsum + col, st2[q]);
+            for (int q = 0; q < 2; ++q) {
+                const int col = (2 * q + cg) * 32 + lane;
+                if ((2 * q + cg) * 32 < BLOCK_N && col < p.Cout && (st1[q] != 0.f || st2[q] != 0.f)) {
+                    atomicAdd(p.stat_acc + col, (double)st1[q]);
+                    atomicAdd(p.stat_acc + CONV_STAT_MAX + col, (double)st2[q]);
                 }
             }
         }
         if (epi_tma && lane == 0) bulk_wait_all();   // outstanding TMA stores complete before the CTA exits
     }
 
-    tc_fence_before();
     __syncthreads();
     if (CLUSTER > 1) cluster_sync_all();   // nobody leaves while a peer may still multicast / arrive into its smem
-    if (warp == 2) {
-        tc_fence_after();
-        if (PAIR)
-            tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-        else
-            tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-    }
 }
 
 }  // namespace b2y

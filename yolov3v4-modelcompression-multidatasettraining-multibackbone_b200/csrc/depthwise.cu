@@ -26,8 +26,8 @@ inline int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     int& s = sms[dev & 63];
-    if (s <= 0 && cudaDeviceGetAttribute(&s, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) s = 148;
-    if (s <= 0) s = 148;
+    if (s <= 0 && cudaDeviceGetAttribute(&s, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) s = 132;
+    if (s <= 0) s = 132;
     return s;
 }
 inline int grid_for_rows(long long rows, int ppb, int per_sm) {

@@ -114,7 +114,7 @@ extern "C" int b2y_kd_soft_rows(const float* student, const float* teacher, long
         return B2Y_ERR_INVALID;
     if (rows == 0) return B2Y_OK;
     long long blocks = (rows + 7) / 8;
-    if (blocks > 148LL * 16) blocks = 148LL * 16;
+    if (blocks > 132LL * 16) blocks = 132LL * 16;
     kd_soft_rows_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         student, teacher, rows, row_len, col0, width, 1.f / temperature, grad_scale / temperature, loss_acc, dstudent);
     B2Y_CUDA_CHECK(cudaGetLastError());

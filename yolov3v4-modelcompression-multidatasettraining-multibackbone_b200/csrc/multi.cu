@@ -79,7 +79,7 @@ pack_multi_kernel(const b2y_pack_item* __restrict__ items, int n_items) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // ---- load: per output channel one contiguous run of ni*k2 floats ----
     // all (<= 4 rows x 9) loads of a thread are issued before the first shared-memory store: with 4 scalar loads in flight
-    // per thread the kernel sat at 2.3 TB/s (latency bound: 25 KB in flight per SM)
+    // per thread the kernel was latency bound (25 KB in flight per SM)
     const int run = ni * k2;
     {
         float v[TO / 8][9];

@@ -9,7 +9,7 @@ using namespace b2y;
 static inline int grid_for(long long n, int block) {
     long long g = (n + block - 1) / block;
     if (g < 1) g = 1;
-    if (g > 148LL * 64) g = 148LL * 64;  // grid-stride beyond ~64 CTAs/SM worth of work
+    if (g > 132LL * 64) g = 132LL * 64;  // grid-stride beyond ~64 CTAs/SM worth of work
     return (int)g;
 }
 
@@ -97,7 +97,7 @@ extern "C" int b2y_stem_conv_fwd(const b2y_conv_desc* d, const float* x_nchw, co
     size_t smem = (size_t)(taps * CO + CO) * sizeof(float);
     if (smem > 48 * 1024) return B2Y_ERR_UNSUPPORTED;
     int grid = (int)((M + 127) / 128);
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > 132 * 16) grid = 132 * 16;
     stem_conv_kernel<CO><<<grid, 128, smem, static_cast<cudaStream_t>(stream)>>>(
         x_nchw, w, bias, reinterpret_cast<__half*>(y), d->batch, d->in_c, d->in_h, d->in_w, d->out_c, d->ksize,
         d->stride, d->pad, Ho, Wo, d->out_pitch, d->act, d->slope);

@@ -11,7 +11,7 @@ using namespace b2y;
 static inline int grid_for(long long n, int block) {
     long long g = (n + block - 1) / block;
     if (g < 1) g = 1;
-    if (g > 148LL * 16) g = 148LL * 16;
+    if (g > 132LL * 16) g = 132LL * 16;
     return (int)g;
 }
 
@@ -216,7 +216,7 @@ extern "C" int b2y_cos_scale_search_ex(const float* x, long long n, int bits, in
     double* acc = reinterpret_cast<double*>(workspace);
     B2Y_CUDA_CHECK(cudaMemsetAsync(acc, 0, sizeof(double) * (1 + 2 * n_cand), st));
     int grid = grid_for(n, 256);
-    if (grid > 148 * 4) grid = 148 * 4;
+    if (grid > 132 * 4) grid = 132 * 4;
     cos_search_kernel<<<grid, 256, 0, st>>>(x, n, bits, n_cand, step0, acc);
     cos_finalize_kernel<<<1, 32, 0, st>>>(acc, n_cand, out_cos);
     B2Y_CUDA_CHECK(cudaGetLastError());
@@ -397,7 +397,7 @@ extern "C" int b2y_qshortcut_i8(const void* x, long long x_pitch, const void* a,
     if (CV <= 256 && 256 % CV == 0) {
         const int ppb = 256 / CV;
         long long g = (pixels + ppb - 1) / ppb;
-        if (g > 148 * 8) g = 148 * 8;
+        if (g > 132 * 8) g = 132 * 8;
         if (g < 1) g = 1;
         const bool exact = is_pow2f(scale_x) && is_pow2f(scale_a) && is_pow2f(scale_sum);
         cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -546,7 +546,7 @@ extern "C" int b2y_stem_conv_fwd_q(const b2y_conv_desc* d, const float* x_nchw, 
     const size_t smem = (size_t)(taps * 32 + 32) * sizeof(float);
     if (smem > 48 * 1024) return B2Y_ERR_UNSUPPORTED;
     int grid = (int)((M + 127) / 128);
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > 132 * 16) grid = 132 * 16;
     stem_conv_q_kernel<<<grid, 128, smem, static_cast<cudaStream_t>(stream)>>>(
         x_nchw, w_q, bias_q, reinterpret_cast<int8_t*>(y_i8), d->batch, d->in_c, d->in_h, d->in_w, d->out_c, d->ksize,
         d->stride, d->pad, d->out_h, d->out_w, d->out_pitch, d->act, d->slope, out_scale, lo, hi);

@@ -8,15 +8,15 @@
 //   A[128 output pixels][32]  : row = one output pixel, columns (kh*K + kw)*Cin + c, zero padded to 32 (64 bytes),
 //                               written with st.shared in the canonical K-major SWIZZLE_64B layout
 //   B[BLOCK_N out channels][32]: the BN-folded weights, same layout, loaded once per CTA
-//   D = A * B^T               : one tcgen05.mma pair (2 x K=16) per tile, fp32 accumulator in TMEM
+//   D = A * B^T               : two wgmma.mma_async pairs (M = 2 x 64, K = 2 x 16) per tile, fp32 accumulators in
+//                               registers, staged through shared memory for the row-per-thread epilogue
 //
-// Persistent CTAs (one per SM).  NG groups of four "worker" warps; a group owns every NG-th tile of the CTA and runs a
-// three-stage software pipeline per thread (thread = one pixel row of the tile = one TMEM lane):
+// Persistent CTAs (one per SM).  NG warpgroups of "worker" warps; a group owns every NG-th tile of the CTA and runs a
+// three-stage software pipeline per thread (thread = one pixel row of the tile):
 //     issue the image loads of tile j      (27 predicated LDGs for 3x3 RGB)
-//     epilogue of tile j-1                 (TMEM -> bias/act -> 64-byte fp16 row), overlapping the loads in flight
-//     convert + store the A row of tile j  -> fence.proxy.async -> mbarrier arrive -> MMA warp issues tile j
-// Two smem/TMEM stages per group (tile parity); the accumulator-full barrier of tile j-2 doubles as the "stage free"
-// signal, so no empty barriers are needed.
+//     epilogue of tile j-1                 (staged accumulators -> bias/act -> 64-byte fp16 row), overlapping the
+//                                          loads in flight
+//     convert + store the A row of tile j  -> fence.proxy.async -> group barrier -> wgmma -> accumulators to smem
 #include <cmath>
 #include <cstdlib>
 
@@ -58,36 +58,20 @@ __device__ __forceinline__ float stem_ld<uint8_t>(const uint8_t* p) { return (fl
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 template <typename XT, int CIN, int K, int BLOCK_N, int NG>
-__global__ void __launch_bounds__(128 * NG + 64, 1) stem_fused_kernel(const __grid_constant__ StemParams p) {
+__global__ void __launch_bounds__(128 * NG, 1) stem_fused_kernel(const __grid_constant__ StemParams p) {
     constexpr int KK = CIN * K * K;            // <= 32
     constexpr int A_BYTES = 128 * 64;
     constexpr int B_BYTES = BLOCK_N * 64;
-    constexpr int NSTAGE = 2 * NG;
-    constexpr uint32_t IDESC = make_idesc(/*c=F32*/ 1, 0, 0, 0, 0, 128, BLOCK_N);
-    constexpr int TMEM_COLS = NSTAGE * BLOCK_N < 32 ? 32 : NSTAGE * BLOCK_N;   // power of two for NG in {1,2,4}
+    constexpr int ACC_BYTES = 128 * BLOCK_N * 4;
 
+    // smem: [NG A tiles] [B] [NG accumulator tiles]
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* smem_b = smem + NSTAGE * A_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + B_BYTES);   // [NSTAGE] A tile written (4 warp arrivals)
-    uint64_t* acc_bar = full_bar + NSTAGE;                                 // [NSTAGE] accumulator complete (commit)
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(acc_bar + NSTAGE);
+    uint8_t* smem_b = smem + NG * A_BYTES;
+    uint8_t* smem_acc = smem_b + B_BYTES;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    constexpr int MMA_WARP = 4 * NG;
-
-    if (warp == MMA_WARP && lane == 0) {
-        for (int i = 0; i < NSTAGE; ++i) {
-            mbar_init(&full_bar[i], 4);
-            mbar_init(&acc_bar[i], 1);
-        }
-        fence_barrier_init();
-    }
-    if (warp == MMA_WARP + 1) {
-        tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-        tmem_relinquish();
-    }
     // weights -> smem (SWIZZLE_64B: 16-byte chunk index ^= (row >> 1) & 3)
     for (int i = threadIdx.x; i < BLOCK_N * 4; i += blockDim.x) {
         const int row = i >> 2, ch = i & 3;
@@ -112,16 +96,13 @@ __global__ void __launch_bounds__(128 * NG + 64, 1) stem_fused_kernel(const __gr
         }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     const int my_tiles = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles of this CTA
 
-    if (warp < 4 * NG) {
-        // ===================== workers: build A rows + epilogue =====================
+    {
+        // ===================== workers: build A rows, MMA, epilogue =====================
         const int g = warp >> 2;
-        const int ew = warp & 3;                 // TMEM lane quarter == warp % 4
+        const int ew = warp & 3;                 // row quarter of the tile
         const int r_in_tile = ew * 32 + lane;
         const XT* xin = reinterpret_cast<const XT*>(p.x);
         const int plane = p.H * p.W;             // 32-bit image indexing (host checks B*Cin*H*W < 2^31)
@@ -135,8 +116,15 @@ __global__ void __launch_bounds__(128 * NG + 64, 1) stem_fused_kernel(const __gr
         const unsigned HoWo = (unsigned)(p.Ho * p.Wo), Wo = (unsigned)p.Wo;
         const unsigned M_total = (unsigned)p.M_total;
         const int my_group_tiles = (my_tiles - g + NG - 1) / NG;
-        uint8_t* arow0 = smem + r_in_tile * 64;
+        uint8_t* const arow = smem + g * A_BYTES + r_in_tile * 64;
+        uint8_t* const acc_tile = smem_acc + g * ACC_BYTES;
         const int sw = (r_in_tile >> 1) & 3;
+        const int tid_wg = (int)threadIdx.x & 127;
+        const uint32_t bar_id = 1 + g;           // named barrier of this group
+        const uint64_t desc_base = smem_desc_base(16, 8 * 64, swizzle_layout_type(64));
+        const uint32_t a_addr = smem_u32(smem + g * A_BYTES);
+        const uint64_t adesc0 = smem_desc_at(desc_base, a_addr), adesc1 = smem_desc_at(desc_base, a_addr + 64 * 64);
+        const uint64_t bdesc = smem_desc_at(desc_base, smem_u32(smem_b));
 
         unsigned prev_row = 0;
         for (int j = 0; j <= my_group_tiles; ++j) {
@@ -169,20 +157,14 @@ __global__ void __launch_bounds__(128 * NG + 64, 1) stem_fused_kernel(const __gr
                     }
                 }
             }
-            // ---- 2. epilogue of tile j-1 (stage (j-1)&1 of this group)
+            // ---- 2. epilogue of tile j-1 (accumulators staged at the end of the previous iteration)
             if (j > 0) {
-                const int jj = j - 1;
-                const int st = g * 2 + (jj & 1);
-                mbar_wait(&acc_bar[st], (uint32_t)(jj >> 1) & 1u);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(st * BLOCK_N);
                 const bool prow_ok = prev_row < M_total;
                 __half* orow = p.out + (long long)prev_row * p.out_pitch;
 #pragma unroll 1
                 for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
                     uint32_t acc[32];
-                    tmem_ld_32x32(taddr + (uint32_t)c0, acc);
-                    tc_wait_ld();
+                    stage_row32<BLOCK_N>(acc_tile, r_in_tile, c0, acc);
                     float v[32];
 #pragma unroll
                     for (int q = 0; q < 32; ++q) v[q] = __uint_as_float(acc[q]);
@@ -270,12 +252,11 @@ __global__ void __launch_bounds__(128 * NG + 64, 1) stem_fused_kernel(const __gr
                         }
                     }
                 }
-                tc_fence_before();   // TMEM reads of this stage are complete before the next arrive releases it
             }
-            // ---- 3. convert + store the A row of tile j, hand it to the MMA warp
+            // ---- 3. convert + store the A row of tile j, multiply, stage the accumulators
             if (have) {
-                const int st = g * 2 + (j & 1);
-                uint8_t* arow = arow0 + st * A_BYTES;
+                // every thread of the group is done with the staged accumulators and the A tile of tile j-1
+                named_bar_sync(bar_id, 128);
                 if (exact_div) {
 #pragma unroll
                     for (int k0 = 0; k0 < KK; ++k0) raw[k0] = __fdiv_rn(raw[k0], p.x_div);
@@ -306,54 +287,39 @@ __global__ void __launch_bounds__(128 * NG + 64, 1) stem_fused_kernel(const __gr
                     *reinterpret_cast<uint4*>(arow + ((ch ^ sw) << 4)) = u;
                 }
                 fence_proxy_async_smem();     // generic-proxy stores -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&full_bar[st]);
+                named_bar_sync(bar_id, 128);
+                float acc0[BLOCK_N / 2], acc1[BLOCK_N / 2];
+                wgmma_fence();
+                wgmma_ss<BLOCK_N, 0, 0>(acc0, adesc0, bdesc, 0u);
+                wgmma_ss<BLOCK_N, 0, 0>(acc0, adesc0 + 2, bdesc + 2, 1u);
+                wgmma_ss<BLOCK_N, 0, 0>(acc1, adesc1, bdesc, 0u);
+                wgmma_ss<BLOCK_N, 0, 0>(acc1, adesc1 + 2, bdesc + 2, 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc0);
+                wgmma_fence_acc(acc1);
+                frag_to_stage<BLOCK_N>(acc0, acc_tile, 0, tid_wg);
+                frag_to_stage<BLOCK_N>(acc1, acc_tile, 64, tid_wg);
+                named_bar_sync(bar_id, 128);
                 prev_row = row;
             }
         }
-    } else if (warp == MMA_WARP) {
-        // ===================== MMA issuer =====================
-        const uint64_t desc_base = smem_desc_base(16, 8 * 64, swizzle_layout_type(64));
-        const uint32_t a_base = smem_u32(smem), b_addr = smem_u32(smem_b);
-        const uint64_t bdesc = desc_base | (uint64_t)((b_addr >> 4) & 0x3FFF);
-        for (int i = 0; i < my_tiles; ++i) {
-            const int g = i % NG, j = i / NG;
-            const int st = g * 2 + (j & 1);
-            mbar_wait(&full_bar[st], (uint32_t)(j >> 1) & 1u);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t a_addr = a_base + st * A_BYTES;
-                const uint64_t adesc = desc_base | (uint64_t)((a_addr >> 4) & 0x3FFF);
-                const uint32_t d_tmem = tmem_base + (uint32_t)(st * BLOCK_N);
-                mma_f16_ss(d_tmem, adesc, bdesc, IDESC, 0u);
-                mma_f16_ss(d_tmem, adesc + 2, bdesc + 2, IDESC, 1u);
-                tc_commit(&acc_bar[st]);
-            }
-            __syncwarp();
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == MMA_WARP + 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
     }
 }
 
 template <typename XT, int CIN, int K, int BLOCK_N, int NG>
 static int stem_launch(const StemParams& p, cudaStream_t st) {
-    constexpr int SMEM = 1024 + 2 * NG * 128 * 64 + BLOCK_N * 64 + 256;
+    constexpr int SMEM = 1024 + NG * 128 * 64 + BLOCK_N * 64 + NG * 128 * BLOCK_N * 4;
     auto kern = stem_fused_kernel<XT, CIN, K, BLOCK_N, NG>;
     static unsigned long long attr_set = 0;      // one bit per device: the attribute is per (function, device)
     if (b2y_first_use_on_device(attr_set)) {
         B2Y_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-    kern<<<grid, 128 * NG + 64, SMEM, st>>>(p);
+    kern<<<grid, 128 * NG, SMEM, st>>>(p);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }

@@ -7,7 +7,7 @@
 
 using namespace b2y;
 
-static inline int grid_for(long long n, int block, int cap = 148 * 16) {
+static inline int grid_for(long long n, int block, int cap = 132 * 16) {
     long long g = (n + block - 1) / block;
     if (g < 1) g = 1;
     if (g > cap) g = cap;
@@ -127,7 +127,7 @@ bn_act_fwd_v2_kernel(const __half* __restrict__ x, long long xp, const float* __
 static inline int v2_grid(long long pixels, int CV) {
     const int ppb = 256 / CV;
     long long g = (pixels + ppb - 1) / ppb;
-    const long long cap = 148 * 8;
+    const long long cap = 132 * 8;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 static inline bool v2_ok(int c) { return c % 8 == 0 && c / 8 <= 256 && 256 % (c / 8) == 0; }
@@ -168,7 +168,7 @@ __global__ void __launch_bounds__(256)
 bn_act_bwd_reduce_kernel(const __half* __restrict__ x, long long xp, const GT* __restrict__ dy, long long dp,
                          const float* __restrict__ scale, const float* __restrict__ shift,
                          const float* __restrict__ mean, const float* __restrict__ invstd,
-                         float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ du_absmax,
+                         double* __restrict__ dgamma, double* __restrict__ dbeta, float* __restrict__ du_absmax,
                          long long pixels, int C, int act, float slope) {
     __shared__ float red[8][32][17];
     float amax = 0.f;
@@ -242,8 +242,8 @@ bn_act_bwd_reduce_kernel(const __half* __restrict__ x, long long xp, const GT* _
                 b += red[w][lc][j];
                 g += red[w][lc][8 + j];
             }
-            atomicAdd(dbeta + cv * 8 + j, b);
-            if (dgamma != nullptr) atomicAdd(dgamma + cv * 8 + j, g);
+            atomicAdd(dbeta + cv * 8 + j, (double)b);
+            if (dgamma != nullptr) atomicAdd(dgamma + cv * 8 + j, (double)g);
         }
     }
 }
@@ -253,7 +253,7 @@ __global__ void __launch_bounds__(256)
 bn_act_bwd_reduce_v2_kernel(const __half* __restrict__ x, long long xp, const GT* __restrict__ dy, long long dp,
                             const float* __restrict__ scale, const float* __restrict__ shift,
                             const float* __restrict__ mean, const float* __restrict__ invstd,
-                            float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ du_absmax,
+                            double* __restrict__ dgamma, double* __restrict__ dbeta, float* __restrict__ du_absmax,
                             long long pixels, int CV, float slope) {
     __shared__ float red[256][17];
     const int cv = threadIdx.x % CV;
@@ -300,16 +300,16 @@ bn_act_bwd_reduce_v2_kernel(const __half* __restrict__ x, long long xp, const GT
         float sum = 0.f;
         for (int k = 0; k < ppb; ++k) sum += red[v + k * CV][comp];
         if (comp < 8)
-            atomicAdd(dbeta + v * 8 + comp, sum);
+            atomicAdd(dbeta + v * 8 + comp, (double)sum);
         else if (dgamma != nullptr)
-            atomicAdd(dgamma + v * 8 + comp - 8, sum);
+            atomicAdd(dgamma + v * 8 + comp - 8, (double)sum);
     }
 }
 
-extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const void* dy, long long dy_pitch,
-                                     const float* scale, const float* shift, const float* save_mean,
-                                     const float* save_invstd, float* dgamma, float* dbeta, float* du_absmax,
-                                     long long pixels, int c, int act, float slope, int grad_dtype, void* stream) {
+static int bn_act_bwd_reduce_launch(const void* x, long long x_pitch, const void* dy, long long dy_pitch,
+                                    const float* scale, const float* shift, const float* save_mean,
+                                    const float* save_invstd, double* dgamma, double* dbeta, float* du_absmax,
+                                    long long pixels, int c, int act, float slope, int grad_dtype, void* stream) {
     if (!x || !dy || !scale || !shift || !dbeta || c % 8 != 0 || x_pitch % 8 != 0 || dy_pitch % 8 != 0)
         return B2Y_ERR_INVALID;
     const int CV = c / 8;
@@ -336,7 +336,7 @@ extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const voi
     }
     dim3 grid(1, (CV + 31) / 32);
     long long want = (pixels + 63) / 64;
-    grid.x = (unsigned)(want < 1 ? 1 : (want > 148 * 4 ? 148 * 4 : want));
+    grid.x = (unsigned)(want < 1 ? 1 : (want > 132 * 4 ? 132 * 4 : want));
     if (grad_dtype == B2Y_DT_BF16)
         bn_act_bwd_reduce_kernel<__nv_bfloat16><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
             reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, scale,
@@ -347,6 +347,23 @@ extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const voi
             save_mean, save_invstd, dgamma, dbeta, du_absmax, pixels, c, act, slope);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
+}
+
+extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const void* dy, long long dy_pitch,
+                                     const float* scale, const float* shift, const float* save_mean,
+                                     const float* save_invstd, float* dgamma, float* dbeta, float* du_absmax,
+                                     long long pixels, int c, int act, float slope, int grad_dtype, void* stream) {
+    if (!dbeta) return B2Y_ERR_INVALID;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* acc = stream_acc(st, 2LL * c);     // [0, C) dbeta, [C, 2C) dgamma
+    if (acc == nullptr) return B2Y_ERR_CUDA;
+    int rc = bn_act_bwd_reduce_launch(x, x_pitch, dy, dy_pitch, scale, shift, save_mean, save_invstd,
+                                      dgamma != nullptr ? acc + c : nullptr, acc, du_absmax, pixels, c, act, slope,
+                                      grad_dtype, stream);
+    if (rc != B2Y_OK) return rc;
+    rc = acc_finalize(acc, dbeta, c, st);
+    if (rc != B2Y_OK || dgamma == nullptr) return rc;
+    return acc_finalize(acc + c, dgamma, c, st);
 }
 
 // backward pass 2: dx = gamma*invstd * (du - dbeta/N - xhat*dgamma/N)
@@ -659,7 +676,7 @@ extern "C" int b2y_yolo_grad_to_raw(const float* dp, void* draw, long long raw_p
     const long long total = (long long)batch * ny * nx * raw_pitch;
     if (raw_pitch <= 256 && (long long)batch * ny * nx < 0x7fffffffLL) {
         long long pb = ((long long)batch * ny * nx + 7) / 8;
-        if (pb > 148 * 8) pb = 148 * 8;
+        if (pb > 132 * 8) pb = 132 * 8;
         if (grad_dtype == B2Y_DT_BF16)
             yolo_grad_to_raw_pixel_kernel<__nv_bfloat16><<<(int)pb, 256, 0, static_cast<cudaStream_t>(stream)>>>(
                 dp, reinterpret_cast<__nv_bfloat16*>(draw), raw_pitch, batch, na, no, ny, nx, scale, scale_ptr);
@@ -790,13 +807,12 @@ __global__ void __launch_bounds__(256) maxpool_plane_bwd_kernel(const __half* __
     __shared__ __align__(16) __half sx[POOL_PLANE_MAX * 8];
     __shared__ __align__(16) __half sr[POOL_PLANE_MAX * 8];
     __shared__ unsigned char sa[POOL_PLANE_MAX * 8];
-    __shared__ float acc[POOL_PLANE_MAX * 8];
+    __shared__ unsigned short sarg[POOL_PLANE_MAX * 8];   // argmax pixel (y * W + x) of every output
     const int CV = C / 8;
     const int n = blockIdx.x / CV, cv = blockIdx.x - n * CV;
     const int HW = H * W, pad = (k - 1) / 2;
     for (int i = threadIdx.x; i < HW; i += blockDim.x)
         reinterpret_cast<uint4*>(sx)[i] = __ldg(reinterpret_cast<const uint4*>(x + ((long long)n * HW + i) * xp) + cv);
-    for (int i = threadIdx.x; i < HW * 8; i += blockDim.x) acc[i] = 0.f;
     __syncthreads();
     for (int i = threadIdx.x; i < HW * 8; i += blockDim.x) {
         const int c = i & 7, pix = i >> 3;
@@ -830,16 +846,28 @@ __global__ void __launch_bounds__(256) maxpool_plane_bwd_kernel(const __half* __
         }
         // NaN rows never win a strict '>' (same as the general kernel, whose -inf start is replaced by the first value)
         const int ax = sa[(ay * W + xo) * 8 + c];
-        const float g = Half8<GT>::to_f(sdy[i]);
-        atomicAdd(&acc[(ay * W + ax) * 8 + c], g);
+        sarg[i] = (unsigned short)(ay * W + ax);
     }
     __syncthreads();
+    // gather: every input sums the gradients of the outputs whose window maximum it is, in a fixed order (no atomics, so
+    // the sum does not depend on scheduling)
     for (int i = threadIdx.x; i < HW; i += blockDim.x) {
+        const int yi = i / W, xi = i - yi * W;
+        const int ya = max(yi + pad - k + 1, 0), yb = min(yi + pad, H - 1);
+        const int xa = max(xi + pad - k + 1, 0), xb = min(xi + pad, W - 1);
+        float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        for (int yo = ya; yo <= yb; ++yo)
+            for (int xo = xa; xo <= xb; ++xo) {
+                const int o = yo * W + xo;
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+                    if (sarg[o * 8 + j] == i) s[j] += Half8<GT>::to_f(sdy[o * 8 + j]);
+            }
         GT* d = dx + ((long long)n * HW + i) * dxp + cv * 8;
         float f[8];
         Half8<GT>::load(d, f);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] += acc[i * 8 + j];
+        for (int j = 0; j < 8; ++j) f[j] += s[j];
         Half8<GT>::store(d, f);
     }
 }
@@ -895,7 +923,7 @@ extern "C" int b2y_maxpool_bwd(const void* x, long long x_pitch, const void* dy,
 // ------------------------------------------------------------------------------------------------
 template <int TPG, typename GT>
 __global__ void __launch_bounds__(256)
-stem_wgrad_kernel(const float* __restrict__ x, const GT* __restrict__ dz, long long dzp, float* __restrict__ dw,
+stem_wgrad_kernel(const float* __restrict__ x, const GT* __restrict__ dz, long long dzp, double* __restrict__ dw,
                   int B, int Cin, int H, int W, int Cout, int k, int stride, int pad, int Ho, int Wo, float scale) {
     const int taps = Cin * k * k;
     const int co_l = threadIdx.x & 31;
@@ -935,7 +963,7 @@ stem_wgrad_kernel(const float* __restrict__ x, const GT* __restrict__ dz, long l
         if (co < Cout) {
 #pragma unroll
             for (int j = 0; j < TPG; ++j)
-                if (grp * TPG + j < taps) atomicAdd(dw + (long long)co * taps + grp * TPG + j, acc[j] * scale);
+                if (grp * TPG + j < taps) atomicAdd(dw + (long long)co * taps + grp * TPG + j, (double)(acc[j] * scale));
         }
     }
 }
@@ -944,18 +972,20 @@ extern "C" int b2y_stem_conv_bwd_weight(const b2y_conv_desc* d, const float* x_n
     if (!d || !x_nchw || !dz || !dw_oihw) return B2Y_ERR_INVALID;
     const int taps = d->in_c * d->ksize * d->ksize;
     if (d->in_c > 4 || taps > 8 * 5) return B2Y_ERR_UNSUPPORTED;
+    double* acc = stream_acc(static_cast<cudaStream_t>(stream), (long long)d->out_c * taps);
+    if (acc == nullptr) return B2Y_ERR_CUDA;
     const long long M = (long long)d->batch * d->out_h * d->out_w;
     int grid = (int)((M + 1023) / 1024);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     if (grid < 1) grid = 1;
     if (grad_dtype == B2Y_DT_BF16)
         stem_wgrad_kernel<5, __nv_bfloat16><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-            x_nchw, reinterpret_cast<const __nv_bfloat16*>(dz), d->out_pitch, dw_oihw, d->batch, d->in_c, d->in_h,
+            x_nchw, reinterpret_cast<const __nv_bfloat16*>(dz), d->out_pitch, acc, d->batch, d->in_c, d->in_h,
             d->in_w, d->out_c, d->ksize, d->stride, d->pad, d->out_h, d->out_w, scale);
     else
         stem_wgrad_kernel<5, __half><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-            x_nchw, reinterpret_cast<const __half*>(dz), d->out_pitch, dw_oihw, d->batch, d->in_c, d->in_h, d->in_w,
+            x_nchw, reinterpret_cast<const __half*>(dz), d->out_pitch, acc, d->batch, d->in_c, d->in_h, d->in_w,
             d->out_c, d->ksize, d->stride, d->pad, d->out_h, d->out_w, scale);
     B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
+    return acc_finalize(acc, dw_oihw, (long long)d->out_c * taps, static_cast<cudaStream_t>(stream));
 }

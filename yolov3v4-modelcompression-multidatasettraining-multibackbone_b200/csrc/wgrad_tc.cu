@@ -1,9 +1,9 @@
-// Weight gradient of a dense convolution as a tcgen05 GEMM with the *pixel* dimension as K:
+// Weight gradient of a dense convolution as a wgmma GEMM with the *pixel* dimension as K:
 //
 //   dW[co][tap][ci] = sum_{pixel m} dY[m][co] * X[m @ tap][ci]
 //
 // Both operands are pixel-major in HBM (NHWC), i.e. "MN-major" for the tensor core: the TMA boxes
-// [64 pixels][64 channels] land in smem exactly as a 128B-swizzled MN-major UMMA operand, so neither
+// [64 pixels][64 channels] land in smem exactly as a 128B-swizzled MN-major wgmma operand, so neither
 // tensor is ever transposed or im2col'ed in memory.  dY comes through a tiled 2-D map, X through the im2col
 // map (tap offset + zero fill for the halo).  Work = (Cout/128) x (Cin/BLOCK_N) x taps x split-K slices;
 // the fp32 accumulator tile is reduced into dW with vector red.global.add.
@@ -23,9 +23,9 @@ struct WgradParams {
     int ksteps_total;         // ceil(K_total / BK)
     int ksteps_per_split;
     float scale;              // multiplies the accumulator (1 / loss-scale)
-    unsigned idesc_ab;        // operand formats (both operands must share it: mixed f16/bf16 faults in hardware)
+    int ab_bf16;              // both operands bf16 (else fp16; wgmma takes one 16-bit format for A and B)
     const float* scale_ptr;   // optional device scalar multiplied into `scale` (per-layer gradient un-scaling)
-    float* dw;                // fp32 [Cout][k][k][Cin], accumulated with atomics
+    double* acc;              // [Cout][k][k][Cin] accumulator (stream_acc), added into dw by acc_finalize
 };
 
 template <int BLOCK_N, int NB_ROW_BYTES>
@@ -39,30 +39,27 @@ struct WgradCfg {
     static constexpr int A_BYTES = A_ATOMS * A_ATOM_BYTES;          // 16 KB
     static constexpr int B_BYTES = B_ATOMS * B_ATOM_BYTES;
     static constexpr int STAGE_BYTES = A_BYTES + ((B_BYTES + 1023) / 1024) * 1024;
-    static constexpr int NUM_STAGES_RAW = (192 * 1024) / STAGE_BYTES;
+    static constexpr int NUM_STAGES_RAW = (225 * 1024) / STAGE_BYTES;
     static constexpr int NUM_STAGES = NUM_STAGES_RAW > 6 ? 6 : NUM_STAGES_RAW;
-    static constexpr int TMEM_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;
     static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + 1024;
 };
 
+// warp 0: TMA producer; warps 4-11: two consumer warpgroups, warpgroup g owns output channels 64 g .. 64 g + 63 of the
+// tile (A atom g) and reduces its accumulator fragment straight from registers into dW.
 template <int BLOCK_N, int NB_ROW_BYTES>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                 const WgradParams p) {
     using Cfg = WgradCfg<BLOCK_N, NB_ROW_BYTES>;
     constexpr int NS = Cfg::NUM_STAGES;
     constexpr int BK = Cfg::BK;
-    constexpr uint32_t IDESC = make_idesc(/*c=F32*/ 1, /*a=F16*/ 0, /*b=F16*/ 0, /*a MN-major*/ 1, /*b MN-major*/ 1,
-                                          128, BLOCK_N);
+    constexpr int CONSUMER_WARPS = 8;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* aux = smem + NS * Cfg::STAGE_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + NS;
-    uint64_t* tmem_full_bar = empty_bar + NS;
-    uint64_t* tmem_empty_bar = tmem_full_bar + 1;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -74,20 +71,11 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant_
     if (warp == 1 && lane == 0) {
         for (int i = 0; i < NS; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
+            mbar_init(&empty_bar[i], CONSUMER_WARPS);
         }
-        mbar_init(tmem_full_bar, 1);
-        mbar_init(tmem_empty_bar, 4);
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
     const int num_tiles = p.m_tiles * p.n_tiles * p.ntaps * p.ksplits;
 
@@ -101,168 +89,134 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant_
         m_tile = t / p.n_tiles;
     };
 
-    // Both issue loops run warp-uniform with one elected lane issuing (same reason as in conv_tc.cuh: a single divergent
-    // lane pays ~10 extra R2UR/ELECT instructions per TMA / MMA issue and the loop becomes the bottleneck).
+    // The issue loop runs warp-uniform with one elected lane issuing (same reason as in conv_tc.cuh).
     if (warp == 0) {
-        {
-            uint32_t stage = 0;
-            uint32_t phase = 0;
-            const int HoWo = p.MH * p.MW;
-            const uint32_t smem_base = smem_u32(smem), full_base = smem_u32(full_bar), empty_base = smem_u32(empty_bar);
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                int m_tile, n_tile, tap, split;
-                decode(tile, m_tile, n_tile, tap, split);
-                const int r = tap / p.ksize, s = tap - r * p.ksize;
-                const int ks0 = split * p.ksteps_per_split;
-                const int ks1 = min(ks0 + p.ksteps_per_split, p.ksteps_total);
-                // pixel coordinates of the k-step, advanced incrementally (BK pixels per step)
-                int k0 = ks0 * BK;
-                int img = k0 / HoWo;
-                int rem = k0 - img * HoWo;
-                for (int ks = ks0; ks < ks1; ++ks) {
-                    const int po = rem / p.MW, qo = rem - po * p.MW;
-                    mbar_wait_s(empty_base + stage * 8, phase ^ 1);
-                    if (elect_one()) {
-                        const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
-                        const uint32_t b_dst = a_dst + Cfg::A_BYTES;
-                        const uint32_t fb = full_base + stage * 8;
-                        mbar_expect_tx_s(fb, Cfg::A_BYTES + Cfg::B_BYTES);
+        uint32_t stage = 0;
+        uint32_t phase = 0;
+        const int HoWo = p.MH * p.MW;
+        const uint32_t smem_base = smem_u32(smem), full_base = smem_u32(full_bar), empty_base = smem_u32(empty_bar);
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            int m_tile, n_tile, tap, split;
+            decode(tile, m_tile, n_tile, tap, split);
+            const int r = tap / p.ksize, s = tap - r * p.ksize;
+            const int ks0 = split * p.ksteps_per_split;
+            const int ks1 = min(ks0 + p.ksteps_per_split, p.ksteps_total);
+            // pixel coordinates of the k-step, advanced incrementally (BK pixels per step)
+            int k0 = ks0 * BK;
+            int img = k0 / HoWo;
+            int rem = k0 - img * HoWo;
+            for (int ks = ks0; ks < ks1; ++ks) {
+                const int po = rem / p.MW, qo = rem - po * p.MW;
+                mbar_wait_s(empty_base + stage * 8, phase ^ 1);
+                if (elect_one()) {
+                    const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
+                    const uint32_t b_dst = a_dst + Cfg::A_BYTES;
+                    const uint32_t fb = full_base + stage * 8;
+                    mbar_expect_tx_s(fb, Cfg::A_BYTES + Cfg::B_BYTES);
 #pragma unroll
-                        for (int at = 0; at < Cfg::A_ATOMS; ++at)
-                            tma_load_2d_s(a_dst + at * Cfg::A_ATOM_BYTES, &tmDy, fb, m_tile * 128 + at * 64, k0);
+                    for (int at = 0; at < Cfg::A_ATOMS; ++at)
+                        tma_load_2d_s(a_dst + at * Cfg::A_ATOM_BYTES, &tmDy, fb, m_tile * 128 + at * 64, k0);
 #pragma unroll
-                        for (int at = 0; at < Cfg::B_ATOMS; ++at)
-                            tma_load_im2col_4d_s(b_dst + at * Cfg::B_ATOM_BYTES, &tmX, fb,
-                                                 n_tile * BLOCK_N + at * Cfg::B_ATOM_CH, qo * p.stride - p.pad,
-                                                 po * p.stride - p.pad, img, (uint16_t)s, (uint16_t)r);
-                    }
-                    k0 += BK;
-                    rem += BK;
-                    if (rem >= HoWo) {      // BK <= HoWo is not guaranteed for tiny maps: general wrap
-                        img += rem / HoWo;
-                        rem = rem % HoWo;
-                    }
-                    if (++stage == NS) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
+                    for (int at = 0; at < Cfg::B_ATOMS; ++at)
+                        tma_load_im2col_4d_s(b_dst + at * Cfg::B_ATOM_BYTES, &tmX, fb,
+                                             n_tile * BLOCK_N + at * Cfg::B_ATOM_CH, qo * p.stride - p.pad,
+                                             po * p.stride - p.pad, img, (uint16_t)s, (uint16_t)r);
                 }
-            }
-        }
-    } else if (warp == 1) {
-        {
-            int stage = 0;
-            uint32_t phase = 0;
-            uint32_t acc_phase = 0;
-            // MN-major canonical layouts: LBO = distance between 64-channel atoms, SBO = 8 K-rows
-            const uint64_t adesc_base = smem_desc_base(Cfg::A_ATOM_BYTES, 8 * 128, swizzle_layout_type(128));
-            const uint64_t bdesc_base =
-                smem_desc_base(Cfg::B_ATOM_BYTES, 8 * NB_ROW_BYTES, swizzle_layout_type(NB_ROW_BYTES));
-            const uint32_t idesc = IDESC | p.idesc_ab;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                int m_tile, n_tile, tap, split;
-                decode(tile, m_tile, n_tile, tap, split);
-                const int ks0 = split * p.ksteps_per_split;
-                const int ks1 = min(ks0 + p.ksteps_per_split, p.ksteps_total);
-                mbar_wait(tmem_empty_bar, acc_phase ^ 1);
-                tc_fence_after();
-                uint32_t accum = 0;
-                for (int ks = ks0; ks < ks1; ++ks) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                        const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            const uint64_t adesc = smem_desc_at(adesc_base, a_addr + k * 16 * 128);
-                            const uint64_t bdesc = smem_desc_at(bdesc_base, b_addr + k * 16 * NB_ROW_BYTES);
-                            mma_f16_ss(tmem_base, adesc, bdesc, idesc, k > 0 ? 1u : accum);
-                        }
-                        tc_commit(&empty_bar[stage]);
-                    }
-                    accum = 1;
-                    if (++stage == NS) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
+                k0 += BK;
+                rem += BK;
+                if (rem >= HoWo) {      // BK <= HoWo is not guaranteed for tiny maps: general wrap
+                    img += rem / HoWo;
+                    rem = rem % HoWo;
                 }
-                if (elect_one()) tc_commit(tmem_full_bar);
-                acc_phase ^= 1;
+                if (++stage == NS) {
+                    stage = 0;
+                    phase ^= 1;
+                }
             }
         }
     } else if (warp >= 4) {
-        const int ew = warp - 4;
-        uint32_t acc_phase = 0;
+        const int wg = (warp - 4) >> 2;
+        const int tid_wg = (int)threadIdx.x & 127;
+        const bool bf16 = p.ab_bf16 != 0;
+        uint32_t stage = 0, phase = 0;
+        // MN-major canonical layouts: LBO = distance between MN atoms, SBO = 8 K-rows
+        const uint64_t adesc_base = smem_desc_base(Cfg::A_ATOM_BYTES, 8 * 128, swizzle_layout_type(128));
+        const uint64_t bdesc_base =
+            smem_desc_base(Cfg::B_ATOM_BYTES, 8 * NB_ROW_BYTES, swizzle_layout_type(NB_ROW_BYTES));
         const float wscale = p.scale * (p.scale_ptr != nullptr ? __ldg(p.scale_ptr) : 1.f);
+        const uint32_t full_base = smem_u32(full_bar), empty_base = smem_u32(empty_bar);
+        // this thread's fragment coordinates (see wgmma.cuh)
+        const int frow = 64 * wg + 16 * (tid_wg >> 5) + ((tid_wg & 31) >> 2);
+        const int fcol = 2 * (tid_wg & 3);
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int m_tile, n_tile, tap, split;
             decode(tile, m_tile, n_tile, tap, split);
             const int ks0 = split * p.ksteps_per_split;
-            const bool has_work = ks0 < p.ksteps_total;
-            mbar_wait(tmem_full_bar, acc_phase);
-            tc_fence_after();
-            const int co = m_tile * 128 + ew * 32 + lane;
-            const uint32_t taddr_row = tmem_base + ((uint32_t)(ew * 32) << 16);
-#pragma unroll 1
-            for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-                uint32_t raw[32];
-                if (BLOCK_N >= 32) {
-                    tmem_ld_32x32(taddr_row + (uint32_t)c0, raw);
-                } else {
-                    // BLOCK_N == 16: the allocation is 32 columns wide, upper half is unused
-                    tmem_ld_32x32(taddr_row, raw);
+            const int ks1 = min(ks0 + p.ksteps_per_split, p.ksteps_total);
+            if (ks0 >= ks1) continue;
+            float acc[BLOCK_N / 2];
+            uint32_t prev = 0;
+            for (int ks = ks0; ks < ks1; ++ks) {
+                mbar_wait_s(full_base + stage * 8, phase);
+                const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * Cfg::A_ATOM_BYTES;
+                const uint32_t b_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint64_t adesc = smem_desc_at(adesc_base, a_addr + k * 16 * 128);
+                    const uint64_t bdesc = smem_desc_at(bdesc_base, b_addr + k * 16 * NB_ROW_BYTES);
+                    const uint32_t sc = (ks > ks0 || k > 0) ? 1u : 0u;
+                    if (bf16)
+                        wgmma_ss<BLOCK_N, 1, 1>(acc, adesc, bdesc, sc);
+                    else
+                        wgmma_ss<BLOCK_N, 0, 1>(acc, adesc, bdesc, sc);
                 }
-                tc_wait_ld();
-                const int ci0 = n_tile * BLOCK_N + c0;
-                if (has_work && co < p.Cout && ci0 < p.Cin) {
-                    float* dst = p.dw + ((long long)co * p.ntaps + tap) * p.Cin + ci0;
-                    const int nvalid = min(min(32, BLOCK_N), p.Cin - ci0);
-                    if (nvalid == 32 && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
+                wgmma_commit();
+                if (ks > ks0) {
+                    wgmma_wait<1>();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = stage;
+                if (++stage == NS) {
+                    stage = 0;
+                    phase ^= 1;
+                }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            // fp32 partial sums -> dW[co][tap][ci], two adjacent channels per vector reduction
 #pragma unroll
-                        for (int q = 0; q < 8; ++q) {
-                            float4 v = make_float4(__uint_as_float(raw[q * 4]) * wscale,
-                                                   __uint_as_float(raw[q * 4 + 1]) * wscale,
-                                                   __uint_as_float(raw[q * 4 + 2]) * wscale,
-                                                   __uint_as_float(raw[q * 4 + 3]) * wscale);
-                            atomicAdd(reinterpret_cast<float4*>(dst) + q, v);
-                        }
-                    } else {
+            for (int h = 0; h < 2; ++h) {
+                const int co = m_tile * 128 + frow + 8 * h;
+                if (co >= p.Cout) continue;
+                double* drow = p.acc + ((long long)co * p.ntaps + tap) * p.Cin;
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < nvalid) atomicAdd(dst + j, __uint_as_float(raw[j]) * wscale);
+                for (int i = 0; i < BLOCK_N / 8; ++i) {
+                    const int ci = n_tile * BLOCK_N + 8 * i + fcol;
+                    if (ci < p.Cin) {
+                        atomicAdd(drow + ci, (double)(acc[4 * i + 2 * h] * wscale));
+                        atomicAdd(drow + ci + 1, (double)(acc[4 * i + 2 * h + 1] * wscale));
                     }
                 }
-                __syncwarp();
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmem_empty_bar);
-            acc_phase ^= 1;
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
     }
 }
 
 // ---- narrow-input 3x3 layers (Cin = 32 / 64) -----------------------------------------------------------------
-// The kernel above re-reads dY once per filter tap and feeds the tensor core N = Cin <= 64 columns: on the first
-// (largest) layers of the net -- 3x3, 32->64 at 320x320 -- it moved 108 KB through L2 per 64 pixels and ran at 106 TF/s
-// (0.28 ms, 12x its HBM time).  Here the GEMM is transposed:
+// The kernel above re-reads dY once per filter tap and feeds the tensor core N = Cin <= 64 columns.  Here the GEMM is
+// transposed:
 //
 //   dW^T[(tap, ci)][co] = sum_{pixel m} X[m @ tap][ci] * dY[m][co]
 //
 // A = X: the nine im2col boxes [64 pixels][Cin] of one k-step sit back to back in smem; 128 / Cin consecutive boxes
-//        are one MN-major M = 128 operand (LBO = box size), so the 9 taps are GROUPS = 3 (Cin 32) or 5 (Cin 64) MMAs;
+//        are one MN-major M = 128 operand (LBO = box size), so the 9 taps are GROUPS = 3 (Cin 32) or 5 (Cin 64) groups;
 // B = dY: one [64 pixels][BLOCK_N] tile per k-step, loaded ONCE and shared by all taps.
-// Per 64 pixels 44 KB (Cin 32) / 80 KB (Cin 64) instead of 108 / 144 KB.  The last group's missing taps read whatever
-// follows in smem (the allocation is padded): garbage rows of D that the epilogue never stores.  Work = n_tiles x
-// split-K slices (~ one per SM); D rows are (tap, ci), columns co -> red.global.add into dW[co][tap][ci], 128 B per warp.
+// Warpgroup w of the two consumer warpgroups owns rows 64 w .. 64 w + 63 of every group, with one register accumulator
+// per group (BLOCK_N = 64 for Cin 32, 32 for Cin 64: 96 / 80 accumulator registers per thread).  The last group's
+// missing taps read whatever follows in smem (the allocation is padded): garbage rows of D that are never stored.
+// Work = n_tiles x split-K slices (~ one per SM); D rows are (tap, ci), columns co.
 template <int ROW_BYTES, int BLOCK_N>
 struct WgradTCfg {
     static constexpr int BK = 64;
@@ -271,35 +225,33 @@ struct WgradTCfg {
     static constexpr int TPG = 128 / CIN;
     static constexpr int GROUPS = (NTAPS + TPG - 1) / TPG;
     static constexpr int X_ATOM_BYTES = BK * ROW_BYTES;
-    static constexpr int DY_ATOMS = BLOCK_N / 64;
-    static constexpr int DY_BYTES = DY_ATOMS * BK * 128;
+    static constexpr int DY_ROW = BLOCK_N >= 64 ? 128 : BLOCK_N * 2;   // swizzle span of the dY tile
+    static constexpr int DY_ATOM_CO = DY_ROW / 2;
+    static constexpr int DY_ATOMS = BLOCK_N / DY_ATOM_CO;
+    static constexpr int DY_BYTES = DY_ATOMS * BK * DY_ROW;
     static constexpr int STAGE_BYTES = DY_BYTES + NTAPS * X_ATOM_BYTES;
-    static constexpr int NUM_STAGES = (190 * 1024) / STAGE_BYTES;
     static constexpr int PAD_BYTES = (GROUPS * TPG - NTAPS) * X_ATOM_BYTES;
-    static constexpr int TMEM_COLS = 512;
+    static constexpr int NUM_STAGES_RAW = (223 * 1024 - PAD_BYTES) / STAGE_BYTES;
+    static constexpr int NUM_STAGES = NUM_STAGES_RAW > 6 ? 6 : NUM_STAGES_RAW;
     static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + PAD_BYTES + 1024;
-    static_assert(GROUPS * BLOCK_N <= 512, "accumulators exceed TMEM");
     static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
+    static_assert(NUM_STAGES >= 2, "pipeline depth");
 };
 
-template <int ROW_BYTES, int BLOCK_N>
-__global__ void __launch_bounds__(256, 1)
+template <int ROW_BYTES, int BLOCK_N, int BF16>
+__global__ void __launch_bounds__(384, 1)
 wgrad_taps_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                   const WgradParams p) {
     using Cfg = WgradTCfg<ROW_BYTES, BLOCK_N>;
     constexpr int NS = Cfg::NUM_STAGES;
     constexpr int BK = Cfg::BK;
-    constexpr uint32_t IDESC = make_idesc(/*c=F32*/ 1, /*a=F16*/ 0, /*b=F16*/ 0, /*a MN-major*/ 1, /*b MN-major*/ 1,
-                                          128, BLOCK_N);
+    constexpr int CONSUMER_WARPS = 8;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* aux = smem + NS * Cfg::STAGE_BYTES + Cfg::PAD_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + NS;
-    uint64_t* tmem_full_bar = empty_bar + NS;
-    uint64_t* tmem_empty_bar = tmem_full_bar + 1;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -311,27 +263,18 @@ wgrad_taps_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     if (warp == 1 && lane == 0) {
         for (int i = 0; i < NS; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
+            mbar_init(&empty_bar[i], CONSUMER_WARPS);
         }
-        mbar_init(tmem_full_bar, 1);
-        mbar_init(tmem_empty_bar, 4);
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
     const int num_items = p.n_tiles * p.ksplits;      // item -> (n_tile, split), split fastest
+    const uint32_t smem_base = smem_u32(smem), full_base = smem_u32(full_bar), empty_base = smem_u32(empty_bar);
 
     if (warp == 0) {
         uint32_t stage = 0, phase = 0;
         const int HoWo = p.MH * p.MW;
-        const uint32_t smem_base = smem_u32(smem), full_base = smem_u32(full_bar), empty_base = smem_u32(empty_bar);
         for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
             const int split = item % p.ksplits, n_tile = item / p.ksplits;
             const int ks0 = split * p.ksteps_per_split;
@@ -349,7 +292,8 @@ wgrad_taps_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
                     mbar_expect_tx_s(fb, Cfg::STAGE_BYTES);
 #pragma unroll
                     for (int at = 0; at < Cfg::DY_ATOMS; ++at)
-                        tma_load_2d_s(dy_dst + at * (BK * 128), &tmDy, fb, n_tile * BLOCK_N + at * 64, k0);
+                        tma_load_2d_s(dy_dst + at * (BK * Cfg::DY_ROW), &tmDy, fb, n_tile * BLOCK_N + at * Cfg::DY_ATOM_CO,
+                                      k0);
 #pragma unroll
                     for (int tap = 0; tap < Cfg::NTAPS; ++tap)
                         tma_load_im2col_4d_s(x_dst + tap * Cfg::X_ATOM_BYTES, &tmX, fb, 0, qo * p.stride - p.pad,
@@ -367,89 +311,76 @@ wgrad_taps_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
                 }
             }
         }
-    } else if (warp == 1) {
-        int stage = 0;
-        uint32_t phase = 0, acc_phase = 0;
+    } else if (warp >= 4) {
+        const int wg = (warp - 4) >> 2;
+        const int tid_wg = (int)threadIdx.x & 127;
+        uint32_t stage = 0, phase = 0;
         const uint64_t adesc_base =
             smem_desc_base(Cfg::X_ATOM_BYTES, 8 * ROW_BYTES, swizzle_layout_type(ROW_BYTES));
-        const uint64_t bdesc_base = smem_desc_base(BK * 128, 8 * 128, swizzle_layout_type(128));
-        const uint32_t idesc = IDESC | p.idesc_ab;
+        const uint64_t bdesc_base = smem_desc_base(BK * Cfg::DY_ROW, 8 * Cfg::DY_ROW, swizzle_layout_type(Cfg::DY_ROW));
+        const float wscale = p.scale * (p.scale_ptr != nullptr ? __ldg(p.scale_ptr) : 1.f);
+        // this thread's fragment rows (see wgmma.cuh): M index 64 wg + frow (+ 8), columns fcol (+ 1) + 8 i
+        const int frow = 16 * (tid_wg >> 5) + ((tid_wg & 31) >> 2);
+        const int fcol = 2 * (tid_wg & 3);
         for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-            const int split = item % p.ksplits;
+            const int split = item % p.ksplits, n_tile = item / p.ksplits;
             const int ks0 = split * p.ksteps_per_split;
             const int ks1 = min(ks0 + p.ksteps_per_split, p.ksteps_total);
-            mbar_wait(tmem_empty_bar, acc_phase ^ 1);
-            tc_fence_after();
-            uint32_t accum = 0;
+            if (ks0 >= ks1) continue;
+            float acc[Cfg::GROUPS][BLOCK_N / 2];
+            uint32_t prev = 0;
             for (int ks = ks0; ks < ks1; ++ks) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t dy_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                    const uint32_t x_addr = dy_addr + Cfg::DY_BYTES;
+                mbar_wait_s(full_base + stage * 8, phase);
+                const uint32_t dy_addr = smem_base + stage * Cfg::STAGE_BYTES;
+                const uint32_t x_addr = dy_addr + Cfg::DY_BYTES + (uint32_t)(wg * (64 / Cfg::CIN) * Cfg::X_ATOM_BYTES);
+                wgmma_fence();
 #pragma unroll
-                    for (int g = 0; g < Cfg::GROUPS; ++g) {
+                for (int g = 0; g < Cfg::GROUPS; ++g) {
 #pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            const uint64_t adesc = smem_desc_at(
-                                adesc_base, x_addr + g * Cfg::TPG * Cfg::X_ATOM_BYTES + k * 16 * ROW_BYTES);
-                            const uint64_t bdesc = smem_desc_at(bdesc_base, dy_addr + k * 16 * 128);
-                            mma_f16_ss(tmem_base + (uint32_t)(g * BLOCK_N), adesc, bdesc, idesc, k > 0 ? 1u : accum);
-                        }
+                    for (int k = 0; k < BK / 16; ++k) {
+                        const uint64_t adesc = smem_desc_at(
+                            adesc_base, x_addr + g * Cfg::TPG * Cfg::X_ATOM_BYTES + k * 16 * ROW_BYTES);
+                        const uint64_t bdesc = smem_desc_at(bdesc_base, dy_addr + k * 16 * Cfg::DY_ROW);
+                        const uint32_t sc = (ks > ks0 || k > 0) ? 1u : 0u;
+                        wgmma_ss<BLOCK_N, BF16, 1>(acc[g], adesc, bdesc, sc);
                     }
-                    tc_commit(&empty_bar[stage]);
                 }
-                accum = 1;
+                wgmma_commit();
+                if (ks > ks0) {
+                    wgmma_wait<1>();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = stage;
                 if (++stage == NS) {
                     stage = 0;
                     phase ^= 1;
                 }
             }
-            if (elect_one()) tc_commit(tmem_full_bar);
-            acc_phase ^= 1;
-        }
-    } else if (warp >= 4) {
-        const int ew = warp - 4;
-        uint32_t acc_phase = 0;
-        const float wscale = p.scale * (p.scale_ptr != nullptr ? __ldg(p.scale_ptr) : 1.f);
-        const int m = ew * 32 + lane;
-        const int tap_local = m / Cfg::CIN, ci = m % Cfg::CIN;
-        for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-            const int split = item % p.ksplits, n_tile = item / p.ksplits;
-            const bool has_work = split * p.ksteps_per_split < p.ksteps_total;
-            mbar_wait(tmem_full_bar, acc_phase);
-            tc_fence_after();
-            const uint32_t taddr_row = tmem_base + ((uint32_t)(ew * 32) << 16);
-#pragma unroll 1
-            for (int g = 0; g < Cfg::GROUPS; ++g) {
-                const int tap = g * Cfg::TPG + tap_local;       // warp-uniform (a warp covers 32 channels of one tap)
-#pragma unroll 1
-                for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-                    uint32_t raw[32];
-                    tmem_ld_32x32(taddr_row + (uint32_t)(g * BLOCK_N + c0), raw);
-                    tc_wait_ld();
-                    if (has_work && tap < Cfg::NTAPS) {
-                        const int co0 = n_tile * BLOCK_N + c0;
-                        float* dst = p.dw + ((long long)co0 * Cfg::NTAPS + tap) * p.Cin + ci;
+            wgmma_wait<0>();
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (co0 + j < p.Cout)
-                                atomicAdd(dst + (long long)j * Cfg::NTAPS * p.Cin, __uint_as_float(raw[j]) * wscale);
+            for (int g = 0; g < Cfg::GROUPS; ++g) wgmma_fence_acc(acc[g]);
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            // D[(tap, ci)][co] -> dW[co][tap][ci]
+#pragma unroll
+            for (int g = 0; g < Cfg::GROUPS; ++g) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = 64 * wg + frow + 8 * h;
+                    const int tap = g * Cfg::TPG + m / Cfg::CIN, ci = m % Cfg::CIN;
+                    if (tap >= Cfg::NTAPS) continue;
+#pragma unroll
+                    for (int i = 0; i < BLOCK_N / 8; ++i) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int co = n_tile * BLOCK_N + 8 * i + fcol + e;
+                            if (co < p.Cout)
+                                atomicAdd(p.acc + ((long long)co * Cfg::NTAPS + tap) * p.Cin + ci,
+                                          (double)(acc[g][4 * i + 2 * h + e] * wscale));
+                        }
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmem_empty_bar);
-            acc_phase ^= 1;
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
     }
 }
 
@@ -464,7 +395,7 @@ typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32
 static PFN_encodeTiled w_encodeTiled = nullptr;
 static PFN_encodeIm2col w_encodeIm2col = nullptr;
 static int w_driver_version = 0;
-static int w_num_sms = 148;
+static int w_num_sms = 132;
 static std::once_flag w_once;
 
 static void w_resolve() {
@@ -494,7 +425,7 @@ static int wgrad_launch_cfg(const CUtensorMap& a, const CUtensorMap& b, const Wg
     }
     const int tiles = p.m_tiles * p.n_tiles * p.ntaps * p.ksplits;
     const int grid = tiles < w_num_sms ? tiles : w_num_sms;
-    kern<<<grid, 256, Cfg::SMEM_BYTES, st>>>(a, b, p);
+    kern<<<grid, 384, Cfg::SMEM_BYTES, st>>>(a, b, p);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }
@@ -502,14 +433,14 @@ static int wgrad_launch_cfg(const CUtensorMap& a, const CUtensorMap& b, const Wg
 template <int ROW_BYTES, int BLOCK_N>
 static int wgrad_taps_launch(const CUtensorMap& a, const CUtensorMap& b, const WgradParams& p, cudaStream_t st) {
     using Cfg = WgradTCfg<ROW_BYTES, BLOCK_N>;
-    auto kern = wgrad_taps_kernel<ROW_BYTES, BLOCK_N>;
-    static unsigned long long attr_set = 0;
-    if (b2y_first_use_on_device(attr_set)) {
+    auto kern = p.ab_bf16 ? wgrad_taps_kernel<ROW_BYTES, BLOCK_N, 1> : wgrad_taps_kernel<ROW_BYTES, BLOCK_N, 0>;
+    static unsigned long long attr_set[2] = {0, 0};
+    if (b2y_first_use_on_device(attr_set[p.ab_bf16 ? 1 : 0])) {
         B2Y_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     }
     const int items = p.n_tiles * p.ksplits;
     const int grid = items < w_num_sms ? items : w_num_sms;
-    kern<<<grid, 256, Cfg::SMEM_BYTES, st>>>(a, b, p);
+    kern<<<grid, 384, Cfg::SMEM_BYTES, st>>>(a, b, p);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }
@@ -535,8 +466,9 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
     int block_n, row_bytes;
     if (d->in_c % 64 == 0) {
         row_bytes = 128;
-        block_n = d->in_c >= 256 ? 256 : (d->in_c >= 128 ? 128 : 64);
-        if (d->in_c % block_n != 0 && d->in_c > block_n) block_n = 64;  // e.g. Cin = 192/320/384: 64-wide tiles
+        // at most 128 columns: the fp32 fragment of a 64 x 128 wgmma is 64 registers per thread
+        block_n = d->in_c >= 128 ? 128 : 64;
+        if (d->in_c % block_n != 0 && d->in_c > block_n) block_n = 64;  // e.g. Cin = 192/320: 64-wide tiles
     } else if (d->in_c % 32 == 0) {
         row_bytes = 64;
         block_n = 32;
@@ -567,8 +499,10 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
     p.ksteps_per_split = (p.ksteps_total + splits - 1) / splits;
     p.ksplits = (p.ksteps_total + p.ksteps_per_split - 1) / p.ksteps_per_split;
     p.scale = scale;
-    p.dw = dw;
-    p.idesc_ab = grad_dtype == B2Y_DT_BF16 ? ((1u << 7) | (1u << 10)) : 0u;
+    const long long dw_elems = (long long)d->out_c * p.ntaps * d->in_c;
+    p.acc = stream_acc(static_cast<cudaStream_t>(stream), dw_elems);
+    if (p.acc == nullptr) return B2Y_ERR_CUDA;
+    p.ab_bf16 = grad_dtype == B2Y_DT_BF16 ? 1 : 0;
     p.scale_ptr = inv_scale_ptr;
 
     CUtensorMap tmDy, tmX;
@@ -604,30 +538,44 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
         }
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc;
     static int taps_on = -1;        // B2Y_WGRAD_TAPS=0: narrow 3x3 layers use the general kernel as well
     if (taps_on < 0) {
         const char* ev = getenv("B2Y_WGRAD_TAPS");
         taps_on = (ev && atoi(ev) == 0) ? 0 : 1;
     }
     if (taps_on && d->ksize == 3 && (d->in_c == 32 || d->in_c == 64)) {
-        const int bn = (d->in_c == 32 && d->out_c > 64) ? 128 : 64;
+        const int bn = d->in_c == 32 ? 64 : 32;
+        CUtensorMap tmDyT = tmDy;
+        if (bn < 64) {
+            // a [64 pixels][32 channels] dY box, SWIZZLE_64B: the MN-major B operand of the N = 32 tiles
+            cuuint64_t gdim[2] = {(cuuint64_t)d->out_c, (cuuint64_t)K};
+            cuuint64_t gstride[1] = {(cuuint64_t)(d->out_pitch * 2)};
+            cuuint32_t box[2] = {(cuuint32_t)bn, 64};
+            cuuint32_t estr[2] = {1, 1};
+            if (w_encodeTiled(&tmDyT, grad_dtype == B2Y_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                              2, const_cast<void*>(dy), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+                return B2Y_ERR_DRIVER;
+        }
         p.n_tiles = (d->out_c + bn - 1) / bn;
         int sp = w_num_sms / p.n_tiles;
         if (sp < 1) sp = 1;
         if (sp > p.ksteps_total) sp = p.ksteps_total;
         p.ksteps_per_split = (p.ksteps_total + sp - 1) / sp;
         p.ksplits = (p.ksteps_total + p.ksteps_per_split - 1) / p.ksteps_per_split;
-        if (d->in_c == 32) return bn == 128 ? wgrad_taps_launch<64, 128>(tmDy, tmX, p, st)
-                                            : wgrad_taps_launch<64, 64>(tmDy, tmX, p, st);
-        return wgrad_taps_launch<128, 64>(tmDy, tmX, p, st);
+        rc = d->in_c == 32 ? wgrad_taps_launch<64, 64>(tmDyT, tmX, p, st) : wgrad_taps_launch<128, 32>(tmDyT, tmX, p, st);
+        if (rc != B2Y_OK) return rc;
+        return acc_finalize(p.acc, dw, dw_elems, st);
     }
-    if (row_bytes == 128) {
-        if (block_n == 256) return wgrad_launch_cfg<256, 128>(tmDy, tmX, p, st);
-        if (block_n == 128) return wgrad_launch_cfg<128, 128>(tmDy, tmX, p, st);
-        return wgrad_launch_cfg<64, 128>(tmDy, tmX, p, st);
-    }
-    if (row_bytes == 64) return wgrad_launch_cfg<32, 64>(tmDy, tmX, p, st);
-    return wgrad_launch_cfg<16, 32>(tmDy, tmX, p, st);
+    if (row_bytes == 128)
+        rc = block_n == 128 ? wgrad_launch_cfg<128, 128>(tmDy, tmX, p, st) : wgrad_launch_cfg<64, 128>(tmDy, tmX, p, st);
+    else
+        rc = row_bytes == 64 ? wgrad_launch_cfg<32, 64>(tmDy, tmX, p, st) : wgrad_launch_cfg<16, 32>(tmDy, tmX, p, st);
+    if (rc != B2Y_OK) return rc;
+    return acc_finalize(p.acc, dw, dw_elems, st);
 }
 
 // [O][kh][kw][I] fp32 -> OIHW fp32: dst = alpha*src (+ dst when accumulate)
@@ -653,7 +601,7 @@ extern "C" int b2y_unpack_wgrad(const float* dw_packed, float* dw_oihw, int out_
     if (!dw_packed || !dw_oihw || out_c <= 0 || in_c <= 0 || ksize <= 0) return B2Y_ERR_INVALID;
     const long long total = (long long)out_c * in_c * ksize * ksize;
     int grid = (int)((total + 255) / 256);
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > 132 * 16) grid = 132 * 16;
     unpack_wgrad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(dw_packed, dw_oihw, out_c, in_c, ksize,
                                                                                alpha, accumulate);
     B2Y_CUDA_CHECK(cudaGetLastError());
@@ -671,7 +619,7 @@ extern "C" int b2y_axpby_f32(const float* src, float* dst, long long n, float al
     if (!src || !dst || n < 0) return B2Y_ERR_INVALID;
     int grid = (int)((n + 255) / 256);
     if (grid < 1) grid = 1;
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > 132 * 16) grid = 132 * 16;
     axpby_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, dst, n, alpha, beta);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;

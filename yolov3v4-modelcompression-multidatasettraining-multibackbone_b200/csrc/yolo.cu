@@ -8,7 +8,7 @@ using namespace b2y;
 static inline int grid_for(long long n, int block) {
     long long g = (n + block - 1) / block;
     if (g < 1) g = 1;
-    if (g > 148LL * 32) g = 148LL * 32;
+    if (g > 132LL * 32) g = 132LL * 32;
     return (int)g;
 }
 
@@ -125,14 +125,14 @@ extern "C" int b2y_yolo_decode(const float* raw, long long raw_pitch, float* p, 
     if (per_pixel && na * no <= 256) {
         const long long pixels = (long long)batch * ny * nx;
         long long pb = (pixels + 7) / 8;
-        if (pb > 148 * 8) pb = 148 * 8;
+        if (pb > 132 * 8) pb = 132 * 8;
         yolo_decode_pixel_kernel<<<(int)pb, 256, 0, static_cast<cudaStream_t>(stream)>>>(
             raw, raw_pitch, p, io, total_rows, row_offset, batch, na, no, ny, nx, anchors_px, stride);
         B2Y_CUDA_CHECK(cudaGetLastError());
         return B2Y_OK;
     }
     long long blocks = (runs + 7) / 8;                 // 8 warps per block
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     yolo_decode_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         raw, raw_pitch, p, io, total_rows, row_offset, batch, na, no, ny, nx, anchors_px, stride);
     B2Y_CUDA_CHECK(cudaGetLastError());

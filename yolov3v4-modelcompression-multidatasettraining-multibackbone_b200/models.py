@@ -1,4 +1,4 @@
-"""Darknet(cfg) model API of the reference (models.py) on top of the B200-native engine.
+"""Darknet(cfg) model API of the reference (models.py) on top of the H100-native engine.
 
 Public surface kept from the reference (file:line are the reference's models.py):
     create_modules :11-347      YOLOLayer :350-437      Darknet :440-580      get_yolo_layers :583
@@ -9,7 +9,7 @@ Upsample / MaxPool2d / YOLOLayer), parameter names, state_dict keys and the Dark
 the reference's, so checkpoints, optimiser grouping (train.py:125-133) and the pruning scripts' indexing
 (module_list[i][0] / [1]) keep working.  What changes is *execution*: Darknet.forward does not walk the modules
 with ATen/cuDNN calls; it hands the graph to b200yolo.engine, which runs fused conv+BN+activation(+shortcut)
-tcgen05 kernels on NHWC fp16 activations and the fp32 YOLO decode kernel.
+wgmma kernels on NHWC fp16 activations and the fp32 YOLO decode kernel.
 """
 from utils.google_utils import *  # noqa: F401,F403
 from utils.parse_config import *  # noqa: F401,F403
@@ -294,7 +294,7 @@ class Darknet(nn.Module):
 
     def forward_once(self, x, augment=False, verbose=False):
         if not x.is_cuda:
-            raise RuntimeError("Darknet.forward runs on a CUDA (sm_100a) device only: the B200 engine has no CPU "
+            raise RuntimeError("Darknet.forward runs on a CUDA (sm_90a) device only: the H100 engine has no CPU "
                                "fallback. Move the model and the input to the GPU.")
         return self.engine().forward(x)
 

@@ -5,12 +5,12 @@ import time
 
 
 def gdrive_download(id='', name=''):
-    raise RuntimeError("gdrive_download(%r): network downloads are not part of the B200 hot path" % name)
+    raise RuntimeError("gdrive_download(%r): network downloads are not part of the H100 hot path" % name)
 
 
 def upload_blob(*a, **k):
-    raise RuntimeError("GCS upload is not part of the B200 hot path")
+    raise RuntimeError("GCS upload is not part of the H100 hot path")
 
 
 def download_blob(*a, **k):
-    raise RuntimeError("GCS download is not part of the B200 hot path")
+    raise RuntimeError("GCS download is not part of the H100 hot path")

@@ -2,7 +2,7 @@
 Mish :146 (analytic backward :117-128), Swish :141, ReLU6 :151, HardSwish :159, HardSigmoid :167, SE :176.
 
 These nn.Modules define the *graph* (class names are what Darknet.forward_once dispatches on, models.py:525-543)
-and hold parameters; on a CUDA device the whole graph is executed by the fused sm_100a engine
+and hold parameters; on a CUDA device the whole graph is executed by the fused sm_90a engine
 (b200yolo/engine.py), and the standalone activation modules call the CUDA kernels directly."""
 from utils.utils import *  # noqa: F401,F403  (the reference's star-import chain: torch, nn, F, np, math ...)
 

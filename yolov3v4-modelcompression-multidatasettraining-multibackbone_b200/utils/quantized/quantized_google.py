@@ -3,7 +3,7 @@ RangeTracker family :16-77, Round (STE) :81, Quantizer family :95-219, BNFold_Qu
 QuantizedShortcut_max/min :839/1066, QuantizedFeatureConcat :1305.
 
 The module forwards run on NHWC fp32 tensors (b200yolo/qat.py QatRunner drives them from Darknet.forward) and are
-composed of the sm_100a kernels: tcgen05 convolutions (forward / data gradient / weight gradient, fp32 accumulation,
+composed of the sm_90a kernels: wgmma convolutions (forward / data gradient / weight gradient, fp32 accumulation,
 BatchNorm channel sums from the conv epilogue), b2y_minmax_f32 (range trackers), b2y_fakequant_f32 with its
 straight-through backward, activation forward / backward.  torch.autograd chains them and differentiates the [C]-sized
 fold arithmetic (batch-statistics fold -> frozen running-statistics fold at 0.9 * steps, google.py:349-370).

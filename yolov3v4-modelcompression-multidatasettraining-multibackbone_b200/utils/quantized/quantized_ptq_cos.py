@@ -4,7 +4,7 @@
 
 The modules carry the same parameters / buffers (state_dict keys of a reference-calibrated PTQ.pt load unchanged);
 the calibrated eval forward of the whole graph is executed in true INT8 by b200yolo/qengine.py
-(tcgen05 kind::i8 convs, int32 accumulation, power-of-two rescale in the epilogue).
+(int8 wgmma convs, int32 accumulation, power-of-two rescale in the epilogue).
 """
 import math
 

@@ -1,4 +1,4 @@
-"""Loss slice of the reference's utils/utils.py under the same names, executed by the sm_100a kernels:
+"""Loss slice of the reference's utils/utils.py under the same names, executed by the sm_90a kernels:
 
     compute_loss(p, targets, model)   reference utils/utils.py:368-432
     build_targets(p, targets, model)  reference utils/utils.py:725-779
@@ -197,7 +197,7 @@ def compute_loss(p, targets, model):
         raise RuntimeError("compute_loss runs on the CUDA device only (no CPU fallback)")
     h = model.hyp
     if h.get('fl_gamma', 0) > 0:
-        raise NotImplementedError("focal loss (hyp['fl_gamma'] > 0) is not part of the fused sm_100a loss")
+        raise NotImplementedError("focal loss (hyp['fl_gamma'] > 0) is not part of the fused sm_90a loss")
     dev = p[0].device
     anchors = [_device_anchor_vec(m, dev) for m in _yolo_modules(model)]
     t = targets.to(dev).float()
