@@ -445,3 +445,8 @@ static inline int acc_finalize(double* acc, float* dst, long long n, cudaStream_
     B2Y_CUDA_CHECK(b2y::launch_pdl(acc_finalize_kernel<0>, dim3((unsigned)grid), dim3(256), 0, st, acc, dst, n));
     return B2Y_OK;
 }
+
+// stream_ws(st, n) returns an fp32 workspace (>= n floats, contents undefined) owned by the current device and stream
+// `st`, on the same terms as stream_acc: the weight gradient stores its split-K partial tiles there and reduces them in
+// a fixed order (wgrad_tc.cu).
+float* stream_ws(cudaStream_t st, long long n);

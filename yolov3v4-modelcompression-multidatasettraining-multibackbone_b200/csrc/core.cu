@@ -49,6 +49,38 @@ double* stream_acc(cudaStream_t st, long long n) {
     return a.ptr;
 }
 
+// ---- split-K partial tiles of the weight gradient (common.cuh: stream_ws) -------------------------------------------
+namespace {
+struct StreamWs {
+    float* ptr = nullptr;
+    long long n = 0;
+};
+std::mutex g_ws_mutex;
+std::map<std::pair<int, cudaStream_t>, StreamWs> g_ws;
+}  // namespace
+
+float* stream_ws(cudaStream_t st, long long n) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || n <= 0) return nullptr;
+    std::lock_guard<std::mutex> lock(g_ws_mutex);
+    StreamWs& w = g_ws[std::make_pair(dev, st)];
+    if (w.n >= n) return w.ptr;
+    // as in stream_acc: the replaced buffer stays allocated for graphs captured earlier, and the allocation is allowed
+    // during a (relaxed) capture.  No fill: every slice is written in full before it is read.
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, (size_t)n * sizeof(float));
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    if (e != cudaSuccess) {
+        b2y_set_last_cuda_error((int)e);
+        return nullptr;
+    }
+    w.ptr = static_cast<float*>(p);
+    w.n = n;
+    return w.ptr;
+}
+
 static thread_local int g_last_cuda_error = 0;
 
 extern "C" void b2y_set_last_cuda_error(int e) { g_last_cuda_error = e; }

@@ -5,8 +5,11 @@
 // Both operands are pixel-major in HBM (NHWC), i.e. "MN-major" for the tensor core: the TMA boxes
 // [64 pixels][64 channels] land in smem exactly as a 128B-swizzled MN-major wgmma operand, so neither
 // tensor is ever transposed or im2col'ed in memory.  dY comes through a tiled 2-D map, X through the im2col
-// map (tap offset + zero fill for the halo).  Work = (Cout/128) x (Cin/BLOCK_N) x taps x split-K slices;
-// the fp32 accumulator tile is reduced into dW with vector red.global.add.
+// map (tap offset + zero fill for the halo).  Work = (Cout/128) x (Cin/BLOCK_N) x taps x split-K slices.
+// With one slice the fp32 accumulator tile is added straight into dW (each element has one owner).  With S > 1 slices
+// every CTA stores its tile into slice `split` of a per-stream workspace, and wgrad_reduce_kernel then sums the S
+// partials of each element in double in a fixed order and adds the rounded total into dW: the result does not depend
+// on which CTA finishes first.
 #include "common.cuh"
 
 #include <mutex>
@@ -25,7 +28,8 @@ struct WgradParams {
     float scale;              // multiplies the accumulator (1 / loss-scale)
     int ab_bf16;              // both operands bf16 (else fp16; wgmma takes one 16-bit format for A and B)
     const float* scale_ptr;   // optional device scalar multiplied into `scale` (per-layer gradient un-scaling)
-    double* acc;              // [Cout][k][k][Cin] accumulator (stream_acc), added into dw by acc_finalize
+    float* out;               // ksplits == 1: dw (+=); else the workspace (stream_ws), slice s at out + s * slice
+    long long slice;          // Cout * k * k * Cin: one slice, laid out as dw [Cout][k][k][Cin]
 };
 
 template <int BLOCK_N, int NB_ROW_BYTES>
@@ -45,7 +49,7 @@ struct WgradCfg {
 };
 
 // warp 0: TMA producer; warps 4-11: two consumer warpgroups, warpgroup g owns output channels 64 g .. 64 g + 63 of the
-// tile (A atom g) and reduces its accumulator fragment straight from registers into dW.
+// tile (A atom g) and writes its accumulator fragment straight from registers (into dW or its workspace slice).
 template <int BLOCK_N, int NB_ROW_BYTES>
 __global__ void __launch_bounds__(384, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
@@ -185,18 +189,26 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant_
             wgmma_wait<0>();
             wgmma_fence_acc(acc);
             if (lane == 0) mbar_arrive(&empty_bar[prev]);
-            // fp32 partial sums -> dW[co][tap][ci], two adjacent channels per vector reduction
+            // fp32 partial sums -> [co][tap][ci] of dW or of the slice, two adjacent channels per thread (__fmul_rn: the
+            // product is rounded before it is added, whichever path takes it)
+            float* const out = p.out + split * p.slice;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int co = m_tile * 128 + frow + 8 * h;
                 if (co >= p.Cout) continue;
-                double* drow = p.acc + ((long long)co * p.ntaps + tap) * p.Cin;
+                float* orow = out + ((long long)co * p.ntaps + tap) * p.Cin;
 #pragma unroll
                 for (int i = 0; i < BLOCK_N / 8; ++i) {
                     const int ci = n_tile * BLOCK_N + 8 * i + fcol;
                     if (ci < p.Cin) {
-                        atomicAdd(drow + ci, (double)(acc[4 * i + 2 * h] * wscale));
-                        atomicAdd(drow + ci + 1, (double)(acc[4 * i + 2 * h + 1] * wscale));
+                        const float v0 = __fmul_rn(acc[4 * i + 2 * h], wscale);
+                        const float v1 = __fmul_rn(acc[4 * i + 2 * h + 1], wscale);
+                        if (p.ksplits == 1) {
+                            orow[ci] += v0;
+                            orow[ci + 1] += v1;
+                        } else {
+                            *reinterpret_cast<float2*>(orow + ci) = make_float2(v0, v1);
+                        }
                     }
                 }
             }
@@ -360,7 +372,9 @@ wgrad_taps_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
 #pragma unroll
             for (int g = 0; g < Cfg::GROUPS; ++g) wgmma_fence_acc(acc[g]);
             if (lane == 0) mbar_arrive(&empty_bar[prev]);
-            // D[(tap, ci)][co] -> dW[co][tap][ci]
+            // D[(tap, ci)][co] -> [co][tap][ci] of dW or of the slice: the 8 lanes of a fragment row hold 8 consecutive
+            // ci, so every store instruction writes whole 32-byte sectors
+            float* const out = p.out + split * p.slice;
 #pragma unroll
             for (int g = 0; g < Cfg::GROUPS; ++g) {
 #pragma unroll
@@ -373,15 +387,80 @@ wgrad_taps_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int co = n_tile * BLOCK_N + 8 * i + fcol + e;
-                            if (co < p.Cout)
-                                atomicAdd(p.acc + ((long long)co * Cfg::NTAPS + tap) * p.Cin + ci,
-                                          (double)(acc[g][4 * i + 2 * h + e] * wscale));
+                            if (co >= p.Cout) continue;
+                            float* o = out + ((long long)co * Cfg::NTAPS + tap) * p.Cin + ci;
+                            const float v = __fmul_rn(acc[g][4 * i + 2 * h + e], wscale);
+                            if (p.ksplits == 1)
+                                *o += v;
+                            else
+                                *o = v;
                         }
                     }
                 }
             }
         }
     }
+}
+
+// ---- fixed-order split-K reduction -----------------------------------------------------------------------------
+// dw[i] += (float) sum_{s < S} (double) ws[s * n + i].  A block is VB = 256 / G float4 columns x G groups of slices:
+// group g sums its contiguous slice range in ascending order, then group 0 adds the G partial sums in ascending g.  The
+// order is fixed by (S, G) alone, and while the double sum is exact (common.cuh) the result equals that of any other
+// order.  G > 1 keeps the serial chain per thread short for the layers with hundreds of slices but few dW elements.
+__global__ void __launch_bounds__(256)
+wgrad_reduce_kernel(const float* __restrict__ ws, float* __restrict__ dw, long long n, int S, int G, int dw_vec) {
+    __shared__ double part[256][4];
+    pdl_wait();
+    const int VB = 256 / G;
+    const int v = (int)threadIdx.x % VB, g = (int)threadIdx.x / VB;
+    const long long i = ((long long)blockIdx.x * VB + v) * 4;
+    const int per = (S + G - 1) / G;
+    const int s0 = g * per, s1 = min(S, s0 + per);
+    double a[4] = {0.0, 0.0, 0.0, 0.0};
+    if (i < n) {
+        const float* src = ws + i;
+#pragma unroll 4
+        for (int s = s0; s < s1; ++s) {
+            const float4 t = *reinterpret_cast<const float4*>(src + s * n);
+            a[0] += t.x;
+            a[1] += t.y;
+            a[2] += t.z;
+            a[3] += t.w;
+        }
+    }
+    if (G > 1) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) part[threadIdx.x][k] = a[k];
+        __syncthreads();
+        if (g != 0) return;
+        for (int q = 1; q < G; ++q)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) a[k] += part[q * VB + v][k];
+    }
+    if (i >= n) return;
+    if (dw_vec) {
+        float4* d = reinterpret_cast<float4*>(dw + i);
+        float4 t = *d;
+        t.x += (float)a[0];
+        t.y += (float)a[1];
+        t.z += (float)a[2];
+        t.w += (float)a[3];
+        *d = t;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) dw[i + k] += (float)a[k];
+    }
+}
+
+// n % 4 == 0 (Cin is a multiple of 16), so every slice starts 16-byte aligned
+static int wgrad_reduce(const float* ws, float* dw, long long n, int S, cudaStream_t st) {
+    int G = 1;
+    while (G < 32 && (S + G - 1) / G > 16) G *= 2;
+    const long long cols = 256 / G;
+    const long long grid = (n / 4 + cols - 1) / cols;
+    const int dw_vec = (reinterpret_cast<uintptr_t>(dw) & 15) == 0 ? 1 : 0;
+    B2Y_CUDA_CHECK(launch_pdl(wgrad_reduce_kernel, dim3((unsigned)grid), dim3(256), 0, st, ws, dw, n, S, G, dw_vec));
+    return B2Y_OK;
 }
 
 // ---- host ------------------------------------------------------------------------------------------------------
@@ -499,9 +578,7 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
     p.ksteps_per_split = (p.ksteps_total + splits - 1) / splits;
     p.ksplits = (p.ksteps_total + p.ksteps_per_split - 1) / p.ksteps_per_split;
     p.scale = scale;
-    const long long dw_elems = (long long)d->out_c * p.ntaps * d->in_c;
-    p.acc = stream_acc(static_cast<cudaStream_t>(stream), dw_elems);
-    if (p.acc == nullptr) return B2Y_ERR_CUDA;
+    p.slice = (long long)d->out_c * p.ntaps * d->in_c;
     p.ab_bf16 = grad_dtype == B2Y_DT_BF16 ? 1 : 0;
     p.scale_ptr = inv_scale_ptr;
 
@@ -544,9 +621,10 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
         const char* ev = getenv("B2Y_WGRAD_TAPS");
         taps_on = (ev && atoi(ev) == 0) ? 0 : 1;
     }
-    if (taps_on && d->ksize == 3 && (d->in_c == 32 || d->in_c == 64)) {
+    const bool taps = taps_on && d->ksize == 3 && (d->in_c == 32 || d->in_c == 64);
+    CUtensorMap tmDyT = tmDy;
+    if (taps) {
         const int bn = d->in_c == 32 ? 64 : 32;
-        CUtensorMap tmDyT = tmDy;
         if (bn < 64) {
             // a [64 pixels][32 channels] dY box, SWIZZLE_64B: the MN-major B operand of the N = 32 tiles
             cuuint64_t gdim[2] = {(cuuint64_t)d->out_c, (cuuint64_t)K};
@@ -566,16 +644,17 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
         if (sp > p.ksteps_total) sp = p.ksteps_total;
         p.ksteps_per_split = (p.ksteps_total + sp - 1) / sp;
         p.ksplits = (p.ksteps_total + p.ksteps_per_split - 1) / p.ksteps_per_split;
-        rc = d->in_c == 32 ? wgrad_taps_launch<64, 64>(tmDyT, tmX, p, st) : wgrad_taps_launch<128, 32>(tmDyT, tmX, p, st);
-        if (rc != B2Y_OK) return rc;
-        return acc_finalize(p.acc, dw, dw_elems, st);
     }
-    if (row_bytes == 128)
+    p.out = p.ksplits == 1 ? dw : stream_ws(st, p.ksplits * p.slice);
+    if (p.out == nullptr) return B2Y_ERR_CUDA;
+    if (taps)
+        rc = d->in_c == 32 ? wgrad_taps_launch<64, 64>(tmDyT, tmX, p, st) : wgrad_taps_launch<128, 32>(tmDyT, tmX, p, st);
+    else if (row_bytes == 128)
         rc = block_n == 128 ? wgrad_launch_cfg<128, 128>(tmDy, tmX, p, st) : wgrad_launch_cfg<64, 128>(tmDy, tmX, p, st);
     else
         rc = row_bytes == 64 ? wgrad_launch_cfg<32, 64>(tmDy, tmX, p, st) : wgrad_launch_cfg<16, 32>(tmDy, tmX, p, st);
     if (rc != B2Y_OK) return rc;
-    return acc_finalize(p.acc, dw, dw_elems, st);
+    return p.ksplits == 1 ? B2Y_OK : wgrad_reduce(p.out, dw, p.slice, p.ksplits, st);
 }
 
 // [O][kh][kw][I] fp32 -> OIHW fp32: dst = alpha*src (+ dst when accumulate)
