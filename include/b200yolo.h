@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define B2Y_ABI_VERSION 1
+#define B2Y_ABI_VERSION 2
 
 /* status codes */
 #define B2Y_OK 0
@@ -258,28 +258,13 @@ int b2y_stem_conv_fwd_q(const b2y_conv_desc* d, const float* x_nchw, const float
  * Training: BatchNorm (batch statistics), backward convolutions, optimiser
  * models.py:92-113 under autograd; train.py:135-151,437-459
  * ------------------------------------------------------------------------------------------------ */
-/* finalize: mean/var from sums, update running stats (momentum, unbiased var), emit scale/shift:
- *   scale = gamma*rsqrt(var_b+eps), shift = beta - mean*scale                         (models.py:100) */
-int b2y_bn_finalize(const float* stat_sum, const float* stat_sqsum, long long count, const float* gamma,
-                    const float* beta, float eps, float momentum, float* running_mean, float* running_var,
-                    float* save_mean, float* save_invstd, float* scale, float* shift, int c, void* stream);
-/* y = act(x*scale[c] + shift[c]) [+ residual]   fp16 NHWC in/out */
-int b2y_bn_act_fwd(const void* x, long long x_pitch, const float* scale, const float* shift, const void* residual,
-                   long long res_pitch, void* y, long long y_pitch, long long pixels, int c, int act, float slope,
-                   void* stream);
-/* backward of the above + BN:  given dy (grad wrt y), raw conv output x, recompute z = x*scale+shift,
- * dz = dy*act'(z); reduce dgamma = sum(dz*xhat), dbeta = sum(dz)  (pass 1), then
- * dx = (gamma*invstd) * (dz - dbeta/N - xhat*dgamma/N)                            (pass 2). */
+/* per-channel gradient reduce of y = act(x*scale[c] + shift[c]):  given dy (grad wrt y) and x, recompute
+ * z = x*scale+shift, du = dy*act'(z); dbeta = sum(du), dgamma = sum(du*xhat) with xhat = (x-mean)*invstd
+ * (mean / invstd optional: 0 / 1).  The BatchNorm layers of the conv stack use b2y_bn_train_bwd_reduce instead. */
 int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const void* dy, long long dy_pitch, const float* scale,
                           const float* shift, const float* save_mean, const float* save_invstd, float* dgamma,
                           float* dbeta, float* du_absmax /* optional: atomicMax of |du|, caller zeroes */,
                           long long pixels, int c, int act, float slope, int grad_dtype, void* stream);
-int b2y_bn_act_bwd_apply(const void* x, long long x_pitch, const void* dy, long long dy_pitch, const float* scale,
-                         const float* shift, const float* gamma, const float* save_mean, const float* save_invstd,
-                         const float* dgamma, const float* dbeta, void* dx /* fp16, times s */, long long dx_pitch,
-                         long long pixels, int c, int act, float slope, int grad_dtype /* of dy */,
-                         const float* du_absmax, float* scale_out /* [s, 1/s] chosen on the device, power of two */,
-                         void* stream);
 /* dX = conv_transpose(dY, W)   (data gradient; implicit GEMM on wgmma) */
 int b2y_conv2d_bwd_data(const b2y_conv_desc* d, const void* dy, const void* w_packed_t, void* dx, int accumulate,
                         int operand_dtype /* dY and weights */, int out_dtype /* dX */,

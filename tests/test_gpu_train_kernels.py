@@ -151,48 +151,6 @@ def test_conv_bwd_data_accumulate():
 
 
 @pytest.mark.parametrize("gdt", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
-@pytest.mark.parametrize("act", ["leaky", "mish", "linear"])
-def test_bn_act_fwd_bwd(act, gdt):
-    ops = _ops()
-    g = torch.Generator().manual_seed(3)
-    B, C, H, W = 4, 64, 12, 10
-    z = (torch.randn(B, C, H, W, generator=g) * 2 + 0.3).half().float()
-    gamma = torch.rand(C, generator=g) + 0.5
-    beta = torch.randn(C, generator=g) * 0.2
-    res = torch.randn(B, C, H, W, generator=g).half().float()
-    dy = torch.randn(B, C, H, W, generator=g).to(gdt).float()
-    rm, rv = torch.zeros(C), torch.ones(C)
-    # reference: torch BN (training) + activation + residual, autograd
-    zr = z.clone().double().requires_grad_(True)
-    gr, br = gamma.clone().double().requires_grad_(True), beta.clone().double().requires_grad_(True)
-    rm_r, rv_r = rm.clone().double(), rv.clone().double()
-    u = F.batch_norm(zr, rm_r, rv_r, gr, br, True, 0.1, 1e-5)
-    y = orc.activation(u, act) + res.double()
-    y.backward(dy.double())
-    # ours: statistics as the conv epilogue would deliver them
-    zn = _nhwc(z)
-    s1 = z.sum(dim=(0, 2, 3)).cuda()
-    s2 = (z * z).sum(dim=(0, 2, 3)).cuda()
-    rmc, rvc = rm.cuda(), rv.cuda()
-    mean, invstd, scale, shift = ops.bn_finalize(s1, s2, B * H * W, gamma.cuda(), beta.cuda(), 1e-5, 0.1, rmc, rvc)
-    out = ops.bn_act_fwd(zn, scale, shift, act, residual=_nhwc(res))
-    dz, dgamma, dbeta, aux = ops.bn_act_bwd(zn, _nhwc(dy, gdt), scale, shift, gamma.cuda(), mean, invstd, act)
-    s_dev, inv_dev = float(aux[1]), float(aux[2])
-    assert s_dev > 0 and abs(s_dev * inv_dev - 1.0) < 1e-6 and float(torch.log2(aux[1])) % 1.0 == 0.0
-    assert float(dz.float().abs().max()) <= 8192.0          # scaled into the fp16 sweet spot
-    dz = dz.float() * inv_dev
-    torch.cuda.synchronize()
-    assert (_nchw(out) - y.detach().float()).abs().max() < 6e-3
-    np.testing.assert_allclose(rmc.cpu().numpy(), rm_r.float().numpy(), rtol=1e-4, atol=1e-5)
-    np.testing.assert_allclose(rvc.cpu().numpy(), rv_r.float().numpy(), rtol=1e-4, atol=1e-5)
-    np.testing.assert_allclose(dgamma.cpu().numpy(), gr.grad.float().numpy(), rtol=2e-3, atol=2e-3)
-    np.testing.assert_allclose(dbeta.cpu().numpy(), br.grad.float().numpy(), rtol=2e-3, atol=2e-3)
-    ref_dz = zr.grad.float()
-    tol = 4e-3 if gdt == torch.float16 else 2e-2
-    assert (dz.permute(0, 3, 1, 2).cpu() - ref_dz).abs().max() < tol * max(1.0, ref_dz.abs().max().item())
-
-
-@pytest.mark.parametrize("gdt", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
 @pytest.mark.parametrize("act,C", [("leaky", 64), ("mish", 32), ("linear", 24), ("relu6", 40), ("h_swish", 72),
                                    ("mish", 512), ("leaky", 8)])
 def test_bn_train_fused_passes(act, C, gdt):

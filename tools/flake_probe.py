@@ -1,15 +1,14 @@
 """Diagnostic: repeat the yolov4 8x640x640 training step and compare every BatchNorm layer's dbeta / dgamma with sums
 recomputed from the engine's own dy and z (the layer-wise gate of tests/test_gpu_baseline_sizes.py, reduced to the BN
-parameter gradients).  Environment knobs are read once per process, so run one process per configuration:
+parameter gradients).
 
-    B2Y_PDL=0 python tools/flake_probe.py 4
+    python tools/flake_probe.py [iterations] [graph]
 
 Finding (an earlier run on another GPU generation; not re-measured on H100): deviations of 1e-3..3e-2 appear on the leaky-ReLU
-layers of the yolov4 neck in about a third of the iterations under EVERY configuration (PDL on / off, weight gradients on
-the side stream or not, TMA-store epilogue or not, eager or graph replay) and never on the Mish layers: they are elements
-with |u| below fp32 rounding, whose branch of the leaky-ReLU derivative differs between the engine's fma(z, scale, shift)
-and this script's ((z - mean) * invstd) * gamma + beta, and which change with the atomics' summation order of the batch
-statistics.  Not a race: the layer-wise gate now subtracts their worst-case contribution (tests/test_gpu_baseline_sizes.py).
+layers of the yolov4 neck in about a third of the iterations, eager or graph replay, and never on the Mish layers: they
+are elements with |u| below fp32 rounding, whose branch of the leaky-ReLU derivative differs between the engine's
+fma(z, scale, shift) and this script's ((z - mean) * invstd) * gamma + beta, and which change with the atomics' summation
+order of the batch statistics.  Not a race: the layer-wise gate now subtracts their worst-case contribution (tests/test_gpu_baseline_sizes.py).
 """
 import os
 import sys

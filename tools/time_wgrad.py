@@ -4,9 +4,6 @@ host cost of the call in the window).  Prints one JSON line: per shape the launc
 the kernel / split-K slices the host chooses, and the sum over the step.
 
     python tools/time_wgrad.py [--batch 8] [--reps 20]
-
-B2Y_WGRAD_TAPS=0 selects the general kernel for the narrow 3x3 layers too (read once per process), so compare two
-processes: python tools/time_wgrad.py; B2Y_WGRAD_TAPS=0 python tools/time_wgrad.py
 """
 import argparse
 import collections
@@ -20,10 +17,10 @@ import bench  # noqa: E402  (puts the package on sys.path; model builders)
 import torch  # noqa: E402
 
 
-def plan(d, sms, taps=True):
+def plan(d, sms):
     """(kernel, N tile width, split-K slices) that b2y_conv2d_bwd_weight chooses for descriptor d."""
     ksteps = -(-d.batch * d.out_h * d.out_w // 64)
-    if taps and d.ksize == 3 and d.in_c in (32, 64):
+    if d.ksize == 3 and d.in_c in (32, 64):
         bn = 64 if d.in_c == 32 else 32
         sp = min(max(1, sms // -(-d.out_c // bn)), ksteps)
         kern = "taps"
@@ -72,7 +69,6 @@ def main():
         shapes.setdefault(key, []).append(a)
     fn = getattr(lib.raw(), "b2y_conv2d_bwd_weight")
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    taps = os.environ.get("B2Y_WGRAD_TAPS", "1") != "0"
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     rows, total_ms, total_flops = [], 0.0, 0.0
     for key, arglist in shapes.items():
@@ -93,7 +89,7 @@ def main():
         ms = e0.elapsed_time(e1) / args.reps
         del g
         flops = bench.conv_desc_flops("b2y_conv2d_bwd_weight", a)
-        kern, bn, splits = plan(a[0]._obj, sms, taps)
+        kern, bn, splits = plan(a[0]._obj, sms)
         k, s, ci, co, h, w, ho, wo = key
         rows.append({"shape": "%dx%d s%d %d->%d in %dx%d out %dx%d" % (k, k, s, ci, co, h, w, ho, wo),
                      "n": len(arglist), "ms": ms, "tflops": flops / ms / 1e9, "kernel": kern, "block_n": bn,
@@ -101,7 +97,7 @@ def main():
         total_ms += ms * len(arglist)
         total_flops += flops * len(arglist)
     rows.sort(key=lambda r: -r["ms"] * r["n"])
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "batch": args.batch, "taps": taps,
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "batch": args.batch,
                       "launches_per_step": len(calls), "ms_per_step": total_ms,
                       "tflops": total_flops / total_ms / 1e9, "shapes": rows}))
 

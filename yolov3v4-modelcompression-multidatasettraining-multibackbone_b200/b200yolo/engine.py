@@ -392,8 +392,7 @@ class Plan:
                 if src is None:
                     if conv.in_channels > 4:
                         raise NotImplementedError("first layer with more than 4 input channels")
-                    if wstem is not None and wstem.dim() == 2 and conv.out_channels <= 64 and \
-                            os.environ.get('B2Y_STEM', 'fused') == 'fused':
+                    if wstem is not None and wstem.dim() == 2 and conv.out_channels <= 64:
                         # full-im2col weight layout: the fused kernel builds the A tile in smem (no workspace)
                         ops.stem_conv_fused(x, wstem, bias, k, s, p, act=act, slope=slope, out=out.view(),
                                             x_div=256.0 if x.dtype == torch.uint8 else 1.0)

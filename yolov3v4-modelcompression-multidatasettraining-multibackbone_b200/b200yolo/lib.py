@@ -104,10 +104,7 @@ _PROTOS = {
     "b2y_requant_i8": (i32, [vp, ll, vp, ll, ll, i32, f32, f32, f32, f32, vp]),
     "b2y_upsample_nearest_i8": (i32, [vp, ll, vp, ll, i32, i32, i32, i32, i32, vp]),
     "b2y_stem_conv_fwd_q": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, f32, f32, f32, vp]),
-    "b2y_bn_finalize": (i32, [vp, vp, ll, vp, vp, f32, f32, vp, vp, vp, vp, vp, vp, i32, vp]),
-    "b2y_bn_act_fwd": (i32, [vp, ll, vp, vp, vp, ll, vp, ll, ll, i32, i32, f32, vp]),
     "b2y_bn_act_bwd_reduce": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, vp, vp, vp, ll, i32, i32, f32, i32, vp]),
-    "b2y_bn_act_bwd_apply": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, vp, vp, vp, vp, ll, ll, i32, i32, f32, i32, vp, vp, vp]),
     "b2y_conv2d_bwd_data": (i32, [C.POINTER(ConvDesc), vp, vp, vp, i32, i32, i32, vp, vp]),
     "b2y_pack_dgrad_weights": (i32, [C.POINTER(ConvDesc), vp, vp, i32, vp]),
     "b2y_conv2d_bwd_weight": (i32, [C.POINTER(ConvDesc), vp, vp, vp, f32, i32, vp, vp]),

@@ -327,48 +327,6 @@ def axpby(src, dst, alpha=1.0, beta=0.0):
     return dst
 
 
-def bn_finalize(s1, s2, count, gamma, beta, eps, momentum, running_mean, running_var):
-    Cn = s1.numel()
-    dev = s1.device
-    mean, invstd, scale, shift = [torch.empty(Cn, dtype=torch.float32, device=dev) for _ in range(4)]
-    call("b2y_bn_finalize", ptr(s1), ptr(s2), int(count), ptr(gamma), ptr(beta), float(eps), float(momentum),
-         ptr(running_mean), ptr(running_var), ptr(mean), ptr(invstd), ptr(scale), ptr(shift), Cn, stream_ptr())
-    return mean, invstd, scale, shift
-
-
-def bn_act_fwd(x, scale, shift, act, slope=0.1, residual=None, out=None):
-    B, H, W, Cc = x.shape
-    if out is None:
-        out = torch.empty((B, H, W, Cc), dtype=torch.float16, device=x.device)
-    call("b2y_bn_act_fwd", ptr(x), _pitch(x), ptr(scale), ptr(shift), ptr(residual),
-         _pitch(residual) if residual is not None else 0, ptr(out), _pitch(out), B * H * W, Cc,
-         ACT[act] if isinstance(act, str) else int(act), float(slope), stream_ptr())
-    return out
-
-
-def bn_act_bwd(x, dy, scale, shift, gamma, mean, invstd, act, slope=0.1, dx=None, dgamma=None, dbeta=None, aux=None):
-    """Backward of y = act(x*scale+shift) with batch statistics.
-    Returns (dz fp16 = s * true gradient, dgamma fp32, dbeta fp32, aux) where aux = device float[3]
-    [max|du|, s, 1/s]: the power-of-two scale s is chosen inside the kernel (no host sync)."""
-    B, H, W, Cc = x.shape
-    dev = x.device
-    if dgamma is None:
-        dgamma = torch.zeros(Cc, dtype=torch.float32, device=dev)
-        dbeta = torch.zeros(Cc, dtype=torch.float32, device=dev)
-    if aux is None:
-        aux = torch.zeros(3, dtype=torch.float32, device=dev)
-    a = ACT[act] if isinstance(act, str) else int(act)
-    call("b2y_bn_act_bwd_reduce", ptr(x), _pitch(x), ptr(dy), _pitch(dy), ptr(scale), ptr(shift), ptr(mean),
-         ptr(invstd), ptr(dgamma), ptr(dbeta), ptr(aux), B * H * W, Cc, a, float(slope), _gdt(dy), stream_ptr())
-    if dx is None:
-        dx = torch.empty((B, H, W, Cc), dtype=torch.float16, device=dev)
-    assert dx.dtype == torch.float16
-    call("b2y_bn_act_bwd_apply", ptr(x), _pitch(x), ptr(dy), _pitch(dy), ptr(scale), ptr(shift), ptr(gamma), ptr(mean),
-         ptr(invstd), ptr(dgamma), ptr(dbeta), ptr(dx), _pitch(dx), B * H * W, Cc, a, float(slope), _gdt(dy),
-         ptr(aux), C.c_void_p(aux.data_ptr() + 4), stream_ptr())
-    return dx, dgamma, dbeta, aux
-
-
 def bn_train_fwd(z, s1, s2, gamma, beta, eps, momentum, running_mean, running_var, act, slope=0.1, residual=None,
                  out=None, save=None):
     """Fused finalize + apply of training-mode BatchNorm (csrc/bn_train.cu). Returns (y, save[4][C])."""

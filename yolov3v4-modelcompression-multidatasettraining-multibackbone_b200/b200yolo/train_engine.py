@@ -2,7 +2,7 @@
 
 Replaces autograd over ~500 ATen/cuDNN calls (reference train.py:380-441 -> models.py:508-551) by a static plan:
 
-  forward   conv (wgmma, per-channel sum / sum^2 from the epilogue) -> bn_finalize -> bn+act(+shortcut) apply
+  forward   conv (wgmma, per-channel sum / sum^2 from the epilogue) -> BatchNorm finalize + act(+shortcut) apply
   backward  yolo permute^T -> [bn+act backward reduce / apply -> wgrad (wgmma, pixel-K GEMM) -> dgrad (wgmma)]
 
 Activations z (raw conv output) and y (post activation) are kept in NHWC fp16 (accurate forward).  Gradients w.r.t.
@@ -42,8 +42,8 @@ def _widen(view, channels):
 
 class _ConvRec:
     __slots__ = ('i', 'conv', 'bn', 'act', 'slope', 'src', 'z', 'y', 'res', 'head', 'stem', 'k', 's', 'p', 'Cout',
-                 'Cpad', 'w16', 'wT', 'stats', 'mean', 'invstd', 'scale', 'shift', 'ones', 'zeros', 'w32', 'aux_row', 'wstem',
-                 'save', 'sums', 'dw', 'fast_bn', 'depthwise', 'Ipad', 'dwg')
+                 'Cpad', 'w16', 'wT', 'stats', 'ones', 'zeros', 'w32', 'aux_row', 'wstem', 'save', 'sums', 'dw',
+                 'depthwise', 'Ipad', 'dwg')
 
     def __init__(self):
         for k in self.__slots__:
@@ -224,11 +224,14 @@ class TrainPlan:
                     l = defs[i + 1]['from'][0]
                     r.res = tens[i + 1 + l if l < 0 else l]
                 if bn is not None:
+                    # csrc/bn_train.cu: a thread owns 8 channels, a CTA of 256 threads at least one pixel row
+                    if r.Cout % 8 != 0 or r.Cout > 2048:
+                        raise NotImplementedError("layer %d: BatchNorm training needs a multiple of 8 channels, at most "
+                                                  "2048 (got %d)" % (i, r.Cout))
                     r.z = _Tensor(r.Cout, r.y.H, r.y.W)
                     r.z.buf = new_buf(r.Cout, r.y.H, r.y.W)
                     r.stats = zeros_later((2, r.Cout), torch.float32)
                     r.sums = zeros_later((2, r.Cout), torch.float32)
-                    r.fast_bn = r.Cout % 8 == 0 and r.Cout // 8 <= 256
                 else:
                     r.z = r.y   # no BN: the conv epilogue applies bias + activation directly
                     r.ones = torch.ones(r.Cpad, dtype=torch.float32, device=dev)
@@ -332,15 +335,11 @@ class TrainPlan:
                 r.save = torch.empty((4, r.Cout), dtype=torch.float32, device=dev)
         # The weight gradients hang off the critical path (dz_i -> dW_i has no consumer until the optimiser), so they run
         # on a second stream concurrently with the data-gradient / BatchNorm chain.  dz is therefore kept per layer
-        # (no buffer shared between a running wgrad and the next layer's BN backward); B2Y_WGRAD_STREAM=0 serialises.
-        self.side_wgrad = os.environ.get('B2Y_WGRAD_STREAM', '1') != '0'
+        # (no buffer shared between a running wgrad and the next layer's BN backward).
         self.dz_bufs = {}
-        if not self.side_wgrad:
-            maxz = max(r.Cpad * r.y.H * r.y.W for r in self.convs)
-            self.dz_scratch = torch.empty(B * maxz, dtype=torch.float16, device=dev)
         self.side_stream = None
         maxc = max(r.Cpad for r in self.convs)
-        self.dgb_scratch = torch.empty((2, maxc), dtype=torch.float32, device=dev)
+        self.db_scratch = torch.empty(maxc, dtype=torch.float32, device=dev)
         self.stem_dw = torch.empty(maxc * 32, dtype=torch.float32, device=dev)
         self.params = [p for p in model.parameters()]
         # plan-owned gradient outputs for the plain-autograd path (no flat sink): OIHW fp32 per parameter
@@ -402,16 +401,15 @@ class TrainPlan:
         when the plan is built: it OVERWRITES (dgrad accumulate=False, copy instead of add) and the buffer leaves the
         zeroed arena.  A buffer stays 'dirty' (zeroed, accumulate-only) when a first writer cannot overwrite (up-sample /
         max-pool / depthwise / SE backward, stride > kernel dgrad), when ranges overlap partially, or when something would
-        read channels nobody has written.  B2Y_GRAD_FIRSTWRITE=0 keeps every buffer dirty."""
+        read channels nobody has written."""
         self.first_write, cov, dirty = {}, {}, set()
         G = lambda t: self.grad_of[id(t)]
-        enabled = os.environ.get('B2Y_GRAD_FIRSTWRITE', '1') != '0'
 
         def write(g, n, key, can_overwrite):
             b, R = id(g.buf), set(range(g.c0, g.c0 + n))
             c = cov.setdefault(b, set())
             inter = R & c
-            if not inter and can_overwrite and enabled:
+            if not inter and can_overwrite:
                 self.first_write[key] = True
             else:
                 self.first_write[key] = False
@@ -635,19 +633,12 @@ class TrainPlan:
         bn = r.bn
         count = z.shape[0] * z.shape[1] * z.shape[2]
         res = r.res.view() if r.res is not None else None
-        if r.fast_bn:
-            y = r.y.view()
-            call("b2y_bn_train_fwd", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
-                 ptr(bn.weight.detach()), ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum),
-                 ptr(bn.running_mean), ptr(bn.running_var), ptr(r.save), ptr(res),
-                 ops._pitch(res) if res is not None else 0, ptr(y), ops._pitch(y), int(count), r.Cout,
-                 ACT[r.act], float(r.slope), stream_ptr())
-            r.mean, r.invstd, r.scale, r.shift = r.save[0], r.save[1], r.save[2], r.save[3]
-            return
-        r.mean, r.invstd, r.scale, r.shift = ops.bn_finalize(r.stats[0], r.stats[1], count, bn.weight.detach(),
-                                                             bn.bias.detach(), bn.eps, bn.momentum, bn.running_mean,
-                                                             bn.running_var)
-        ops.bn_act_fwd(z, r.scale, r.shift, r.act, r.slope, residual=res, out=r.y.view())
+        y = r.y.view()
+        call("b2y_bn_train_fwd", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
+             ptr(bn.weight.detach()), ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum),
+             ptr(bn.running_mean), ptr(bn.running_var), ptr(r.save), ptr(res),
+             ops._pitch(res) if res is not None else 0, ptr(y), ops._pitch(y), int(count), r.Cout,
+             ACT[r.act], float(r.slope), stream_ptr())
 
     # ---------------------------------------------------------------------------------------------------------
     def backward(self, dps):
@@ -659,7 +650,7 @@ class TrainPlan:
         self.sink = getattr(self.model, '_b2y_grad_sink', None)   # FlatDataParallel: write into the flat buffer
         # one memset: BN sums, scale rows, packed weight gradients and the activation gradients that are accumulate-only
         self.bwd_arena[:max(self.bwd_zero_bytes, 1)].zero_()
-        if self.side_wgrad and self.side_stream is None:
+        if self.side_stream is None:
             self.side_stream = torch.cuda.Stream(device=self.device)
         grads = {}
         # head gradients are GEMM operands (fp16): scale them by a power of two derived on the device from max|dp|
@@ -714,8 +705,7 @@ class TrainPlan:
                 gy, gx, xv = G(out).view(), G(src).view(), src.view()
                 call("b2y_maxpool_bwd", ptr(xv), ops._pitch(xv), ptr(gy), ops._pitch(gy), ptr(gx), ops._pitch(gx),
                      self.B, src.H, src.W, src.C, int(k), int(s), 1 if tiny else 0, ops._gdt(gy), stream_ptr())
-        if self.side_wgrad:
-            torch.cuda.current_stream().wait_stream(self.side_stream)      # join: every weight gradient is complete
+        torch.cuda.current_stream().wait_stream(self.side_stream)          # join: every weight gradient is complete
         self._unpack_all()
         if self.own_grads:
             # plain-autograd path: hand out copies (the plan-owned buffers are overwritten by the next step)
@@ -737,42 +727,29 @@ class TrainPlan:
                     ops.copy_channels(dy, gs)
                 else:
                     ops.add(gs, dy, out=gs)
-            if self.side_wgrad:
-                dz = self.dz_bufs.get(r.i)
-                if dz is None:
-                    # pitch = Cout rounded up to the K granule of the data-gradient GEMM; the pad channels stay zero
-                    full = torch.zeros((B, Ho, Wo, r.Cpad), dtype=torch.float16, device=self.device)
-                    dz = self.dz_bufs[r.i] = full[..., :r.Cout]
-            else:
-                if r.Cpad != r.Cout:
-                    raise NotImplementedError("B2Y_WGRAD_STREAM=0 needs channel counts that are multiples of 16")
-                dz = self.dz_scratch[:B * Ho * Wo * r.Cout].view(B, Ho, Wo, r.Cout)
+            dz = self.dz_bufs.get(r.i)
+            if dz is None:
+                # pitch = Cout rounded up to the K granule of the data-gradient GEMM; the pad channels stay zero
+                full = torch.zeros((B, Ho, Wo, r.Cpad), dtype=torch.float16, device=self.device)
+                dz = self.dz_bufs[r.i] = full[..., :r.Cout]
             aux = self.dz_aux[r.aux_row]
             inv_s = aux[2:3]                                   # device scalar 1/s of this layer's dz
-            if r.fast_bn:
-                z = r.z.view()
-                pixels = B * Ho * Wo
-                a = ACT[r.act]
-                call("b2y_bn_train_bwd_reduce", ptr(z), ops._pitch(z), ptr(dy), ops._pitch(dy), ptr(r.save),
-                     ptr(r.sums), ptr(aux), pixels, r.Cout, a, float(r.slope), ops._gdt(dy), stream_ptr())
-                call("b2y_bn_train_bwd_apply", ptr(z), ops._pitch(z), ptr(dy), ops._pitch(dy),
-                     ptr(bn.weight.detach()), ptr(r.save), ptr(r.sums), ptr(dz), ops._pitch(dz), pixels, r.Cout, a,
-                     float(r.slope), ops._gdt(dy), ptr(aux), C.c_void_p(aux.data_ptr() + 4),
-                     ptr(self._grad_dst(bn.weight)), ptr(self._grad_dst(bn.bias)), float(inv), stream_ptr())
-            else:
-                dgb = self.dgb_scratch[:, :r.Cout]
-                dgb.zero_()
-                ops.bn_act_bwd(r.z.view(), dy, r.scale, r.shift, bn.weight.detach(), r.mean, r.invstd, r.act, r.slope,
-                               dx=dz, dgamma=dgb[0], dbeta=dgb[1], aux=aux)
-                self._emit(grads, bn.weight, dgb[0], inv)
-                self._emit(grads, bn.bias, dgb[1], inv)
+            z = r.z.view()
+            pixels = B * Ho * Wo
+            a = ACT[r.act]
+            call("b2y_bn_train_bwd_reduce", ptr(z), ops._pitch(z), ptr(dy), ops._pitch(dy), ptr(r.save),
+                 ptr(r.sums), ptr(aux), pixels, r.Cout, a, float(r.slope), ops._gdt(dy), stream_ptr())
+            call("b2y_bn_train_bwd_apply", ptr(z), ops._pitch(z), ptr(dy), ops._pitch(dy),
+                 ptr(bn.weight.detach()), ptr(r.save), ptr(r.sums), ptr(dz), ops._pitch(dz), pixels, r.Cout, a,
+                 float(r.slope), ops._gdt(dy), ptr(aux), C.c_void_p(aux.data_ptr() + 4),
+                 ptr(self._grad_dst(bn.weight)), ptr(self._grad_dst(bn.bias)), float(inv), stream_ptr())
         else:
             dz = gy.buf[..., :r.Cpad] if r.head else gy.view()
             inv_s = self.head_scale[1:2]
             if r.act != 'linear':
                 raise NotImplementedError("activation without BatchNorm in training")
             if conv.bias is not None:
-                db = self.dgb_scratch[1, :r.Cpad]
+                db = self.db_scratch[:r.Cpad]
                 db.zero_()
                 ops.bias_act_bwd_reduce(dz, dz, r.ones, r.zeros, 'linear', dbeta=db)
                 self._emit(grads, conv.bias, db[:r.Cout] * inv_s, inv)
@@ -804,12 +781,8 @@ class TrainPlan:
             # K operands are taken with their zero pad: x with Ipad channels, dz with Cpad channels.
             xk = r.src.view_k()
             dzk = dz if dz.shape[3] == r.Cpad else _widen(dz, r.Cpad)
-            if self.side_wgrad:
-                main = torch.cuda.current_stream()
-                self.side_stream.wait_stream(main)              # dz (and 1/s) of this layer are complete
-                with torch.cuda.stream(self.side_stream):
-                    ops.conv2d_bwd_weight(xk, dzk, r.k, r.s, r.p, scale=inv, dw=r.dw, inv_scale=inv_s)
-            else:
+            self.side_stream.wait_stream(torch.cuda.current_stream())   # dz (and 1/s) of this layer are complete
+            with torch.cuda.stream(self.side_stream):
                 ops.conv2d_bwd_weight(xk, dzk, r.k, r.s, r.p, scale=inv, dw=r.dw, inv_scale=inv_s)
             gx = self.grad_of[id(r.src)]
             ops.conv2d_bwd_data(dzk, r.wT, (B, r.src.H, r.src.W, I), r.k, r.s, r.p, out=gx.view(),

@@ -66,7 +66,7 @@ bn_train_fwd_kernel(const __half* __restrict__ z, long long zp, const float* __r
                     const float* __restrict__ s2, const float* __restrict__ gamma, const float* __restrict__ beta,
                     float count, float eps, float momentum, float* __restrict__ rmean, float* __restrict__ rvar,
                     float* __restrict__ save, const __half* __restrict__ res, long long rp, __half* __restrict__ y,
-                    long long yp, long long pixels, int CV, int PPB, int act_rt, float slope, int pf) {
+                    long long yp, long long pixels, int CV, int PPB, int act_rt, float slope) {
     pdl_wait();                     // launched as a programmatic dependent (launch_pdl): the statistics / z come from
     pdl_launch_dependents();        // the previous kernel
     const int tid = threadIdx.x;
@@ -106,7 +106,7 @@ bn_train_fwd_kernel(const __half* __restrict__ z, long long zp, const float* __r
                 if (res != nullptr) r[u] = __ldg(reinterpret_cast<const uint4*>(res + pix * rp) + cv);
             }
             const long long nxt = pix + stride * U;
-            if (pf && nxt < pixels) {
+            if (nxt < pixels) {
                 prefetch_l2(reinterpret_cast<const uint4*>(z + nxt * zp) + cv);
                 if (res != nullptr) prefetch_l2(reinterpret_cast<const uint4*>(res + nxt * rp) + cv);
             }
@@ -142,7 +142,7 @@ template <typename GT, int ACT, int U>
 __global__ void __launch_bounds__(256, 2)
 bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT* __restrict__ dy, long long dp,
                            const float* __restrict__ save, double* __restrict__ sums, float* __restrict__ du_absmax,
-                           long long pixels, int CV, int PPB, int act_rt, float slope, int pf) {
+                           long long pixels, int CV, int PPB, int act_rt, float slope) {
     __shared__ float red[256][17];
     pdl_wait();
     pdl_launch_dependents();
@@ -172,7 +172,7 @@ bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT*
                     g[u] = __ldg(reinterpret_cast<const uint4*>(dy + pix * dp) + cv);
                 }
                 const long long nxt = pix + stride * U;
-                if (pf && nxt < pixels) {
+                if (nxt < pixels) {
                     prefetch_l2(reinterpret_cast<const uint4*>(z + nxt * zp) + cv);
                     prefetch_l2(reinterpret_cast<const uint4*>(dy + nxt * dp) + cv);
                 }
@@ -230,7 +230,7 @@ bn_train_bwd_apply_kernel(const __half* __restrict__ z, long long zp, const GT* 
                           const float* __restrict__ sums, __half* __restrict__ dz, long long dzp, long long pixels,
                           int CV, int PPB, int act_rt, float slope, const float* __restrict__ du_absmax,
                           float* __restrict__ scale_out, float* __restrict__ dgamma_out,
-                          float* __restrict__ dbeta_out, float grad_out_scale, int pf) {
+                          float* __restrict__ dbeta_out, float grad_out_scale) {
     pdl_wait();
     pdl_launch_dependents();
     const int C = CV * 8;
@@ -294,7 +294,7 @@ bn_train_bwd_apply_kernel(const __half* __restrict__ z, long long zp, const GT* 
                 g[u] = __ldg(reinterpret_cast<const uint4*>(dy + pix * dp) + cv);
             }
             const long long nxt = pix + stride * U;
-            if (pf && nxt < pixels) {
+            if (nxt < pixels) {
                 prefetch_l2(reinterpret_cast<const uint4*>(z + nxt * zp) + cv);
                 prefetch_l2(reinterpret_cast<const uint4*>(dy + nxt * dp) + cv);
             }
@@ -326,15 +326,6 @@ inline void dispatch_act(int act, F&& f) {
     else f(std::integral_constant<int, ACT_RT>{});
 }
 
-inline int bn_prefetch() {       // B2Y_BN_PREFETCH=0: no L2 prefetch one iteration ahead
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("B2Y_BN_PREFETCH");
-        v = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    return v;
-}
-
 inline bool shape_ok(int c, long long p0, long long p1, long long p2 = 8) {
     return c > 0 && c % 8 == 0 && c / 8 <= 256 && p0 % 8 == 0 && p1 % 8 == 0 && p2 % 8 == 0;
 }
@@ -355,7 +346,7 @@ extern "C" int b2y_bn_train_fwd(const void* z, long long z_pitch, const float* s
         launch_pdl(bn_train_fwd_kernel<decltype(A)::value, 4>, dim3(grid), dim3(256), 0, st, 
             reinterpret_cast<const __half*>(z), z_pitch, stat_sum, stat_sqsum, gamma, beta, (float)count, eps, momentum,
             running_mean, running_var, save, reinterpret_cast<const __half*>(residual), res_pitch,
-            reinterpret_cast<__half*>(y), y_pitch, pixels, g.CV, g.PPB, act, slope, bn_prefetch());
+            reinterpret_cast<__half*>(y), y_pitch, pixels, g.CV, g.PPB, act, slope);
     });
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
@@ -376,11 +367,11 @@ extern "C" int b2y_bn_train_bwd_reduce(const void* z, long long z_pitch, const v
         if (grad_dtype == B2Y_DT_BF16)
             launch_pdl(bn_train_bwd_reduce_kernel<__nv_bfloat16, ACT, 4>, dim3(grid), dim3(256), 0, st, 
                 reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, save,
-                acc, du_absmax, pixels, g.CV, g.PPB, act, slope, bn_prefetch());
+                acc, du_absmax, pixels, g.CV, g.PPB, act, slope);
         else
             launch_pdl(bn_train_bwd_reduce_kernel<__half, ACT, 4>, dim3(grid), dim3(256), 0, st, 
                 reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, save, acc,
-                du_absmax, pixels, g.CV, g.PPB, act, slope, bn_prefetch());
+                du_absmax, pixels, g.CV, g.PPB, act, slope);
     });
     B2Y_CUDA_CHECK(cudaGetLastError());
     return acc_finalize(acc, sums, 2LL * c, st);
@@ -402,12 +393,12 @@ extern "C" int b2y_bn_train_bwd_apply(const void* z, long long z_pitch, const vo
             launch_pdl(bn_train_bwd_apply_kernel<__nv_bfloat16, ACT, 4>, dim3(grid), dim3(256), 0, st, 
                 reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, gamma,
                 save, sums, reinterpret_cast<__half*>(dz), dz_pitch, pixels, g.CV, g.PPB, act, slope, du_absmax,
-                scale_out, dgamma_out, dbeta_out, grad_out_scale, bn_prefetch());
+                scale_out, dgamma_out, dbeta_out, grad_out_scale);
         else
             launch_pdl(bn_train_bwd_apply_kernel<__half, ACT, 4>, dim3(grid), dim3(256), 0, st, 
                 reinterpret_cast<const __half*>(z), z_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, gamma, save,
                 sums, reinterpret_cast<__half*>(dz), dz_pitch, pixels, g.CV, g.PPB, act, slope, du_absmax, scale_out,
-                dgamma_out, dbeta_out, grad_out_scale, bn_prefetch());
+                dgamma_out, dbeta_out, grad_out_scale);
     });
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;

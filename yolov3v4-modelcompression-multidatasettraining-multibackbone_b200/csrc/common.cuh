@@ -82,18 +82,10 @@ __device__ __forceinline__ void mbar_expect_tx_s(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// Host side: launch `kern` as a programmatic dependent of the previous kernel in the stream (B2Y_PDL=0: plain stream
-// order).  The grid may become resident while its predecessor drains, so the kernel MUST execute pdl_wait() before it
-// touches anything the predecessor wrote (and should call pdl_launch_dependents() right after, so that at most one
-// grid is ever parked behind a running one).  In a captured graph the edge becomes a programmatic dependency.
-inline bool b2y_pdl_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("B2Y_PDL");
-        v = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    return v != 0;
-}
+// Host side: launch `kern` as a programmatic dependent of the previous kernel in the stream.  The grid may become
+// resident while its predecessor drains, so the kernel MUST execute pdl_wait() before it touches anything the
+// predecessor wrote (and should call pdl_launch_dependents() right after, so that at most one grid is ever parked
+// behind a running one).  In a captured graph the edge becomes a programmatic dependency.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                               Args&&... args) {
@@ -103,14 +95,10 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
-    int na = 0;
-    if (b2y_pdl_enabled()) {
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        na = 1;
-    }
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = na;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 

@@ -3,7 +3,6 @@
 #include "conv_tc.cuh"
 
 #include <cmath>
-#include <cstdlib>
 #include <mutex>
 
 #include "b200yolo.h"
@@ -116,11 +115,6 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
     const int items = ((p.num_m_tiles + CLUSTER - 1) / CLUSTER) * p.num_n_tiles;
     const int max_clusters = g_num_sms / CLUSTER;
     const int clusters = items < max_clusters ? items : max_clusters;
-    static int pdl = -1;        // B2Y_PDL=0: plain stream order (no programmatic dependent launch)
-    if (pdl < 0) {
-        const char* e = getenv("B2Y_PDL");
-        pdl = (e && atoi(e) == 0) ? 0 : 1;
-    }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(clusters * CLUSTER);
     cfg.blockDim = dim3(ConvTcEpi::THREADS);
@@ -135,13 +129,11 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
         attr[na].val.clusterDim.z = 1;
         ++na;
     }
-    if (pdl) {
-        // the kernel's prologue (and its static weight loads) may start while the previous kernel drains; it executes
-        // griddepcontrol.wait before touching activations
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
+    // the kernel's prologue (and its static weight loads) may start while the previous kernel drains; it executes
+    // griddepcontrol.wait before touching activations
+    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
     cfg.attrs = attr;
     cfg.numAttrs = na;
     B2Y_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, p));
@@ -163,17 +155,12 @@ static int dispatch(int block_n, int kbytes, int cluster, const CUtensorMap& a, 
     return B2Y_ERR_UNSUPPORTED;
 }
 
-// cluster size for a launch: B2Y_CLUSTER env (1 = off, 2 default) when the tile shape supports multicast and there is
-// more than one M tile per cluster to share the weights across
+// cluster size for a launch: 2 when the tile shape supports multicast and there is more than one M tile per cluster to
+// share the weights across
 static int pick_cluster(int block_n, int kbytes, int num_m_tiles) {
-    static int want = -1;
-    if (want < 0) {
-        const char* e = getenv("B2Y_CLUSTER");
-        want = (e && atoi(e) == 1) ? 1 : 2;
-    }
     if (kbytes != 128 || block_n < 128) return 1;
-    if (num_m_tiles < 2 * want) return 1;
-    return want;
+    if (num_m_tiles < 4) return 1;
+    return 2;
 }
 
 struct EpilogueArgs {
@@ -287,11 +274,6 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
         p.stat_acc = stream_acc(st, 2 * CONV_STAT_MAX);
         if (p.stat_acc == nullptr) return B2Y_ERR_CUDA;
     }
-    static int tma_on = -1;      // B2Y_EPI_TMA=0: direct 16-byte stores from registers instead of smem + TMA
-    if (tma_on < 0) {
-        const char* ev = getenv("B2Y_EPI_TMA");
-        tma_on = (ev && atoi(ev) == 0) ? 0 : 1;
-    }
     {
         // the short epilogue: fp16/bf16 output (fp32 only through TMA), everything 16-byte addressable; a clipped last
         // N tile (Cout = 255 heads) needs the TMA store's clipping and has no residual
@@ -300,36 +282,27 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
                             (e.act == B2Y_ACT_LEAKY && e.slope >= 0.f && e.slope <= 1.f);
         const bool out16 = e.out_dtype == OUT_F16 || e.out_dtype == OUT_BF16;
         const bool out32 = e.out_dtype == OUT_F32;
-        const bool tma_ok = tma_on && g.out_identity;
+        // the TMA store needs the identity row mapping; the strided dgrad scatters rows through the register stores
+        const bool tma_ok = g.out_identity;
         const bool full = g.Nout % block_n == 0;
-        static int stats_fast = -1;   // B2Y_STATS_FAST=0: training forward convs (BN statistics) use the general epilogue
-        if (stats_fast < 0) {
-            const char* ev = getenv("B2Y_STATS_FAST");
-            stats_fast = (ev && atoi(ev) == 0) ? 0 : 1;
-        }
         // batch statistics ride on the short path when it stores through TMA and nothing is added to the accumulators
         const bool stats_ok = e.stat_sum == nullptr ||
-                              (stats_fast && out16 && tma_ok && e.bias == nullptr && e.res == nullptr);
+                              (out16 && tma_ok && e.bias == nullptr && e.res == nullptr);
         p.epi_fast = g.kind == CONV_KIND_F16 && (out16 || (out32 && tma_ok)) && !e.out_fakequant &&
                      stats_ok && act_ok && al16(e.out) && e.out_pitch % (out16 ? 8 : 4) == 0 &&
                      (e.bias == nullptr || al16(e.bias)) && (e.res == nullptr || (al16(e.res) && e.res_pitch % 8 == 0)) &&
                      (full || (tma_ok && e.res == nullptr));
-        // int8 graph (B2Y_I8_FAST=0 disables): int8 codes out, no residual, whole N tiles, and a power-of-two accumulator
-        // scale so that fma(acc, s, bias) equals the general path's (acc * s) + bias bit for bit
-        static int i8_fast = -1;
-        if (i8_fast < 0) {
-            const char* ev = getenv("B2Y_I8_FAST");
-            i8_fast = (ev && atoi(ev) == 0) ? 0 : 1;
-        }
+        // int8 graph: int8 codes out, no residual, whole N tiles, and a power-of-two accumulator scale so that
+        // fma(acc, s, bias) equals the general path's (acc * s) + bias bit for bit
         int ex = 0;
         const bool pow2 = e.acc_scale > 0.f && frexpf(e.acc_scale, &ex) == 0.5f && e.acc_scale_ptr == nullptr;
-        if (i8_fast && g.kind == CONV_KIND_I8 && e.out_dtype == OUT_I8 && !e.out_fakequant && e.stat_sum == nullptr &&
+        if (g.kind == CONV_KIND_I8 && e.out_dtype == OUT_I8 && !e.out_fakequant && e.stat_sum == nullptr &&
             (e.act == B2Y_ACT_LINEAR || (e.act == B2Y_ACT_LEAKY && e.slope >= 0.f && e.slope <= 1.f)) && pow2 && full &&
             e.res == nullptr && al16(e.out) && e.out_pitch % 16 == 0 && (e.bias == nullptr || al16(e.bias)) &&
             e.q_lo >= -128.f && e.q_hi <= 127.f && e.q_lo == floorf(e.q_lo) && e.q_hi == floorf(e.q_hi))
             p.epi_fast = 1;
         // fake-quantised / linear fp32 rows of the int8 graph (the YOLO heads): through the TMA store, which clips Cout = 255
-        if (i8_fast && g.kind == CONV_KIND_I8 && out32 && tma_ok && e.stat_sum == nullptr && e.act == B2Y_ACT_LINEAR &&
+        if (g.kind == CONV_KIND_I8 && out32 && tma_ok && e.stat_sum == nullptr && e.act == B2Y_ACT_LINEAR &&
             pow2 && e.res == nullptr && al16(e.out) && e.out_pitch % 4 == 0 && (e.bias == nullptr || al16(e.bias)) &&
             (!e.out_fakequant || (e.q_lo >= -4194304.f && e.q_hi <= 4194303.f && e.q_lo == floorf(e.q_lo) &&
                                   e.q_hi == floorf(e.q_hi))))
@@ -373,22 +346,13 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
     if (rc != B2Y_OK) return rc;
 
     {
-        // smem ring depth; weight-stationary mode when the whole weight panel of a single N tile fits beside >= min_stages
-        // A stages (B2Y_BRES=0 disables, B2Y_BRES_MIN_STAGES overrides the default of 6)
-        static int bres_on = -1, bres_min = 6;
-        if (bres_on < 0) {
-            const char* e = getenv("B2Y_BRES");
-            bres_on = (e && atoi(e) == 0) ? 0 : 1;
-            const char* m = getenv("B2Y_BRES_MIN_STAGES");
-            if (m && atoi(m) >= 2) bres_min = atoi(m);
-        }
+        // smem ring depth; weight-stationary mode when the whole weight panel of a single N tile fits beside >= 6 A stages
         const long long max_smem = conv_max_stage_smem(block_n);
         const long long a_bytes = 128LL * kbytes, b_bytes = (long long)block_n * kbytes;
         const long long res_bytes = (long long)p.ntaps * p.k_chunks * b_bytes;
         p.b_resident = 0;
         long long ns = max_smem / (a_bytes + b_bytes);
-        if (bres_on && cluster == 1 && p.num_n_tiles == 1 && p.num_m_tiles > g_num_sms &&
-            res_bytes + bres_min * a_bytes <= max_smem) {
+        if (cluster == 1 && p.num_n_tiles == 1 && p.num_m_tiles > g_num_sms && res_bytes + 6 * a_bytes <= max_smem) {
             p.b_resident = 1;
             ns = (max_smem - res_bytes) / a_bytes;
         }
@@ -397,7 +361,7 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
     // output map for the TMA-store epilogue (16-bit outputs on the short path with identity row mapping)
     CUtensorMap tmC = tmB;
     p.epi_tma = 0;
-    if (tma_on && p.epi_fast && p.out_identity) {
+    if (p.epi_fast && p.out_identity) {
         const bool o32 = e.out_dtype == OUT_F32, o8 = e.out_dtype == OUT_I8;
         rc = make_map_2d(&tmC, e.out, o32 ? 4 : (o8 ? 1 : 2), M, g.Nout, e.out_pitch, 32, 32, o32 ? 128 : (o8 ? 32 : 64),
                          e.out_dtype == OUT_BF16);

@@ -11,20 +11,20 @@
 //   D = A * B^T               : two wgmma.mma_async pairs (M = 2 x 64, K = 2 x 16) per tile, fp32 accumulators in
 //                               registers, staged through shared memory for the row-per-thread epilogue
 //
-// Persistent CTAs (one per SM).  NG warpgroups of "worker" warps; a group owns every NG-th tile of the CTA and runs a
-// three-stage software pipeline per thread (thread = one pixel row of the tile):
+// Persistent CTAs (one per SM).  STEM_NG warpgroups of "worker" warps; a group owns every STEM_NG-th tile of the CTA
+// and runs a three-stage software pipeline per thread (thread = one pixel row of the tile):
 //     issue the image loads of tile j      (27 predicated LDGs for 3x3 RGB)
 //     epilogue of tile j-1                 (staged accumulators -> bias/act -> 64-byte fp16 row), overlapping the
 //                                          loads in flight
 //     convert + store the A row of tile j  -> fence.proxy.async -> group barrier -> wgmma -> accumulators to smem
 #include <cmath>
-#include <cstdlib>
 
 #include "common.cuh"
 
 namespace b2y {
 
 enum { STEM_X_F32 = 0, STEM_X_F16 = 1, STEM_X_U8 = 2 };
+constexpr int STEM_NG = 4;      // worker warpgroups per CTA
 
 struct StemParams {
     const void* x;        // NCHW image
@@ -57,17 +57,17 @@ __device__ __forceinline__ float stem_ld<uint8_t>(const uint8_t* p) { return (fl
 
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-template <typename XT, int CIN, int K, int BLOCK_N, int NG>
-__global__ void __launch_bounds__(128 * NG, 1) stem_fused_kernel(const __grid_constant__ StemParams p) {
+template <typename XT, int CIN, int K, int BLOCK_N>
+__global__ void __launch_bounds__(128 * STEM_NG, 1) stem_fused_kernel(const __grid_constant__ StemParams p) {
     constexpr int KK = CIN * K * K;            // <= 32
     constexpr int A_BYTES = 128 * 64;
     constexpr int B_BYTES = BLOCK_N * 64;
     constexpr int ACC_BYTES = 128 * BLOCK_N * 4;
 
-    // smem: [NG A tiles] [B] [NG accumulator tiles]
+    // smem: [STEM_NG A tiles] [B] [STEM_NG accumulator tiles]
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* smem_b = smem + NG * A_BYTES;
+    uint8_t* smem_b = smem + STEM_NG * A_BYTES;
     uint8_t* smem_acc = smem_b + B_BYTES;
 
     const int warp = threadIdx.x >> 5;
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(128 * NG, 1) stem_fused_kernel(const __grid_co
         const bool leaky_max = act == B2Y_ACT_LEAKY && slope >= 0.f && slope <= 1.f;
         const unsigned HoWo = (unsigned)(p.Ho * p.Wo), Wo = (unsigned)p.Wo;
         const unsigned M_total = (unsigned)p.M_total;
-        const int my_group_tiles = (my_tiles - g + NG - 1) / NG;
+        const int my_group_tiles = (my_tiles - g + STEM_NG - 1) / STEM_NG;
         uint8_t* const arow = smem + g * A_BYTES + r_in_tile * 64;
         uint8_t* const acc_tile = smem_acc + g * ACC_BYTES;
         const int sw = (r_in_tile >> 1) & 3;
@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(128 * NG, 1) stem_fused_kernel(const __grid_co
             const bool have = j < my_group_tiles;
             unsigned row = 0;
             if (have) {
-                const unsigned tile = blockIdx.x + (unsigned)(g + j * NG) * gridDim.x;
+                const unsigned tile = blockIdx.x + (unsigned)(g + j * STEM_NG) * gridDim.x;
                 row = tile * 128u + (unsigned)r_in_tile;
                 // ---- 1. issue the image loads of tile j
                 const bool row_ok = row < M_total;
@@ -307,10 +307,10 @@ __global__ void __launch_bounds__(128 * NG, 1) stem_fused_kernel(const __grid_co
     }
 }
 
-template <typename XT, int CIN, int K, int BLOCK_N, int NG>
+template <typename XT, int CIN, int K, int BLOCK_N>
 static int stem_launch(const StemParams& p, cudaStream_t st) {
-    constexpr int SMEM = 1024 + NG * 128 * 64 + BLOCK_N * 64 + NG * 128 * BLOCK_N * 4;
-    auto kern = stem_fused_kernel<XT, CIN, K, BLOCK_N, NG>;
+    constexpr int SMEM = 1024 + STEM_NG * 128 * 64 + BLOCK_N * 64 + STEM_NG * 128 * BLOCK_N * 4;
+    auto kern = stem_fused_kernel<XT, CIN, K, BLOCK_N>;
     static unsigned long long attr_set = 0;      // one bit per device: the attribute is per (function, device)
     if (b2y_first_use_on_device(attr_set)) {
         B2Y_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
@@ -319,26 +319,17 @@ static int stem_launch(const StemParams& p, cudaStream_t st) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-    kern<<<grid, 128 * NG, SMEM, st>>>(p);
+    kern<<<grid, 128 * STEM_NG, SMEM, st>>>(p);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }
 
 template <typename XT>
 static int stem_dispatch(const StemParams& p, int cin, int k, cudaStream_t st) {
-    static int ng = 0;      // worker groups per CTA: B2Y_STEM_NG = 2 or 4 (default)
-    if (ng == 0) {
-        const char* e = getenv("B2Y_STEM_NG");
-        ng = (e && atoi(e) == 2) ? 2 : 4;
-    }
 #define B2Y_STEM_CASE(CI, KK)                                                                  \
     if (cin == CI && k == KK) {                                                                 \
-        if (ng == 2) {                                                                          \
-            if (p.Cout <= 32) return stem_launch<XT, CI, KK, 32, 2>(p, st);                    \
-            return stem_launch<XT, CI, KK, 64, 2>(p, st);                                      \
-        }                                                                                       \
-        if (p.Cout <= 32) return stem_launch<XT, CI, KK, 32, 4>(p, st);                        \
-        return stem_launch<XT, CI, KK, 64, 4>(p, st);                                          \
+        if (p.Cout <= 32) return stem_launch<XT, CI, KK, 32>(p, st);                           \
+        return stem_launch<XT, CI, KK, 64>(p, st);                                             \
     }
     B2Y_STEM_CASE(3, 3) B2Y_STEM_CASE(1, 3) B2Y_STEM_CASE(1, 5) B2Y_STEM_CASE(3, 1) B2Y_STEM_CASE(1, 1)
 #undef B2Y_STEM_CASE

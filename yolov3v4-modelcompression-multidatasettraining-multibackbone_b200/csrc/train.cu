@@ -1,7 +1,7 @@
-// Training-mode BatchNorm + activation (forward apply, backward reduce / apply) on NHWC fp16 tensors with fp32
-// statistics, and the fused SGD-Nesterov step over a flat fp32 parameter buffer.
-// Reference semantics: nn.BatchNorm2d(momentum=0.1, eps=1e-5) + activation under autograd (models.py:100-113),
-// optimizer train.py:135-144.  The batch sums themselves come out of the conv epilogue (conv_tc.cuh).
+// Training-mode backward helpers on NHWC fp16 tensors (the per-channel (BatchNorm/bias) + activation gradient reduce,
+// the YOLO-head, upsample and max-pool gradients), and the fused SGD-Nesterov step over a flat fp32 parameter buffer.
+// Reference semantics: activation under autograd (models.py:100-113), optimizer train.py:135-144.  The BatchNorm
+// training passes of the conv layers are in bn_train.cu.
 #include "b200yolo.h"
 #include "common.cuh"
 
@@ -14,116 +14,8 @@ static inline int grid_for(long long n, int block, int cap = 132 * 16) {
     return (int)g;
 }
 
-// ------------------------------------------------------------------------------------------------
-__global__ void bn_finalize_kernel(const float* __restrict__ s1, const float* __restrict__ s2, float count,
-                                   const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                   float momentum, float* __restrict__ rmean, float* __restrict__ rvar,
-                                   float* __restrict__ save_mean, float* __restrict__ save_invstd,
-                                   float* __restrict__ scale, float* __restrict__ shift, int C) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    const float mean = s1[c] / count;
-    float var = s2[c] / count - mean * mean;  // biased variance used for normalisation
-    var = fmaxf(var, 0.f);
-    const float invstd = 1.f / sqrtf(var + eps);
-    if (rmean != nullptr) {
-        const float unbiased = count > 1.f ? var * (count / (count - 1.f)) : var;
-        rmean[c] = (1.f - momentum) * rmean[c] + momentum * mean;
-        rvar[c] = (1.f - momentum) * rvar[c] + momentum * unbiased;
-    }
-    save_mean[c] = mean;
-    save_invstd[c] = invstd;
-    const float g = gamma != nullptr ? gamma[c] : 1.f;
-    const float sc = g * invstd;
-    scale[c] = sc;
-    shift[c] = (beta != nullptr ? beta[c] : 0.f) - mean * sc;
-}
-
-extern "C" int b2y_bn_finalize(const float* stat_sum, const float* stat_sqsum, long long count, const float* gamma,
-                               const float* beta, float eps, float momentum, float* running_mean, float* running_var,
-                               float* save_mean, float* save_invstd, float* scale, float* shift, int c,
-                               void* stream) {
-    if (!stat_sum || !stat_sqsum || !save_mean || !save_invstd || !scale || !shift || c <= 0 || count <= 0)
-        return B2Y_ERR_INVALID;
-    bn_finalize_kernel<<<(c + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-        stat_sum, stat_sqsum, (float)count, gamma, beta, eps, momentum, running_mean, running_var, save_mean,
-        save_invstd, scale, shift, c);
-    B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-__global__ void bn_act_fwd_kernel(const __half* __restrict__ x, long long xp, const float* __restrict__ scale,
-                                  const float* __restrict__ shift, const __half* __restrict__ res, long long rp,
-                                  __half* __restrict__ y, long long yp, long long pixels, int C, int act,
-                                  float slope) {
-    const int CV = C / 8;
-    const long long total = pixels * CV;
-    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int cv = (int)(idx % CV);
-        const long long pix = idx / CV;
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + pix * xp) + cv);
-        const __half* h = reinterpret_cast<const __half*>(&v);
-        const float4 sa = __ldg(reinterpret_cast<const float4*>(scale) + cv * 2);
-        const float4 sb = __ldg(reinterpret_cast<const float4*>(scale) + cv * 2 + 1);
-        const float4 ta = __ldg(reinterpret_cast<const float4*>(shift) + cv * 2);
-        const float4 tb = __ldg(reinterpret_cast<const float4*>(shift) + cv * 2 + 1);
-        const float sc[8] = {sa.x, sa.y, sa.z, sa.w, sb.x, sb.y, sb.z, sb.w};
-        const float sh[8] = {ta.x, ta.y, ta.z, ta.w, tb.x, tb.y, tb.z, tb.w};
-        float r[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) r[j] = apply_act(fmaf(__half2float(h[j]), sc[j], sh[j]), act, slope);
-        if (res != nullptr) {
-            const uint4 rv = __ldg(reinterpret_cast<const uint4*>(res + pix * rp) + cv);
-            const __half* rh = reinterpret_cast<const __half*>(&rv);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) r[j] += __half2float(rh[j]);
-        }
-        uint4 o;
-        __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(r[2 * j], r[2 * j + 1]);
-        reinterpret_cast<uint4*>(y + pix * yp)[cv] = o;
-    }
-}
-
-// v2 layout for the three BatchNorm passes: a thread owns ONE 8-channel vector (its per-channel coefficients live in
-// registers for the whole kernel) and walks the pixels with a fixed stride, so the loop body is loads + math + store:
-// no index divisions, no per-element coefficient loads, the activation resolved at compile time.  Needs 256 % (C/8) == 0.
-template <int ACT>
-__global__ void __launch_bounds__(256)
-bn_act_fwd_v2_kernel(const __half* __restrict__ x, long long xp, const float* __restrict__ scale,
-                     const float* __restrict__ shift, const __half* __restrict__ res, long long rp,
-                     __half* __restrict__ y, long long yp, long long pixels, int CV, float slope) {
-    const int cv = threadIdx.x % CV;
-    const int ppb = 256 / CV;
-    float sc[8], sh[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        sc[j] = __ldg(scale + cv * 8 + j);
-        sh[j] = __ldg(shift + cv * 8 + j);
-    }
-    for (long long pix = (long long)blockIdx.x * ppb + threadIdx.x / CV; pix < pixels; pix += (long long)gridDim.x * ppb) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + pix * xp) + cv);
-        const __half* h = reinterpret_cast<const __half*>(&v);
-        float r[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) r[j] = apply_act(fmaf(__half2float(h[j]), sc[j], sh[j]), ACT, slope);
-        if (res != nullptr) {
-            const uint4 rv = __ldg(reinterpret_cast<const uint4*>(res + pix * rp) + cv);
-            const __half* rh = reinterpret_cast<const __half*>(&rv);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) r[j] += __half2float(rh[j]);
-        }
-        uint4 o;
-        __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(r[2 * j], r[2 * j + 1]);
-        reinterpret_cast<uint4*>(y + pix * yp)[cv] = o;
-    }
-}
-
+// v2 layout: a thread owns ONE 8-channel vector (its per-channel coefficients live in registers for the whole kernel)
+// and walks the pixels with a fixed stride; the activation is resolved at compile time.  Needs 256 % (C/8) == 0.
 static inline int v2_grid(long long pixels, int CV) {
     const int ppb = 256 / CV;
     long long g = (pixels + ppb - 1) / ppb;
@@ -131,33 +23,6 @@ static inline int v2_grid(long long pixels, int CV) {
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 static inline bool v2_ok(int c) { return c % 8 == 0 && c / 8 <= 256 && 256 % (c / 8) == 0; }
-
-extern "C" int b2y_bn_act_fwd(const void* x, long long x_pitch, const float* scale, const float* shift,
-                              const void* residual, long long res_pitch, void* y, long long y_pitch,
-                              long long pixels, int c, int act, float slope, void* stream) {
-    if (!x || !y || !scale || !shift || c % 8 != 0 || x_pitch % 8 != 0 || y_pitch % 8 != 0) return B2Y_ERR_INVALID;
-    if (residual != nullptr && res_pitch % 8 != 0) return B2Y_ERR_INVALID;
-    if (v2_ok(c) && (act == B2Y_ACT_LEAKY || act == B2Y_ACT_MISH || act == B2Y_ACT_LINEAR)) {
-        const int CV = c / 8;
-        const int grid = v2_grid(pixels, CV);
-        cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define B2Y_FWD_V2(A)                                                                                                  \
-    bn_act_fwd_v2_kernel<A><<<grid, 256, 0, st>>>(reinterpret_cast<const __half*>(x), x_pitch, scale, shift,           \
-                                                  reinterpret_cast<const __half*>(residual), res_pitch,               \
-                                                  reinterpret_cast<__half*>(y), y_pitch, pixels, CV, slope)
-        if (act == B2Y_ACT_LEAKY) B2Y_FWD_V2(B2Y_ACT_LEAKY);
-        else if (act == B2Y_ACT_MISH) B2Y_FWD_V2(B2Y_ACT_MISH);
-        else B2Y_FWD_V2(B2Y_ACT_LINEAR);
-#undef B2Y_FWD_V2
-        B2Y_CUDA_CHECK(cudaGetLastError());
-        return B2Y_OK;
-    }
-    bn_act_fwd_kernel<<<grid_for(pixels * (c / 8), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const __half*>(x), x_pitch, scale, shift, reinterpret_cast<const __half*>(residual), res_pitch,
-        reinterpret_cast<__half*>(y), y_pitch, pixels, c, act, slope);
-    B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
-}
 
 // ------------------------------------------------------------------------------------------------
 // backward pass 1: dbeta[c] = sum du, dgamma[c] = sum du * xhat   with  u = x*scale+shift, du = dy*act'(u)
@@ -364,188 +229,6 @@ extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const voi
     rc = acc_finalize(acc, dbeta, c, st);
     if (rc != B2Y_OK || dgamma == nullptr) return rc;
     return acc_finalize(acc + c, dgamma, c, st);
-}
-
-// backward pass 2: dx = gamma*invstd * (du - dbeta/N - xhat*dgamma/N)
-// The data gradient dz feeds two tensor-core GEMMs whose operands must share one 16-bit format with the fp16
-// activations / weights, so dz is written in fp16 multiplied by a per-layer power of two s chosen on the device from
-// a bound of max|dz| (no host sync); the GEMM epilogues multiply by 1/s (scale_out[1]) read from device memory.
-template <typename GT>
-__global__ void bn_act_bwd_apply_kernel(const __half* __restrict__ x, long long xp, const GT* __restrict__ dy,
-                                        long long dp, const float* __restrict__ scale, const float* __restrict__ shift,
-                                        const float* __restrict__ gamma, const float* __restrict__ mean,
-                                        const float* __restrict__ invstd, const float* __restrict__ dgamma,
-                                        const float* __restrict__ dbeta, __half* __restrict__ dx, long long dxp,
-                                        long long pixels, int C, int act, float slope,
-                                        const float* __restrict__ du_absmax, float* __restrict__ scale_out) {
-    const int CV = C / 8;
-    const long long total = pixels * CV;
-    const float inv_n = 1.f / (float)pixels;
-    // every CTA derives the same scale: bound = max_c |gamma_c*invstd_c| * (max|du| + |dbeta_c|/N + 16*|dgamma_c|/N)
-    __shared__ float s_red[32];
-    __shared__ float s_scale;
-    float bound = 0.f;
-    {
-        const float dumax = du_absmax != nullptr ? *du_absmax : 1.f;
-        for (int c = threadIdx.x; c < C; c += blockDim.x) {
-            const float g = gamma != nullptr ? gamma[c] : 1.f;
-            const float b = fabsf(g * invstd[c]) * (dumax + fabsf(dbeta[c]) * inv_n + 16.f * fabsf(dgamma[c]) * inv_n);
-            bound = fmaxf(bound, b);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) bound = fmaxf(bound, __shfl_xor_sync(0xffffffffu, bound, o));
-        if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = bound;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            float m = 0.f;
-            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, s_red[w]);
-            float sc = 1.f;
-            if (m > 0.f && m < 3.0e38f) sc = exp2f(floorf(log2f(4096.f / m)));   // target max |dz|*s <= 2^12
-            sc = fminf(fmaxf(sc, 1.0e-30f), 1.0e30f);
-            s_scale = sc;
-            if (blockIdx.x == 0 && scale_out != nullptr) {
-                scale_out[0] = sc;
-                scale_out[1] = 1.f / sc;
-            }
-        }
-        __syncthreads();
-    }
-    const float sc = s_scale;
-    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int cv = (int)(idx % CV);
-        const long long pix = idx / CV;
-        float xf8[8], g8[8];
-        Half8<__half>::load(x + pix * xp + cv * 8, xf8);
-        Half8<GT>::load(dy + pix * dp + cv * 8, g8);
-        float r[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int c = cv * 8 + j;
-            const float xf = xf8[j];
-            const float u = fmaf(xf, scale[c], shift[c]);
-            const float du = g8[j] * act_grad(u, act, slope);
-            const float xhat = (xf - mean[c]) * invstd[c];
-            const float g = gamma != nullptr ? gamma[c] : 1.f;
-            r[j] = sc * (g * invstd[c] * (du - dbeta[c] * inv_n - xhat * dgamma[c] * inv_n));
-        }
-        Half8<__half>::store(dx + pix * dxp + cv * 8, r);
-    }
-}
-
-template <typename GT, int ACT>
-__global__ void __launch_bounds__(256)
-bn_act_bwd_apply_v2_kernel(const __half* __restrict__ x, long long xp, const GT* __restrict__ dy, long long dp,
-                           const float* __restrict__ scale, const float* __restrict__ shift,
-                           const float* __restrict__ gamma, const float* __restrict__ mean,
-                           const float* __restrict__ invstd, const float* __restrict__ dgamma,
-                           const float* __restrict__ dbeta, __half* __restrict__ dx, long long dxp, long long pixels,
-                           int CV, float slope, const float* __restrict__ du_absmax, float* __restrict__ scale_out) {
-    const int C = CV * 8;
-    const float inv_n = 1.f / (float)pixels;
-    __shared__ float s_red[8];
-    __shared__ float s_scale;
-    float bound = 0.f;
-    {   // same bound / scale as bn_act_bwd_apply_kernel (every CTA derives it identically)
-        const float dumax = du_absmax != nullptr ? *du_absmax : 1.f;
-        for (int c = threadIdx.x; c < C; c += 256) {
-            const float g = gamma != nullptr ? gamma[c] : 1.f;
-            const float b = fabsf(g * invstd[c]) * (dumax + fabsf(dbeta[c]) * inv_n + 16.f * fabsf(dgamma[c]) * inv_n);
-            bound = fmaxf(bound, b);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) bound = fmaxf(bound, __shfl_xor_sync(0xffffffffu, bound, o));
-        if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = bound;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            float m = 0.f;
-            for (int w = 0; w < 8; ++w) m = fmaxf(m, s_red[w]);
-            float sc = 1.f;
-            if (m > 0.f && m < 3.0e38f) sc = exp2f(floorf(log2f(4096.f / m)));
-            sc = fminf(fmaxf(sc, 1.0e-30f), 1.0e30f);
-            s_scale = sc;
-            if (blockIdx.x == 0 && scale_out != nullptr) {
-                scale_out[0] = sc;
-                scale_out[1] = 1.f / sc;
-            }
-        }
-        __syncthreads();
-    }
-    const float scl = s_scale;
-    const int cv = threadIdx.x % CV;
-    const int ppb = 256 / CV;
-    float sc[8], sh[8], mu[8], is[8], gi[8], db[8], dg[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const int c = cv * 8 + j;
-        sc[j] = __ldg(scale + c);
-        sh[j] = __ldg(shift + c);
-        mu[j] = __ldg(mean + c);
-        is[j] = __ldg(invstd + c);
-        gi[j] = (gamma != nullptr ? __ldg(gamma + c) : 1.f) * is[j];
-        db[j] = __ldg(dbeta + c) * inv_n;
-        dg[j] = __ldg(dgamma + c) * inv_n;
-    }
-    for (long long pix = (long long)blockIdx.x * ppb + threadIdx.x / CV; pix < pixels; pix += (long long)gridDim.x * ppb) {
-        float xf8[8], g8[8];
-        Half8<__half>::load(x + pix * xp + cv * 8, xf8);
-        Half8<GT>::load(dy + pix * dp + cv * 8, g8);
-        float r[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float xf = xf8[j];
-            const float u = fmaf(xf, sc[j], sh[j]);
-            const float du = g8[j] * act_grad(u, ACT, slope);
-            const float xhat = (xf - mu[j]) * is[j];
-            r[j] = scl * (gi[j] * (du - db[j] - xhat * dg[j]));
-        }
-        Half8<__half>::store(dx + pix * dxp + cv * 8, r);
-    }
-}
-
-extern "C" int b2y_bn_act_bwd_apply(const void* x, long long x_pitch, const void* dy, long long dy_pitch,
-                                    const float* scale, const float* shift, const float* gamma,
-                                    const float* save_mean, const float* save_invstd, const float* dgamma,
-                                    const float* dbeta, void* dx, long long dx_pitch, long long pixels, int c, int act,
-                                    float slope, int grad_dtype, const float* du_absmax, float* scale_out,
-                                    void* stream) {
-    if (!x || !dy || !scale || !shift || !save_mean || !save_invstd || !dgamma || !dbeta || !dx || c % 8 != 0)
-        return B2Y_ERR_INVALID;
-    if (v2_ok(c) && (act == B2Y_ACT_LEAKY || act == B2Y_ACT_MISH || act == B2Y_ACT_LINEAR)) {
-        const int CV = c / 8;
-        const int g2 = v2_grid(pixels, CV);
-        cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define B2Y_APP_V2(T, A)                                                                                               \
-    bn_act_bwd_apply_v2_kernel<T, A><<<g2, 256, 0, st>>>(                                                               \
-        reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const T*>(dy), dy_pitch, scale, shift, gamma,    \
-        save_mean, save_invstd, dgamma, dbeta, reinterpret_cast<__half*>(dx), dx_pitch, pixels, CV, slope, du_absmax,  \
-        scale_out)
-        if (grad_dtype == B2Y_DT_BF16) {
-            if (act == B2Y_ACT_LEAKY) B2Y_APP_V2(__nv_bfloat16, B2Y_ACT_LEAKY);
-            else if (act == B2Y_ACT_MISH) B2Y_APP_V2(__nv_bfloat16, B2Y_ACT_MISH);
-            else B2Y_APP_V2(__nv_bfloat16, B2Y_ACT_LINEAR);
-        } else {
-            if (act == B2Y_ACT_LEAKY) B2Y_APP_V2(__half, B2Y_ACT_LEAKY);
-            else if (act == B2Y_ACT_MISH) B2Y_APP_V2(__half, B2Y_ACT_MISH);
-            else B2Y_APP_V2(__half, B2Y_ACT_LINEAR);
-        }
-#undef B2Y_APP_V2
-        B2Y_CUDA_CHECK(cudaGetLastError());
-        return B2Y_OK;
-    }
-    if (grad_dtype == B2Y_DT_BF16)
-        bn_act_bwd_apply_kernel<__nv_bfloat16><<<grid_for(pixels * (c / 8), 256), 256, 0,
-                                                 static_cast<cudaStream_t>(stream)>>>(
-            reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, scale,
-            shift, gamma, save_mean, save_invstd, dgamma, dbeta, reinterpret_cast<__half*>(dx), dx_pitch, pixels, c,
-            act, slope, du_absmax, scale_out);
-    else
-        bn_act_bwd_apply_kernel<__half><<<grid_for(pixels * (c / 8), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-            reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, scale, shift,
-            gamma, save_mean, save_invstd, dgamma, dbeta, reinterpret_cast<__half*>(dx), dx_pitch, pixels, c, act,
-            slope, du_absmax, scale_out);
-    B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

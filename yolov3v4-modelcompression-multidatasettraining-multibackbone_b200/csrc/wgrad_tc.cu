@@ -616,12 +616,7 @@ extern "C" int b2y_conv2d_bwd_weight(const b2y_conv_desc* d, const void* x, cons
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int rc;
-    static int taps_on = -1;        // B2Y_WGRAD_TAPS=0: narrow 3x3 layers use the general kernel as well
-    if (taps_on < 0) {
-        const char* ev = getenv("B2Y_WGRAD_TAPS");
-        taps_on = (ev && atoi(ev) == 0) ? 0 : 1;
-    }
-    const bool taps = taps_on && d->ksize == 3 && (d->in_c == 32 || d->in_c == 64);
+    const bool taps = d->ksize == 3 && (d->in_c == 32 || d->in_c == 64);
     CUtensorMap tmDyT = tmDy;
     if (taps) {
         const int bn = d->in_c == 32 ? 64 : 32;

@@ -117,12 +117,7 @@ extern "C" int b2y_yolo_decode(const float* raw, long long raw_pitch, float* p, 
     if (raw_pitch < (long long)na * no) return B2Y_ERR_INVALID;
     const long long runs = (long long)batch * na * ny * nx;
     if (runs > 0x7fffffffLL) return B2Y_ERR_UNSUPPORTED;
-    static int per_pixel = -1;     // B2Y_DECODE_PIXEL=0: the one-warp-per-run kernel for every shape
-    if (per_pixel < 0) {
-        const char* ev = getenv("B2Y_DECODE_PIXEL");
-        per_pixel = (ev && atoi(ev) == 0) ? 0 : 1;
-    }
-    if (per_pixel && na * no <= 256) {
+    if (na * no <= 256) {
         const long long pixels = (long long)batch * ny * nx;
         long long pb = (pixels + 7) / 8;
         if (pb > 132 * 8) pb = 132 * 8;
