@@ -366,7 +366,8 @@ int b2y_dwconv_bwd_data(const b2y_conv_desc* d, const void* dz, const float* w, 
 int b2y_dwconv_bwd_weight(const b2y_conv_desc* d, const void* x, const void* dz, float* dw, float alpha,
                           const float* inv_scale_ptr, void* stream);
 /* SE forward: y = x * hsigmoid(W2 relu(W1 mean_hw(x))).  ws = fp32 [batch][3c + cr] scratch that the backward reads
- * (mean, h, pre-activation v, gate s) */
+ * (mean [batch][c] | pre-activation v [batch][c] | gate s [batch][c] | h [batch][cr]: s, read with 16-byte loads, stays
+ * aligned for every batch) */
 int b2y_se_fwd(const void* x, long long x_pitch, const float* w1, const float* w2, void* y, long long y_pitch, int batch,
                int hw, int c, int cr, float* ws, void* stream);
 /* SE backward: dx (+)= dy*s + dmean/hw;  dw1 [cr][c], dw2 [c][cr] = grad_scale * gradients (overwritten) */

@@ -84,29 +84,98 @@ def _block_parts(block):
     return conv, bn, act, slope
 
 
-def _new_act(shape, device):
-    """fp16 NHWC activation buffer; widths that are not a multiple of 16 get a zero-filled pad (see _Tensor.view_k)."""
-    B, H, W, C = shape
-    if C % 16 == 0:
-        return torch.empty((B, H, W, C), dtype=torch.float16, device=device)
-    return torch.zeros((B, H, W, (C + 15) // 16 * 16), dtype=torch.float16, device=device)
+class SlotStore:
+    """Device storage that the plans of one model share across input shapes.
+
+    A slot is named by what a buffer is (layer index, role, channel pitch, dtype), never by its shape; its capacity is
+    the largest request made so far.  A plan's tensor is a prefix of its slot: with the pitch fixed by the channel count,
+    pixel n of a smaller plan sits on pixel n of a larger one, so pad channels land on pad channels and stay zero (slots
+    are zero-filled when allocated and nobody writes pad channels).  Slot bases come straight from the caching allocator
+    (512-byte aligned).  A request above a slot's capacity reallocates that slot and bumps its version: every plan that
+    took the old slot still points at the old memory (tensor views, tensor maps, CUDA graphs) and is dropped by the
+    engine, which frees the old slot.
+
+    A training forward that waits for its backward pins the store (`pin`, a weak reference to the pin that the step's
+    autograd node owns); the engine then builds plans of other shapes on private storage until the backward has run or
+    the graph has been freed."""
+
+    def __init__(self, device):
+        self.device = device
+        self.slots = {}
+        self.versions = {}
+        self.generation = 0     # bumped by every reallocation
+        self.pin = None
+
+    def take(self, name, shape, dtype):
+        nbytes = 1
+        for s in shape:
+            nbytes *= int(s)
+        nbytes *= torch.empty((), dtype=dtype).element_size()
+        slot = self.slots.get(name)
+        if slot is None or slot.numel() < nbytes:
+            if slot is not None:
+                self.generation += 1
+                del self.slots[name], slot          # plans built on the old slot hold it until they are dropped
+            slot = self.slots[name] = torch.zeros(max(nbytes, 1), dtype=torch.uint8, device=self.device)
+            self.versions[name] = self.versions.get(name, -1) + 1
+        return slot[:nbytes].view(dtype).view(shape)
+
+    def pinned_by(self):
+        """The plan whose pending backward holds the store, or None."""
+        pin = self.pin() if self.pin is not None else None
+        return pin.plan if pin is not None else None
+
+    def stale(self, held):
+        """held: {slot name: version} of one plan.  True when one of those slots has been reallocated since."""
+        return any(self.versions[n] != v for n, v in held.items())
+
+
+class EvalWeights:
+    """Packed inference weights of one model, shared by its eval plans of every shape and re-packed once per parameter
+    version.  Entries are keyed (layer index, layout): the pixel-pair layouts depend on the plan (an odd width rules
+    them out), the base layout does not."""
+
+    def __init__(self):
+        self.version = None
+        self.packs = {}
 
 
 class Plan:
-    def __init__(self, model, x_shape, device, training, keep_features=False):
+    def __init__(self, model, x_shape, device, training, keep_features=False, store=None, shared_weights=None):
         if training:
             raise NotImplementedError("training plan is built by b200yolo.train_engine")
         self.model = model
         self.keep_features = bool(keep_features)
         self.device = device
         self.B, self.Cin, self.H, self.W = x_shape
+        self.store = store if store is not None else SlotStore(device)
+        self.shared_weights = shared_weights if shared_weights is not None else EvalWeights()
+        self.held = {}          # slot name -> version taken
         self.steps = []
-        self.weights = {}       # layer index -> packed weights
+        self.wkey = {}          # layer index -> key of its packed weights in shared_weights.packs
         self.param_version = None
         self.graph = None
         self.runs = 0
         self.static_x = None
         self._build()
+
+    def _take(self, name, shape, dtype=torch.float16):
+        t = self.store.take(name, shape, dtype)
+        self.held[name] = self.store.versions[name]
+        return t
+
+    def _new_act(self, name, C, H, W):
+        """fp16 NHWC activation buffer; widths that are not a multiple of 16 get a zero pad (see _Tensor.view_k)."""
+        pitch = (C + 15) // 16 * 16
+        return self._take(('act', name, pitch, torch.float16), (self.B, H, W, pitch))
+
+    def _w(self, i):
+        return self.shared_weights.packs[self.wkey[i]]
+
+    def _stem_workspace(self, conv):
+        d = ops.make_conv_desc((self.B, self.H, self.W, conv.in_channels), conv.in_channels, conv.out_channels,
+                               conv.kernel_size[0], conv.stride[0], conv.padding[0], conv.out_channels)
+        return self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,))
 
     # ---------------------------------------------------------------------------------------------------------
     def _build(self):
@@ -195,7 +264,7 @@ class Plan:
                 continue
             srcs = [i + l if l < 0 else l for l in d['layers']]
             dst = tens[i]
-            dst.buf = _new_act((B, dst.H, dst.W, dst.C), dev)
+            dst.buf = self._new_act(('cat', i), dst.C, dst.H, dst.W)
             off = 0
             for s in srcs:
                 st = tens[s]
@@ -211,12 +280,13 @@ class Plan:
                 pass  # resolved at allocation time below (needs the source buffer)
 
         # 5) allocate what is left and emit the launch list
-        def alloc(t):
+        def alloc(t, i):
             if t.buf is None:
                 if t.dtype == torch.float16:
-                    t.buf = _new_act((B, t.H, t.W, t.C), dev)
+                    t.buf = self._new_act(i, t.C, t.H, t.W)
                 else:
-                    t.buf = torch.empty((B, t.H, t.W, ((t.C + 3) // 4) * 4), dtype=t.dtype, device=dev)
+                    pitch = ((t.C + 3) // 4) * 4
+                    t.buf = self._take(('head', i, pitch, t.dtype), (B, t.H, t.W, pitch), t.dtype)
                 t.c0 = 0
             return t
 
@@ -229,17 +299,17 @@ class Plan:
                 conv, bn, act, slope = _block_parts(m)
                 if conv.groups != conv.in_channels or conv.out_channels != conv.in_channels:
                     raise NotImplementedError("only channel-multiplier-1 depthwise convolutions are supported")
-                self.steps.append(('dw', i, tens[i - 1], alloc(tens[i]), conv, bn, act, slope))
+                self.steps.append(('dw', i, tens[i - 1], alloc(tens[i], i), conv, bn, act, slope))
             elif t == 'se':
                 fc = m[0].fc if isinstance(m, nn.Sequential) else m.fc
                 src = tens[i - 1]
-                ws = ops.se_workspace(B, src.C, fc[0].out_features, dev)
-                self.steps.append(('se', i, src, alloc(tens[i]), fc[0], fc[2], ws))
+                ws = self._take(('se_ws', i), (B, 3 * src.C + fc[0].out_features), torch.float32)
+                self.steps.append(('se', i, src, alloc(tens[i], i), fc[0], fc[2], ws))
             elif t == 'convolutional':
                 conv, bn, act, slope = _block_parts(m)
                 if conv.groups != 1:
                     raise NotImplementedError("grouped convolution is not supported by the sm_90a engine yet")
-                out = alloc(tens[i])
+                out = alloc(tens[i], i)
                 res = None
                 if i + 1 < n and fused_into[i + 1] == i:
                     l = defs[i + 1]['from'][0]
@@ -252,7 +322,7 @@ class Plan:
                 frm = [i + l if l < 0 else l for l in d['from']]
                 if getattr(m, 'weight', False):
                     raise NotImplementedError("weighted shortcut is not supported by the sm_90a engine yet")
-                out = alloc(tens[i])
+                out = alloc(tens[i], i)
                 cur = tens[i - 1]
                 for s in frm:
                     # widths may differ (layers.py:57-72): the sum covers the first min(nx, na) channels, the rest of x
@@ -269,10 +339,10 @@ class Plan:
                 for st, off in copies.get(i, []):
                     self.steps.append(('copy', st, tens[i], off))
             elif t == 'upsample':
-                self.steps.append(('upsample', tens[i - 1], alloc(tens[i]), d['stride']))
+                self.steps.append(('upsample', tens[i - 1], alloc(tens[i], i), d['stride']))
             elif t == 'maxpool':
                 k, s = d['size'], d['stride']
-                self.steps.append(('maxpool', tens[i - 1], alloc(tens[i]), k, s, k == 2 and s == 1))
+                self.steps.append(('maxpool', tens[i - 1], alloc(tens[i], i), k, s, k == 2 and s == 1))
             elif t == 'yolo':
                 raw = tens[i - 1]
                 rows = m.na * raw.H * raw.W
@@ -296,10 +366,20 @@ class Plan:
             v += t._version + (t.data_ptr() & 0xffff)
         return v
 
-    def _pack_weights(self):
+    def _pack_weights(self, ver):
+        """Look up (and pack on first use at this parameter version) the weights of every layer in the engine-wide
+        EvalWeights; the plan keeps only the keys, so it never holds packed weights of an outdated version."""
+        sw = self.shared_weights
+        if sw.version != ver:
+            sw.packs = {}
+            sw.version = ver
+        packs = sw.packs
         for st in self.steps:
             if st[0] == 'dw':
                 _, i, src, out, conv, bn, act, slope = st
+                key = self.wkey[i] = (i, 'dw')
+                if key in packs:
+                    continue
                 w = conv.weight.detach().float().contiguous()
                 if bn is not None:           # fold: y = conv * gamma/sqrt(var+eps) + (beta - mean*gamma/sqrt(var+eps))
                     sc = (bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)).float()
@@ -309,34 +389,40 @@ class Plan:
                 else:
                     sc = None
                     bi = conv.bias.detach().float().contiguous() if conv.bias is not None else None
-                self.weights[i] = (w, sc.contiguous() if sc is not None else None,
-                                   bi.contiguous() if bi is not None else None)
+                packs[key] = (w, sc.contiguous() if sc is not None else None,
+                              bi.contiguous() if bi is not None else None)
                 continue
             if st[0] != 'conv':
                 continue
             _, i, src, out, res, conv, bn, act, slope = st
+            layout = 'pair' if self._pair_packable(st) else 's2' if self._s2_pair_packable(st) else 'base'
+            key = self.wkey[i] = (i, layout)
+            if key in packs:
+                continue
             bnp = None
             eps = 1e-5
             if bn is not None:
                 bnp = (bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var)
                 eps = bn.eps
-            stem = conv.in_channels <= 4
-            wsrc = conv.weight.detach()
-            if not stem and conv.in_channels % 16 != 0:      # zero columns for the padded K channels (view_k)
-                wsrc = torch.nn.functional.pad(wsrc, (0, 0, 0, 0, 0, (-conv.in_channels) % 16))
-            wp, bias, w32 = ops.pack_conv_weights(wsrc, conv.bias.detach() if conv.bias is not None
-                                                  else None, bnp, eps, want_fp32=stem)
-            wstem = None
-            if stem and (conv.in_channels * conv.kernel_size[0] <= 16 or
-                         conv.in_channels * conv.kernel_size[0] ** 2 <= 32):
-                wstem = ops.pack_stem_weights(w32)
-            self.weights[i] = (wp, bias, w32, wstem)
-            if self._pair_packable(st):
-                self.weights[i] = self.weights[i] + (self._pair_pack(conv, bnp, eps),)
-            elif self._s2_pair_packable(st):
+            base = packs.get((i, 'base'))
+            if base is None:
+                stem = conv.in_channels <= 4
+                wsrc = conv.weight.detach()
+                if not stem and conv.in_channels % 16 != 0:      # zero columns for the padded K channels (view_k)
+                    wsrc = torch.nn.functional.pad(wsrc, (0, 0, 0, 0, 0, (-conv.in_channels) % 16))
+                wp, bias, w32 = ops.pack_conv_weights(wsrc, conv.bias.detach() if conv.bias is not None
+                                                      else None, bnp, eps, want_fp32=stem)
+                wstem = None
+                if stem and (conv.in_channels * conv.kernel_size[0] <= 16 or
+                             conv.in_channels * conv.kernel_size[0] ** 2 <= 32):
+                    wstem = ops.pack_stem_weights(w32)
+                base = packs[(i, 'base')] = (wp, bias, w32, wstem)
+            if layout == 'pair':
+                packs[key] = base + (self._pair_pack(conv, bnp, eps),)
+            elif layout == 's2':
                 _, bias_f, w32f = ops.pack_conv_weights(conv.weight.detach(), conv.bias.detach() if conv.bias is not None
                                                         else None, bnp, eps, want_fp32=True)
-                self.weights[i] = self.weights[i] + (('s2', ops.s2_pair_weights(w32f).half(), bias_f),)
+                packs[key] = base + (('s2', ops.s2_pair_weights(w32f).half(), bias_f),)
 
     # ---- pixel-pair packing of the Cin = 32 3x3 layers --------------------------------------------------------------
     # With 32 input channels a tap of the im2col gather is a 64-byte row: one TMA request per pixel per tap, and the
@@ -387,7 +473,7 @@ class Plan:
             kind = st[0]
             if kind == 'conv':
                 _, i, src, out, res, conv, bn, act, slope = st
-                wp, bias, w32, wstem = self.weights[i][:4]
+                wp, bias, w32, wstem = self._w(i)[:4]
                 k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
                 if src is None:
                     if conv.in_channels > 4:
@@ -400,22 +486,20 @@ class Plan:
                         if x.dtype != torch.float32:
                             x = x.float() / 256.0 if x.dtype == torch.uint8 else x.float()
                         if getattr(self, 'stem_ws', None) is None:
-                            self.stem_ws = ops.stem_workspace(
-                                ops.make_conv_desc((self.B, self.H, self.W, conv.in_channels), conv.in_channels,
-                                                   conv.out_channels, k, s, p, conv.out_channels), self.device)
+                            self.stem_ws = self._stem_workspace(conv)
                         ops.stem_conv_tc(x, wstem, bias, conv.in_channels, k, s, p, act=act, slope=slope,
                                          out=out.view(), workspace=self.stem_ws)
                     else:
                         if x.dtype != torch.float32:
                             x = x.float() / 256.0 if x.dtype == torch.uint8 else x.float()
                         ops.stem_conv(x, w32, bias, k, s, p, act=act, slope=slope, out=out.view())
-                elif len(self.weights[i]) == 5 and isinstance(self.weights[i][4][0], str):
-                    _, wps2, bias_s2 = self.weights[i][4]
+                elif len(self._w(i)) == 5 and isinstance(self._w(i)[4][0], str):
+                    _, wps2, bias_s2 = self._w(i)[4]
                     ops.conv2d(src.view(), wps2, bias_s2, k, s, p, act=act, slope=slope,
                                residual=res.view() if res is not None else None, out=out.view(),
                                w_layout=WLAYOUT_S2_PAIRS)
-                elif len(self.weights[i]) == 5:
-                    wp2, bias2 = self.weights[i][4]
+                elif len(self._w(i)) == 5:
+                    wp2, bias2 = self._w(i)[4]
                     pairs = lambda t: t.buf.view(t.buf.shape[0], t.H, t.W // 2, 2 * t.C)
                     ops.conv2d(pairs(src), wp2, bias2, 3, 1, 1, act=act, slope=slope,
                                residual=pairs(res) if res is not None else None, out=pairs(out))
@@ -424,7 +508,7 @@ class Plan:
                                residual=res.view() if res is not None else None, out=out.view())
             elif kind == 'dw':
                 _, i, src, out, conv, bn, act, slope = st
-                w, sc, bi = self.weights[i]
+                w, sc, bi = self._w(i)
                 ops.dwconv2d(src.view(), w, conv.kernel_size[0], conv.stride[0], conv.padding[0], scale=sc, bias=bi,
                              act=act, slope=slope, out=out.view())
             elif kind == 'se':
@@ -551,7 +635,7 @@ class Plan:
         model = self.model
         ver = self._params_version()
         if ver != self.param_version:
-            self._pack_weights()
+            self._pack_weights(ver)
             self.param_version = ver
             self.graph = None
         # fp32 / fp16 images go to the stem as they are; uint8 images (the reference's dataloader output before
@@ -569,7 +653,7 @@ class Plan:
             io, p = self.io, tuple(self.p_out)
         else:
             if self.graph is None:
-                self.static_x = torch.empty_like(x)
+                self.static_x = self._take(('x', x.dtype), tuple(x.shape), x.dtype)
                 self.static_x.copy_(x)
                 self.io = torch.empty((self.B, self.total_rows, no), dtype=torch.float32, device=self.device)
                 g = torch.cuda.CUDAGraph()
@@ -596,9 +680,33 @@ class Engine:
     def __init__(self, model):
         self.model = model
         self.plans = {}
+        self._reset_shared()
+
+    def _reset_shared(self):
+        # shape-dependent buffers: one slot store for the training plans, one for the eval plans (created on the
+        # model's device at first use); shape-independent state: packed weights, gradient outputs, side stream
+        self.train_store = self.eval_store = None
+        self.eval_weights = EvalWeights()
+        self.train_shared = None
 
     def invalidate(self):
         self.plans.clear()
+        self._reset_shared()
+
+    def weights_changed(self):
+        """The parameters were written in place without a version bump (fused optimiser on the flat buffers): every
+        plan re-packs its weights on its next forward."""
+        self.eval_weights.version = None
+        for plan in self.plans.values():
+            plan.param_version = None
+
+    def _drop_stale(self):
+        """Drop the plans whose slots were reallocated by a larger request (their graphs point at the old memory)."""
+        for store in (self.train_store, self.eval_store):
+            if store is None:
+                continue
+            for k in [k for k, p in self.plans.items() if getattr(p, 'store', None) is store and store.stale(p.held)]:
+                del self.plans[k]
 
     def _forward_quantized(self, x):
         model = self.model
@@ -629,9 +737,7 @@ class Engine:
 
     def plan_for(self, x):
         self.forward(x)
-        model = self.model
-        keep = bool(model.keep_features)
-        return self.plans[(tuple(x.shape), bool(model.training), x.device.index, keep, x.dtype)]
+        return self.last_plan
 
     def _check_device(self, x):
         """One engine serves ONE device: the packed weights, plans and CUDA graphs live where the parameters are.
@@ -662,22 +768,41 @@ class Engine:
             return self._accurate.forward(x)
         keep = bool(model.keep_features)
         key = (tuple(x.shape), bool(model.training), x.device.index, keep, x.dtype)
+        if model.training:
+            from .train_engine import TrainPlan, TrainShared
+            if self.train_store is None:
+                self.train_store, self.train_shared = SlotStore(x.device), TrainShared(x.device)
+            store = self.train_store
+        else:
+            if self.eval_store is None:
+                self.eval_store = SlotStore(x.device)
+            store = self.eval_store
         plan = self.plans.get(key)
-        if plan is None:
-            # bounded plan cache (multi-scale training visits ~11 image sizes, each plan owns all its activation /
-            # gradient buffers and CUDA graphs): least recently used plans are dropped beyond B2Y_MAX_PLANS (default 6)
-            limit = int(os.environ.get('B2Y_MAX_PLANS', '6'))
+        owner = store.pinned_by()
+        if owner is not None and owner is not plan:
+            # a training forward of another shape still waits for its backward and owns the shared slots: this step
+            # runs on a plan with private storage, which is not cached
+            plan = TrainPlan(model, tuple(x.shape), x.device, keep, SlotStore(x.device), self.train_shared)
+        elif plan is None:
+            # bounded plan cache: a cached plan holds its tensor maps, CUDA graphs and caller-visible outputs, while the
+            # activation / gradient buffers are slots shared by every shape; least recently used plans are dropped
+            # beyond B2Y_MAX_PLANS (default 32: 11 multi-scale training sizes plus a rectangular evaluation set)
+            limit = int(os.environ.get('B2Y_MAX_PLANS', '32'))
             while len(self.plans) >= limit > 0:
                 self.plans.pop(next(iter(self.plans)))
+            gen = store.generation
             if model.training:
-                from .train_engine import TrainPlan
-                plan = TrainPlan(model, tuple(x.shape), x.device, keep)
+                plan = TrainPlan(model, tuple(x.shape), x.device, keep, store, self.train_shared)
             else:
-                plan = Plan(model, tuple(x.shape), x.device, False, keep)
+                plan = Plan(model, tuple(x.shape), x.device, False, keep, store, self.eval_weights)
             self.plans[key] = plan
+            if store.generation != gen:
+                self._drop_stale()
         else:
             self.plans[key] = self.plans.pop(key)      # move to the most-recently-used end
         self.last_plan = plan
-        if model.training:
-            return plan.run(x)
-        return plan.forward(x)
+        gen = store.generation
+        out = plan.run(x) if model.training else plan.forward(x)
+        if store.generation != gen:                 # a slot taken on first use grew
+            self._drop_stale()
+        return out

@@ -111,18 +111,23 @@ def stem_conv(x_nchw, w_oihw, bias, k, stride, pad, act="linear", slope=0.1, out
     return out
 
 
-def pack_stem_weights(w_oihw_folded):
+def pack_stem_weights(w_oihw_folded, out=None):
     O, I, k, _ = w_oihw_folded.shape
     shape = (O, 32) if I * k * k <= 32 else (O, k, 16)     # full-im2col row vs one row per kernel row (conv_tc.cu)
-    out = torch.empty(shape, dtype=torch.float16, device=w_oihw_folded.device)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float16, device=w_oihw_folded.device)
+    assert out.shape == shape and out.dtype == torch.float16 and out.is_contiguous()
     call("b2y_pack_stem_weights", ptr(w_oihw_folded.contiguous().float()), O, I, k, ptr(out), stream_ptr())
     return out
 
 
-def stem_workspace(desc, device):
+def stem_workspace_bytes(desc):
     from .lib import raw
-    nbytes = int(raw().b2y_stem_workspace_bytes(C.byref(desc)))
-    return torch.empty((nbytes // 2,), dtype=torch.float16, device=device)
+    return int(raw().b2y_stem_workspace_bytes(C.byref(desc)))
+
+
+def stem_workspace(desc, device):
+    return torch.empty((stem_workspace_bytes(desc) // 2,), dtype=torch.float16, device=device)
 
 
 def stem_conv_tc(x_nchw, w_stem, bias, in_c, k, stride, pad, act="linear", slope=0.1, out=None, workspace=None,

@@ -176,5 +176,4 @@ class FlatDataParallel:
         self.steps += 1
         eng = self.module.__dict__.get('_engine')
         if eng is not None:
-            for plan in eng.plans.values():
-                plan.param_version = None    # weights changed through the flat buffer: re-pack on the next forward
+            eng.weights_changed()            # weights changed through the flat buffer: re-pack on the next forward

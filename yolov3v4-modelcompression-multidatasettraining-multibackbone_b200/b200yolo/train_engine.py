@@ -18,12 +18,13 @@ loss.backward(), DistributedDataParallel hooks and torch optimisers work unchang
 import ctypes as C
 
 import os
+import weakref
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import LazyFeatures, _Tensor, _block_parts
+from .engine import LazyFeatures, SlotStore, _Tensor, _block_parts
 from .lib import ACT, ConvDesc, OUT_F16, call, ptr, stream_ptr
 
 GDT = torch.bfloat16   # gradient tensors: bf16 (range of fp32) -- fp16 over/underflows across ~100 BN layers
@@ -50,16 +51,51 @@ class _ConvRec:
             setattr(self, k, None)
 
 
+class TrainShared:
+    """Training state of one model that does not depend on the input shape, shared by its plans of every shape: the
+    packed fp16 weights and data-gradient slabs (`w16`, `wT`) and the stem's packed weights, keyed by layer index, with
+    their pack tables; the OIHW fp32 gradient outputs of the plain-autograd path; and the side stream of the weight
+    gradients, so that one split-K workspace (`stream_ws`, keyed by stream) serves every plan."""
+
+    def __init__(self, device):
+        self.device = device
+        self.w16, self.wT, self.wstem = {}, {}, {}
+        self.pack_tables = {}
+        self.own_grads = {}
+        self.side_stream = None
+
+
+class _Pin:
+    """Holds a SlotStore for one training forward until its backward has run or its autograd graph is freed.  The
+    step's autograd node owns the pin; the store only keeps a weak reference, so freeing the graph frees the pin."""
+
+    def __init__(self, store, plan):
+        self.store, self.plan = store, plan
+        store.pin = weakref.ref(self)
+
+    def release(self):
+        if self.store.pin is not None and self.store.pin() is self:
+            self.store.pin = None
+
+
 class TrainPlan:
-    def __init__(self, model, x_shape, device, keep_features=False):
+    def __init__(self, model, x_shape, device, keep_features=False, store=None, shared=None):
         self.model = model
         self.device = device
         self.keep_features = bool(keep_features)
         self.B, self.Cin, self.H, self.W = x_shape
+        self.store = store if store is not None else SlotStore(device)
+        self.shared = shared if shared is not None else TrainShared(device)
+        self.held = {}          # slot name -> version taken
         self.convs = []
         self.order = []        # forward step list
         self.param_version = None
         self._build()
+
+    def _take(self, name, shape, dtype):
+        t = self.store.take(name, shape, dtype)
+        self.held[name] = self.store.versions[name]
+        return t
 
     # ---------------------------------------------------------------------------------------------------------
     def _build(self):
@@ -132,13 +168,11 @@ class TrainPlan:
         placed, copies = set(), {}
         self.bufs = []   # (activation buffer, gradient buffer) pairs to keep alive
 
-        def new_buf(Cc, H, W, dtype=torch.float16):
-            if dtype != torch.float16:
-                return torch.empty((B, H, W, _round_up(Cc, 4)), dtype=dtype, device=dev)
-            if Cc % 16 == 0:
-                return torch.empty((B, H, W, Cc), dtype=dtype, device=dev)
-            # MobileNet widths (24, 40, 72 ...): pitch rounded up to the MMA K granule, pad channels stay zero forever
-            return torch.zeros((B, H, W, _round_up(Cc, 16)), dtype=dtype, device=dev)
+        def new_buf(name, Cc, H, W, dtype=torch.float16):
+            # fp16: MobileNet widths (24, 40, 72 ...) get a pitch rounded up to the MMA K granule, pad channels stay
+            # zero forever (slots are zero-filled and the pitch depends on the width only)
+            pitch = _round_up(Cc, 4 if dtype != torch.float16 else 16)
+            return self._take((name, pitch, dtype), (B, H, W, pitch), dtype)
 
         def zeros_later(shape, dtype):
             """placeholder (meta tensor) for a buffer that is carved out of the zero-at-start-of-backward arena"""
@@ -157,7 +191,7 @@ class TrainPlan:
                 continue
             srcs = [i + l if l < 0 else l for l in d['layers']]
             dst = tens[i]
-            dst.buf = new_buf(dst.C, dst.H, dst.W)
+            dst.buf = new_buf(('cat', i), dst.C, dst.H, dst.W)
             gdst = make_grad(dst, zeros_later(dst.buf.shape, GDT))
             off = 0
             for s in srcs:
@@ -171,9 +205,9 @@ class TrainPlan:
                     copies.setdefault(i, []).append((st, off))
                 off += st.C
 
-        def alloc(t):
+        def alloc(t, i):
             if t.buf is None:
-                t.buf = new_buf(t.C if t.dtype == torch.float16 else HEAD_PAD, t.H, t.W, t.dtype)
+                t.buf = new_buf(('act', i), t.C if t.dtype == torch.float16 else HEAD_PAD, t.H, t.W, t.dtype)
                 t.c0 = 0
             if id(t) not in self.grad_of:
                 if t.dtype == torch.float16:
@@ -192,10 +226,11 @@ class TrainPlan:
             if t == 'se':
                 fc = m[0].fc if isinstance(m, nn.Sequential) else m.fc
                 src = tens[i - 1]
-                out = alloc(tens[i])
+                out = alloc(tens[i], i)
                 cr = fc[0].out_features
                 rec = {'i': i, 'src': src, 'y': out, 'fc1': fc[0], 'fc2': fc[2],
-                       'ws': ops.se_workspace(B, src.C, cr, dev), 'ws_bwd': ops.se_workspace(B, src.C, cr, dev)}
+                       'ws': self._take(('se_ws', i), (B, 3 * src.C + cr), torch.float32),
+                       'ws_bwd': self._take(('se_ws_bwd', i), (B, 3 * src.C + cr), torch.float32)}
                 self.order.append(('se', rec))
                 feat_idx[i] = out
             elif t in ('convolutional', 'depthwise'):
@@ -219,7 +254,7 @@ class TrainPlan:
                 if r.head and (r.Cout > HEAD_PAD or bn is not None or act != 'linear'):
                     raise NotImplementedError("unsupported YOLO head conv")
                 r.src = None if i == 0 else tens[i - 1]
-                r.y = alloc(tens[i])
+                r.y = alloc(tens[i], i)
                 if i + 1 < n and fused_into[i + 1] == i:
                     l = defs[i + 1]['from'][0]
                     r.res = tens[i + 1 + l if l < 0 else l]
@@ -229,7 +264,7 @@ class TrainPlan:
                         raise NotImplementedError("layer %d: BatchNorm training needs a multiple of 8 channels, at most "
                                                   "2048 (got %d)" % (i, r.Cout))
                     r.z = _Tensor(r.Cout, r.y.H, r.y.W)
-                    r.z.buf = new_buf(r.Cout, r.y.H, r.y.W)
+                    r.z.buf = new_buf(('z', i), r.Cout, r.y.H, r.y.W)
                     r.stats = zeros_later((2, r.Cout), torch.float32)
                     r.sums = zeros_later((2, r.Cout), torch.float32)
                 else:
@@ -249,7 +284,7 @@ class TrainPlan:
                 frm = [i + l if l < 0 else l for l in d['from']]
                 if getattr(m, 'weight', False):
                     raise NotImplementedError("weighted shortcut is not supported yet")
-                out = alloc(tens[i])
+                out = alloc(tens[i], i)
                 self.order.append(('add', tens[i - 1], [tens[s] for s in frm], out))
             elif t == 'route':
                 if len(d['layers']) == 1:
@@ -262,10 +297,10 @@ class TrainPlan:
                 for st, off in copies.get(i, []):
                     self.order.append(('copy', st, tens[i], off))
             elif t == 'upsample':
-                self.order.append(('upsample', tens[i - 1], alloc(tens[i]), d['stride']))
+                self.order.append(('upsample', tens[i - 1], alloc(tens[i], i), d['stride']))
             elif t == 'maxpool':
                 k, s = d['size'], d['stride']
-                self.order.append(('maxpool', tens[i - 1], alloc(tens[i]), k, s, k == 2 and s == 1))
+                self.order.append(('maxpool', tens[i - 1], alloc(tens[i], i), k, s, k == 2 and s == 1))
                 if m.__class__.__name__ == 'Sequential':
                     feat_idx[i] = tens[i]
             elif t == 'yolo':
@@ -308,18 +343,27 @@ class TrainPlan:
             want(bwd_req, r, 'dwg')
         want(bwd_req, self, 'dz_aux')
 
-        # gradient buffers whose first writer overwrites (see _plan_grad_writes) go behind the part that is memset
+        # gradient buffers whose first writer overwrites (see _plan_grad_writes) go behind the part that is memset.  The
+        # arena is a slot that plans of other shapes lay out differently, so bytes behind the memset hold whatever the
+        # last plan wrote there: a buffer with pad channels (MobileNet widths) stays in the memset part to keep its
+        # pad zero.
+        width = {}
+        for g in self.grad_of.values():
+            width[id(g.buf)] = max(width.get(id(g.buf), 0), g.c0 + g.C)
+        for g in self.grad_of.values():
+            if g.buf.shape[-1] > width[id(g.buf)]:
+                self.dirty_grad_bufs.add(id(g.buf))
         grad_ids = {id(g.buf) for g in self.grad_of.values()}
         is_clean = lambda t: id(t) in grad_ids and id(t) not in self.dirty_grad_bufs
         bwd_req = [t for t in bwd_req if not is_clean(t)] + [t for t in bwd_req if is_clean(t)]
         self.bwd_zero_bytes = sum(_round_up(t.numel() * t.element_size(), 256) for t in bwd_req if not is_clean(t))
 
-        def carve(reqs):
+        def carve(name, reqs):
             offs, total = [], 0
             for t in reqs:
                 offs.append(total)
                 total += _round_up(t.numel() * t.element_size(), 256)
-            arena = torch.zeros(max(total, 256), dtype=torch.uint8, device=dev)
+            arena = self._take(name, (max(total, 256),), torch.uint8)
             for t, off in zip(reqs, offs):
                 nbytes = t.numel() * t.element_size()
                 real = arena[off:off + nbytes].view(t.dtype).view(t.shape)
@@ -327,25 +371,42 @@ class TrainPlan:
                     setattr(holder, attr, real)
             return arena
 
-        self.fwd_arena = carve(fwd_req)
-        self.bwd_arena = carve(bwd_req)
+        self.fwd_arena = carve(('fwd_arena',), fwd_req)
+        self.bwd_arena = carve(('bwd_arena',), bwd_req)
         # BatchNorm statistics saved by the forward for the backward: [mean, invstd, scale, shift] per layer
         for r in self.convs:
             if r.bn is not None:
                 r.save = torch.empty((4, r.Cout), dtype=torch.float32, device=dev)
         # The weight gradients hang off the critical path (dz_i -> dW_i has no consumer until the optimiser), so they run
         # on a second stream concurrently with the data-gradient / BatchNorm chain.  dz is therefore kept per layer
-        # (no buffer shared between a running wgrad and the next layer's BN backward).
+        # (no buffer shared between a running wgrad and the next layer's BN backward).  The pitch is Cout rounded up to
+        # the K granule of the data-gradient GEMM; the pad channels stay zero.
         self.dz_bufs = {}
-        self.side_stream = None
+        for r in self.convs:
+            if r.bn is not None:
+                full = self._take(('dz', r.i, r.Cpad), (B, r.y.H, r.y.W, r.Cpad), torch.float16)
+                self.dz_bufs[r.i] = full[..., :r.Cout]
         maxc = max(r.Cpad for r in self.convs)
         self.db_scratch = torch.empty(maxc, dtype=torch.float32, device=dev)
         self.stem_dw = torch.empty(maxc * 32, dtype=torch.float32, device=dev)
         self.params = [p for p in model.parameters()]
-        # plan-owned gradient outputs for the plain-autograd path (no flat sink): OIHW fp32 per parameter
-        self.own_grads = None
-        self.pack_table = self.unpack_table = None
-        self.pack_key = self.unpack_key = None
+        for r in self.convs:
+            if not r.stem and not r.depthwise:
+                # zero-filled once: the K-pad columns (>= I) and pad rows (>= O) are never written again
+                O, I, k = r.conv.weight.shape[0], r.conv.weight.shape[1], r.k
+                if r.i not in self.shared.w16:
+                    self.shared.w16[r.i] = torch.zeros((r.Cpad, k, k, r.Ipad), dtype=torch.float16, device=dev)
+                    self.shared.wT[r.i] = torch.zeros(r.Cpad * I * k * k, dtype=torch.float16, device=dev)
+                r.w16, r.wT = self.shared.w16[r.i], self.shared.wT[r.i]
+        # the graph input and the tensor-core stem's im2col workspace (kept for the weight gradient) are taken here, not
+        # on first use, so that a larger shape grows every slot while its plan is built
+        self.static_x = self._take(('x',), (B, self.Cin, self.H, self.W), torch.float32)
+        st = self.convs[0]
+        if st.stem and st.bn is not None and not st.head and st.conv.in_channels * st.k * st.k <= 32:
+            d = ops.make_conv_desc((B, self.H, self.W, st.conv.in_channels), st.conv.in_channels, st.Cout, st.k, st.s,
+                                   st.p, st.Cout)
+            self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,), torch.float16)
+        self.unpack_table = self.unpack_key = None
         self.runs = 0
         self.fwd_graph = self.bwd_graph = None
         self.bwd_key = None
@@ -360,14 +421,13 @@ class TrainPlan:
         from .lib import PackItem, raw
         body = [r for r in self.convs if not r.stem and not r.depthwise]
         key = tuple(r.conv.weight.data_ptr() for r in body)
-        if self.pack_table is None or key != self.pack_key:
+        # one table per set of weight pointers, kept for the life of the shared state: captured graphs of every plan
+        # read the table they were captured with
+        table = self.shared.pack_tables.get(key)
+        if table is None:
             items, tiles = [], 0
             for r in body:
                 O, I, k = r.conv.weight.shape[0], r.conv.weight.shape[1], r.k
-                if r.w16 is None:
-                    # zero-filled once: the K-pad columns (>= I) and pad rows (>= O) are never written again
-                    r.w16 = torch.zeros((r.Cpad, k, k, r.Ipad), dtype=torch.float16, device=self.device)
-                    r.wT = torch.zeros(r.Cpad * I * k * k, dtype=torch.float16, device=self.device)
                 w = r.conv.weight.detach()
                 assert w.is_contiguous() and w.dtype == torch.float32
                 ti = int(raw().b2y_layout_tile_i(k))
@@ -378,9 +438,8 @@ class TrainPlan:
                 tiles += ((r.Cpad + 31) // 32) * ((I + ti - 1) // ti)
             arr = (PackItem * len(items))(*items)
             host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-            self.pack_table = (host.to(self.device), len(items), tiles)
-            self.pack_key = key
-        tab, n, tiles = self.pack_table
+            table = self.shared.pack_tables[key] = (host.to(self.device), len(items), tiles)
+        tab, n, tiles = table
         call("b2y_pack_conv_weights_multi", ptr(tab), n, tiles, stream_ptr())
         for r in self.convs:
             if r.stem:
@@ -390,7 +449,12 @@ class TrainPlan:
                     w = torch.cat([w, pad], 0)
                 r.w32 = w.float().contiguous()
                 # tensor-core stem: full-im2col weight layout when the receptive field fits one 64-byte GEMM row
-                r.wstem = ops.pack_stem_weights(r.w32) if w.shape[1] * r.k * r.k <= 32 and not r.head else None
+                if w.shape[1] * r.k * r.k <= 32 and not r.head:
+                    if r.i not in self.shared.wstem:
+                        self.shared.wstem[r.i] = torch.empty((r.Cout, 32), dtype=torch.float16, device=self.device)
+                    r.wstem = ops.pack_stem_weights(r.w32, out=self.shared.wstem[r.i])
+                else:
+                    r.wstem = None
 
     def _plan_grad_writes(self):
         """Which backward write into an activation-gradient buffer is the FIRST one of its channel range.
@@ -469,12 +533,10 @@ class TrainPlan:
             d = self.sink.get(id(param))
             if d is not None:
                 return d
-        if self.own_grads is None:
-            self.own_grads = {}
-        d = self.own_grads.get(id(param))
+        d = self.shared.own_grads.get(id(param))
         if d is None:
             d = torch.zeros_like(param, dtype=torch.float32, memory_format=torch.contiguous_format)
-            self.own_grads[id(param)] = d
+            self.shared.own_grads[id(param)] = d
         return d
 
     def _unpack_all(self):
@@ -514,7 +576,6 @@ class TrainPlan:
             self.runs += 1
             return self.forward(x)
         if self.fwd_graph is None:
-            self.static_x = torch.empty((self.B, self.Cin, self.H, self.W), dtype=torch.float32, device=self.device)
             self.static_x.copy_(x)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
@@ -610,10 +671,6 @@ class TrainPlan:
         if r.stem and getattr(r, 'wstem', None) is not None:
             # im2col workspace [B*Ho*Wo][32] fp16 (kept for the weight gradient) + one-k-step GEMM with the BN sums
             # coming out of its epilogue
-            d = ops.make_conv_desc((self.B, self.H, self.W, r.conv.in_channels), r.conv.in_channels, r.Cout, r.k, r.s,
-                                   r.p, r.Cout)
-            if getattr(self, 'stem_ws', None) is None:
-                self.stem_ws = ops.stem_workspace(d, self.device)
             ops.stem_conv_tc(x, r.wstem, None, r.conv.in_channels, r.k, r.s, r.p, act='linear', out=z,
                              workspace=self.stem_ws, stats=(r.stats[0], r.stats[1]))
         elif r.stem:
@@ -650,8 +707,9 @@ class TrainPlan:
         self.sink = getattr(self.model, '_b2y_grad_sink', None)   # FlatDataParallel: write into the flat buffer
         # one memset: BN sums, scale rows, packed weight gradients and the activation gradients that are accumulate-only
         self.bwd_arena[:max(self.bwd_zero_bytes, 1)].zero_()
-        if self.side_stream is None:
-            self.side_stream = torch.cuda.Stream(device=self.device)
+        if self.shared.side_stream is None:
+            self.shared.side_stream = torch.cuda.Stream(device=self.device)
+        self.side_stream = self.shared.side_stream
         grads = {}
         # head gradients are GEMM operands (fp16): scale them by a power of two derived on the device from max|dp|
         live = [dp for dp in dps if dp is not None]
@@ -707,10 +765,10 @@ class TrainPlan:
                      self.B, src.H, src.W, src.C, int(k), int(s), 1 if tiny else 0, ops._gdt(gy), stream_ptr())
         torch.cuda.current_stream().wait_stream(self.side_stream)          # join: every weight gradient is complete
         self._unpack_all()
-        if self.own_grads:
-            # plain-autograd path: hand out copies (the plan-owned buffers are overwritten by the next step)
+        if self.shared.own_grads:
+            # plain-autograd path: hand out copies (the shared buffers are overwritten by the next step)
             by_id = {id(p): p for p in self.params}
-            for pid, g in self.own_grads.items():
+            for pid, g in self.shared.own_grads.items():
                 grads[by_id[pid]] = g
         return grads
 
@@ -727,11 +785,7 @@ class TrainPlan:
                     ops.copy_channels(dy, gs)
                 else:
                     ops.add(gs, dy, out=gs)
-            dz = self.dz_bufs.get(r.i)
-            if dz is None:
-                # pitch = Cout rounded up to the K granule of the data-gradient GEMM; the pad channels stay zero
-                full = torch.zeros((B, Ho, Wo, r.Cpad), dtype=torch.float16, device=self.device)
-                dz = self.dz_bufs[r.i] = full[..., :r.Cout]
+            dz = self.dz_bufs[r.i]
             aux = self.dz_aux[r.aux_row]
             inv_s = aux[2:3]                                   # device scalar 1/s of this layer's dz
             z = r.z.view()
@@ -793,8 +847,11 @@ class TrainPlan:
 
     # ---------------------------------------------------------------------------------------------------------
     def run(self, x):
-        """autograd entry: returns (yolo_out list, feature_out)."""
+        """autograd entry: returns (yolo_out list, feature_out).  While the step's backward is pending (autograd
+        recorded it), the plan's slot store is pinned: the engine runs plans of other shapes on private storage."""
         outs = _DarknetTrain.apply(self, x, *self.params)
+        if outs[0].grad_fn is not None:
+            outs[0].grad_fn.b2y_pin = _Pin(self.store, self)   # released by backward or when the graph is freed
         # the running statistics were just updated through raw pointers (also under graph replay): eval plans re-fold
         object.__setattr__(self.model, '_b2y_epoch', getattr(self.model, '_b2y_epoch', 0) + 1)
         feats = LazyFeatures([None if t is None else t.view() for t in self.feature_views])
@@ -815,6 +872,9 @@ class _DarknetTrain(torch.autograd.Function):
         plan = ctx.plan
         with torch.no_grad():
             grads = plan.backward_graphed(dps)
+        pin = getattr(ctx, 'b2y_pin', None)
+        if pin is not None:
+            pin.release()
         out = []
         for p in ctx.params:
             g = grads.get(p)

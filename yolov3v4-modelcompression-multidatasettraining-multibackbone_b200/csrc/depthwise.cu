@@ -496,11 +496,12 @@ extern "C" int b2y_se_fwd(const void* x, long long x_pitch, const float* w1, con
     if (!x || !w1 || !w2 || !y || !ws || batch <= 0 || hw <= 0 || cr <= 0) return B2Y_ERR_INVALID;
     if (!vec_ok(c, x_pitch, y_pitch)) return B2Y_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // workspace layout: pooled sum / mean [N][C] | h [N][Cr] | v [N][C] | s [N][C]
+    // workspace layout: pooled sum / mean [N][C] | v [N][C] | s [N][C] | h [N][Cr].  h goes last: se_scale_kernel
+    // reads s with float4 loads, and N * Cr is not a multiple of 4 for every batch (e.g. N = 3, Cr = 18)
     float* pooled = ws;
-    float* h = pooled + (long long)batch * c;
-    float* v = h + (long long)batch * cr;
+    float* v = pooled + (long long)batch * c;
     float* s = v + (long long)batch * c;
+    float* h = s + (long long)batch * c;
     B2Y_CUDA_CHECK(cudaMemsetAsync(pooled, 0, sizeof(float) * (size_t)batch * c, st));
     const Geo g = geo_for(c);
     int gx = (hw + g.PPB - 1) / g.PPB;
@@ -526,10 +527,10 @@ extern "C" int b2y_se_bwd(const void* x, long long x_pitch, const void* dy, long
     if (!x || !dy || !w1 || !w2 || !ws || !ws_bwd || !dx || !dw1 || !dw2) return B2Y_ERR_INVALID;
     if (!vec_ok(c, x_pitch, dy_pitch) || dx_pitch % 8 != 0) return B2Y_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const float* mean = ws;
-    const float* h = mean + (long long)batch * c;
-    const float* v = h + (long long)batch * cr;
+    const float* mean = ws;                               // layout of b2y_se_fwd
+    const float* v = mean + (long long)batch * c;
     const float* s = v + (long long)batch * c;
+    const float* h = s + (long long)batch * c;
     float* ds = ws_bwd;                                   // [N][C]  sum dy*x, then reused as dv
     float* dh = ds + (long long)batch * c;                // [N][Cr]
     float* dmean = dh + (long long)batch * cr;            // [N][C]
