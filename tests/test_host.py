@@ -156,6 +156,96 @@ def test_cpu_tensors_fail_loudly():
         my_utils.compute_loss([torch.zeros(1, 3, 2, 2, 85)], torch.zeros(0, 6), m)
 
 
+_LAYOUT_CFG = """
+[net]
+width=96
+height=96
+channels=3
+""" + "".join("\n[%s]\n%s\n" % (kind, "\n".join(opts.split())) for kind, opts in (
+    ("convolutional", "batch_normalize=1 filters=16 size=3 stride=1 pad=1 activation=leaky"),     # 0
+    ("convolutional", "batch_normalize=1 filters=32 size=3 stride=2 pad=1 activation=leaky"),     # 1
+    ("route", "layers=-1 groups=2 group_id=1"),                                                   # 2 upper half of 1
+    ("convolutional", "batch_normalize=1 filters=16 size=3 stride=1 pad=1 activation=leaky"),     # 3
+    ("convolutional", "batch_normalize=1 filters=16 size=3 stride=1 pad=1 activation=leaky"),     # 4
+    ("route", "layers=-1,-2"),                                                                    # 5
+    ("convolutional", "batch_normalize=1 filters=32 size=1 stride=1 pad=1 activation=leaky"),     # 6
+    ("route", "layers=-6,-1"),                                                                    # 7 = [1 | 6]
+    ("maxpool", "size=2 stride=2"),                                                               # 8
+    ("convolutional", "batch_normalize=1 filters=32 size=1 stride=1 pad=1 activation=leaky"),     # 9
+    ("convolutional", "batch_normalize=1 filters=64 size=3 stride=1 pad=1 activation=leaky"),     # 10
+    ("shortcut", "from=-2 activation=linear"),                                                    # 11 addend narrower
+    ("route", "layers=-1"),                                                                       # 12 = 11
+    ("route", "layers=-1"),                                                                       # 13 = 12 = 11
+    ("convolutional", "batch_normalize=1 filters=32 size=1 stride=1 pad=1 activation=leaky"),     # 14
+    ("route", "layers=-1,-3"),                                                                    # 15 = [14 | 11]
+    ("convolutional", "batch_normalize=1 filters=32 size=1 stride=1 pad=1 activation=leaky"),     # 16
+    ("route", "layers=-1,11"),                                                                    # 17: 11 is taken
+    ("convolutional", "batch_normalize=1 filters=64 size=3 stride=1 pad=1 activation=leaky"),     # 18
+    ("convolutional", "batch_normalize=1 filters=64 size=1 stride=1 pad=1 activation=leaky"),     # 19
+    ("convolutional", "batch_normalize=1 filters=64 size=3 stride=1 pad=1 activation=leaky"),     # 20
+    ("shortcut", "from=-3 activation=linear"),                                                    # 21 into conv 20
+    ("convolutional", "filters=64 size=1 stride=1 pad=1 activation=linear"),                      # 22 no BatchNorm
+    ("shortcut", "from=-2 activation=linear"),                                                    # 23
+    ("convolutional", "filters=255 size=1 stride=1 pad=1 activation=linear"),                     # 24
+    ("yolo", "mask=0,1,2 anchors=10,14,23,27,37,58,81,82,135,169,344,319 classes=80 num=6")))     # 25
+
+
+def test_layout_is_decided_once_for_inference_and_training():
+    """b200yolo.layout on the CPU: shapes, folded shortcuts per mode, aliases, zero-copy concat placement."""
+    import models
+    from b200yolo import layout
+    from utils.parse_config import parse_model_cfg_text
+
+    def layouts(model, chw=(3, 96, 160)):
+        shapes = layout.infer_shapes(model, chw)
+        bn_of = lambda i: layout._block_parts(model.module_list[i])[1]
+        return (layout.build_layout(model, shapes, False, lambda i: shapes[i][0] % 8 == 0),
+                layout.build_layout(model, shapes, False, lambda i: bn_of(i) is not None),
+                layout.build_layout(model, shapes, True, lambda i: True))
+    n_fused = lambda lay: sum(f is not None for f in lay.fused_into)
+
+    # shortcuts folded into the conv before them (inference, training, keep_features), feature_out entries
+    for name, want in (("yolov3", (23, 23, 0, 72)), ("yolov3-tiny", (0, 0, 0, 12)), ("yolov4", (23, 23, 0, 107)),
+                       ("yolov3-mobilenet", (10, 10, 0, 75))):
+        model = models.Darknet(cfg_path(name))
+        inf, trn, keep = layouts(model)
+        assert (n_fused(inf), n_fused(trn), n_fused(keep), len(layout.feature_slots(model))) == want, name
+        if name == "yolov4":    # every concat source is written in place, SPP included
+            assert sorted(inf.concats) == [9, 22, 53, 84, 103, 113, 121, 131, 142, 153]
+            assert all(placed for parts in inf.concats.values() for _, _, placed in parts)
+            assert [off for _, off, _ in inf.concats[113]] == [0, 512, 1024, 1536]
+            assert inf.shapes[113] == (2048, 3, 5)
+        if name == "yolov3-tiny":   # the 2/1 max-pool keeps the size
+            assert inf.shapes[10] == inf.shapes[11] == (512, 3, 5)
+        if name == "yolov3-mobilenet":
+            odd = sorted({(t.C, layout.pitch(t.C, t.dtype)) for t in inf.tens if t is not None and t.C % 16})
+            assert odd == [(24, 32), (40, 48), (72, 80), (120, 128), (168, 176), (184, 192), (200, 208), (255, 256)]
+
+    model = models.Darknet(parse_model_cfg_text(_LAYOUT_CFG))
+    inf, trn, keep = layouts(model)
+    assert (n_fused(inf), n_fused(trn), n_fused(keep)) == (2, 1, 0)     # conv 22 has no BatchNorm
+    assert inf.fused_into[21] == trn.fused_into[21] == 20 and inf.fused_into[11] is None
+    assert inf.fused_into[23] == 22 and trn.fused_into[23] is None
+    for lay in (inf, trn):
+        t = lay.tens
+        assert lay.shapes[2] == (16, 48, 80) and lay.shapes[8] == (64, 24, 40) and lay.shapes[17] == (96, 24, 40)
+        assert t[12] is t[11] and t[13] is t[11] and t[20] is t[21] and t[25] is None
+        # conv 1 sits at the start of concat 7; the grouped route is the upper half of its channels, same buffer
+        assert lay.concats[7] == [(t[1], 0, True), (t[6], 32, True)]
+        assert lay.grouped == {2: t[1]} and (t[2].c0, t[2].C) == (t[1].c0 + 16, 16)
+        assert lay.concats[5] == [(t[4], 0, True), (t[3], 16, True)]
+        assert lay.concats[15] == [(t[14], 0, True), (t[11], 32, True)]
+        assert lay.concats[17] == [(t[16], 0, True), (t[11], 32, False)]     # already inside concat 15: copied
+        assert t[11].c0 == 32 and t[24].dtype == torch.float32 and lay.is_head[24]
+
+    model = models.Darknet(parse_model_cfg_text(_LAYOUT_CFG.replace("[maxpool]", "[reorg3d]")))
+    with pytest.raises(NotImplementedError, match="reorg3d"):
+        layout.infer_shapes(model, (3, 96, 96))
+    with pytest.raises(NotImplementedError, match="int8 graph"):
+        layout.infer_shapes(models.Darknet(cfg_path("yolov3-tiny")), (3, 96, 96), ('convolutional', 'yolo'),
+                            "layer type '%s' in the int8 graph")
+
+
 @pytest.mark.parametrize("name", ["yolov3", "yolov3-tiny", "yolov4", "yolov3-mobilenet"])
 def test_generated_cfg_equals_reference_cfg(name):
     """the generated cfgs against the reference's own .cfg files, as parsed (tests/golden/ref_cfg_layers.json,

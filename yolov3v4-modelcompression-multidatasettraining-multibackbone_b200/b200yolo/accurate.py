@@ -17,7 +17,8 @@ this verification mode).
 import torch
 
 from . import ops
-from .engine import _block_parts
+from .engine import LazyFeatures, fold_bn
+from .layout import _block_parts, feature_slots
 
 
 class AccurateRunner:
@@ -31,14 +32,11 @@ class AccurateRunner:
         if c is not None and c[0] == key:
             return c[1]
         w = conv.weight.detach().float()
-        if bn is not None:
-            s = (bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)).float()
-            b = (bn.bias.detach() - bn.running_mean * s).float()
-            if conv.bias is not None:
-                b = b + conv.bias.detach().float() * s
+        s, b = fold_bn(conv, bn)
+        if s is not None:
             w = w * s.view(-1, 1, 1, 1)
-        else:
-            b = conv.bias.detach().float() if conv.bias is not None else torch.zeros(w.shape[0], device=w.device)
+        if b is None:
+            b = torch.zeros(w.shape[0], device=w.device)
         I = w.shape[1]
         Ik = (I + 15) // 16 * 16
         if Ik != I:
@@ -67,7 +65,6 @@ class AccurateRunner:
 
     @torch.no_grad()
     def forward(self, x):
-        from .engine import LazyFeatures
         model = self.model
         if model.training:
             raise RuntimeError("model.accurate is an inference-only verification mode")
@@ -121,6 +118,4 @@ class AccurateRunner:
             else:
                 raise NotImplementedError("layer type '%s' in the accurate mode" % t)
             outs.append(h if model.routs[i] else None)
-        nfeat = sum(1 for j, mm in enumerate(mods) if mm.__class__.__name__ == 'Sequential' and j + 1 < len(defs)
-                    and defs[j + 1]['type'] != 'yolo')
-        return torch.cat(io_list, 1), tuple(p_list), LazyFeatures([None] * nfeat)
+        return torch.cat(io_list, 1), tuple(p_list), LazyFeatures([None] * len(feature_slots(model)))

@@ -9,17 +9,86 @@ by a static plan over NHWC fp16 buffers:
   * the launch sequence is captured once into a CUDA graph per input shape and replayed.
 
 Parameters stay in the nn.Module tree (fp32, NCHW) and are folded/packed on the device whenever they change.
+Shapes, folded shortcuts and the concat placement come from layout.py, which the training plan shares.
 """
+import collections
 import os
 
 import torch
 import torch.nn as nn
 
 from . import ops
+from .layout import _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources
 from .lib import WLAYOUT_S2_PAIRS
 
-_ACT_OF_CLASS = {'LeakyReLU': 'leaky', 'Mish': 'mish', 'ReLU6': 'relu6', 'HardSwish': 'h_swish', 'ReLU': 'relu',
-                 'Swish': 'swish'}
+
+# ---- launch list vocabulary: field 0 is the step's kind; src / out / res / dst are layout._Tensor -------------------
+# conv: src is None for the stem (it reads the image), res is the source of the shortcut folded into the conv, or None
+ConvStep = collections.namedtuple('ConvStep', 'kind i src out res conv bn act slope')
+DwStep = collections.namedtuple('DwStep', 'kind i src out conv bn act slope')
+SeStep = collections.namedtuple('SeStep', 'kind i src out fc1 fc2 ws')
+# out = first + others[0] + ...; widths may differ (layers.py:57-72): a sum covers the first min(nx, na) channels, the
+# rest of x passes through
+AddStep = collections.namedtuple('AddStep', 'kind first others out')
+# a concat source that could not be placed inside the concat buffer `dst`: copied to channel offset `off`
+CopyStep = collections.namedtuple('CopyStep', 'kind src dst off')
+UpsampleStep = collections.namedtuple('UpsampleStep', 'kind src out stride')
+# tiny_pad: k = 2, s = 1 (yolov3-tiny), padded on the right / bottom only
+MaxpoolStep = collections.namedtuple('MaxpoolStep', 'kind src out k s tiny_pad')
+
+
+def pointwise_steps(lay, i, d, m, alloc):
+    """The steps of layer i when it is a shortcut, route, up-sample or max-pool (the same in inference and training);
+    `alloc(tensor, i)` binds the plan's buffer of a tensor that has none yet and returns the tensor."""
+    t, tens = d['type'], lay.tens
+    if t == 'shortcut':
+        if lay.fused_into[i] is not None:
+            return []
+        if getattr(m, 'weight', False):
+            raise NotImplementedError("weighted shortcut is not supported by the sm_90a engine yet")
+        return [AddStep('add', tens[i - 1], [tens[s] for s in sources(i, d['from'])], alloc(tens[i], i))]
+    if t == 'route':
+        if i in lay.grouped:
+            tens[i].buf = lay.grouped[i].buf
+        return [CopyStep('copy', st, tens[i], off) for st, off, placed in lay.concats.get(i, ()) if not placed]
+    if t == 'upsample':
+        return [UpsampleStep('upsample', tens[i - 1], alloc(tens[i], i), d['stride'])]
+    if t == 'maxpool':
+        k, s = d['size'], d['stride']
+        return [MaxpoolStep('maxpool', tens[i - 1], alloc(tens[i], i), k, s, k == 2 and s == 1)]
+    return []
+
+
+def launch_pointwise(st):
+    """Forward launches of an add / copy / upsample / maxpool step."""
+    if st.kind == 'add':
+        cur, ov = st.first, st.out.view()
+        for a in st.others:
+            xv, av = cur.view(), a.view()
+            n = min(xv.shape[3], av.shape[3])
+            ops.add(xv[..., :n], av[..., :n], out=ov[..., :n])
+            if xv.shape[3] > n and cur is not st.out:
+                ops.copy_channels(xv[..., n:], ov[..., n:])
+            cur = st.out
+    elif st.kind == 'copy':
+        ops.copy_channels(st.src.view(), st.dst.buf[..., st.off:st.off + st.src.C])
+    elif st.kind == 'upsample':
+        ops.upsample(st.src.view(), st.stride, out=st.out.view())
+    elif st.kind == 'maxpool':
+        ops.maxpool(st.src.view(), st.k, st.s, tiny_pad=st.tiny_pad, out=st.out.view())
+
+
+def fold_bn(conv, bn):
+    """Eval-mode BatchNorm (+ conv bias) as a per-channel (scale, bias) in fp32: y = conv * scale + bias with
+    scale = gamma / sqrt(var + eps), bias = beta - mean * scale (+ conv.bias * scale).  Without a BatchNorm the scale is
+    None and the bias is the conv's (None when it has none)."""
+    if bn is None:
+        return None, conv.bias.detach().float() if conv.bias is not None else None
+    sc = (bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)).float()
+    bi = (bn.bias.detach() - bn.running_mean * sc).float()
+    if conv.bias is not None:
+        bi = bi + conv.bias.detach().float() * sc
+    return sc, bi
 
 
 class LazyFeatures(list):
@@ -41,47 +110,6 @@ class LazyFeatures(list):
 
     def __iter__(self):
         return (self[i] for i in range(len(self)))
-
-
-class _Tensor:
-    """Logical activation tensor: NHWC view = buffer[..., c0:c0+C]."""
-    __slots__ = ('C', 'H', 'W', 'buf', 'c0', 'dtype')
-
-    def __init__(self, C, H, W, dtype=torch.float16):
-        self.C, self.H, self.W, self.dtype = C, H, W, dtype
-        self.buf, self.c0 = None, 0
-
-    def view(self):
-        return self.buf[..., self.c0:self.c0 + self.C]
-
-    def view_k(self):
-        """View for a tensor-core consumer: the channel count rounded up to 16 (the MMA K granule is 16 fp16 elements).
-        MobileNet widths (24, 40, 72, 120, 184, 200) are not: their buffers are allocated zero-filled with a pitch that
-        is a multiple of 16 and nobody ever writes the pad channels, the packed weights carry zero columns there (a
-        tensor living inside a concat buffer may see its neighbour's channels instead of zeros: finite values times
-        zero weights)."""
-        ck = (self.C + 15) // 16 * 16
-        if ck == self.C:
-            return self.view()
-        if self.c0 + ck > self.buf.shape[3]:
-            raise RuntimeError("activation buffer too narrow for the padded channel view (C=%d)" % self.C)
-        return self.buf[..., self.c0:self.c0 + ck]
-
-
-def _block_parts(block):
-    """nn.Sequential conv block -> (conv, bn or None, activation name, slope)."""
-    conv, bn, act, slope = None, None, 'linear', 0.1
-    for m in block:
-        name = m.__class__.__name__
-        if isinstance(m, nn.Conv2d):
-            conv = m
-        elif isinstance(m, nn.BatchNorm2d):
-            bn = m
-        elif name in _ACT_OF_CLASS:
-            act = _ACT_OF_CLASS[name]
-            if name == 'LeakyReLU':
-                slope = m.negative_slope
-    return conv, bn, act, slope
 
 
 class SlotStore:
@@ -141,9 +169,7 @@ class EvalWeights:
 
 
 class Plan:
-    def __init__(self, model, x_shape, device, training, keep_features=False, store=None, shared_weights=None):
-        if training:
-            raise NotImplementedError("training plan is built by b200yolo.train_engine")
+    def __init__(self, model, x_shape, device, keep_features=False, store=None, shared_weights=None):
         self.model = model
         self.keep_features = bool(keep_features)
         self.device = device
@@ -152,7 +178,7 @@ class Plan:
         self.shared_weights = shared_weights if shared_weights is not None else EvalWeights()
         self.held = {}          # slot name -> version taken
         self.steps = []
-        self.wkey = {}          # layer index -> key of its packed weights in shared_weights.packs
+        self.wkey = {}          # layer index -> key (layer index, weight layout) of its pack in shared_weights.packs
         self.param_version = None
         self.graph = None
         self.runs = 0
@@ -166,8 +192,8 @@ class Plan:
 
     def _new_act(self, name, C, H, W):
         """fp16 NHWC activation buffer; widths that are not a multiple of 16 get a zero pad (see _Tensor.view_k)."""
-        pitch = (C + 15) // 16 * 16
-        return self._take(('act', name, pitch, torch.float16), (self.B, H, W, pitch))
+        pc = pitch(C, torch.float16)
+        return self._take(('act', name, pc, torch.float16), (self.B, H, W, pc))
 
     def _w(self, i):
         return self.shared_weights.packs[self.wkey[i]]
@@ -180,118 +206,32 @@ class Plan:
     # ---------------------------------------------------------------------------------------------------------
     def _build(self):
         model, B = self.model, self.B
-        defs, mods, routs = model.module_defs, model.module_list, model.routs
+        defs, mods = model.module_defs, model.module_list
         n = len(defs)
-        dev = self.device
+        shapes = infer_shapes(model, (self.Cin, self.H, self.W))
+        # inference folds a shortcut into the residual epilogue of the conv before it for multiples of 8 channels
+        lay = build_layout(model, shapes, self.keep_features, lambda i: shapes[i][0] % 8 == 0)
+        tens, fused_into = lay.tens, lay.fused_into
 
-        # 1) shapes
-        shapes = []  # (C,H,W) of every layer output
-        prev = (self.Cin, self.H, self.W)
-        for i, (d, m) in enumerate(zip(defs, mods)):
-            t = d['type']
-            C, H, W = prev
-            if t in ('convolutional', 'depthwise'):
-                conv = _block_parts(m)[0]
-                k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-                H, W = ops.conv_out_hw(H, W, k, s, p)
-                C = conv.out_channels
-            elif t == 'se':
-                pass
-            elif t == 'maxpool':
-                k, s = d['size'], d['stride']
-                if k == 2 and s == 1:
-                    H, W = (H + 1 - k) // s + 1, (W + 1 - k) // s + 1
-                else:
-                    p = (k - 1) // 2
-                    H, W = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
-            elif t == 'upsample':
-                H, W = H * d['stride'], W * d['stride']
-            elif t == 'route':
-                srcs = [i + l if l < 0 else l for l in d['layers']]
-                C = sum(shapes[s][0] for s in srcs)
-                if 'groups' in d:
-                    C //= 2
-                H, W = shapes[srcs[0]][1], shapes[srcs[0]][2]
-            elif t in ('shortcut', 'yolo'):
-                pass
-            else:
-                raise NotImplementedError("layer type '%s' is not supported by the sm_90a engine yet" % t)
-            prev = (C, H, W)
-            shapes.append(prev)
-
-        # 2) fusion decisions
-        is_head = [False] * n       # conv directly followed by a yolo layer -> fp32 output
-        fused_into = [None] * n     # shortcut i fused into conv i-1
-        for i, d in enumerate(defs):
-            if d['type'] == 'yolo' and i > 0 and defs[i - 1]['type'] == 'convolutional':
-                is_head[i - 1] = True
-            if d['type'] == 'shortcut' and i > 0:
-                frm = [i + l if l < 0 else l for l in d['from']]
-                if (not self.keep_features  # feature_out must expose the conv output *before* the add
-                        and len(frm) == 1 and defs[i - 1]['type'] == 'convolutional' and not routs[i - 1]
-                        and not getattr(mods[i], 'weight', False) and shapes[frm[0]] == shapes[i - 1]
-                        and shapes[i - 1][0] % 8 == 0 and i - 1 > 0):
-                    fused_into[i] = i - 1
-
-        # 3) logical tensors; aliases for single-source routes
-        tens = [None] * n
-        for i, d in enumerate(defs):
-            t = d['type']
-            if t == 'yolo':
-                continue
-            if t == 'route' and len(d['layers']) == 1 and 'groups' not in d:
-                continue  # alias, resolved below
-            C, H, W = shapes[i]
-            tens[i] = _Tensor(C, H, W, torch.float32 if is_head[i] else torch.float16)
-        for i, d in enumerate(defs):
-            if fused_into[i] is not None:
-                tens[fused_into[i]] = tens[i]  # the conv writes the shortcut's output tensor
-        alias = {}
-        for i, d in enumerate(defs):
-            if d['type'] == 'route' and len(d['layers']) == 1 and 'groups' not in d:
-                l = d['layers'][0]
-                src = i + l if l < 0 else l
-                while src in alias:
-                    src = alias[src]
-                alias[i] = src
-                tens[i] = tens[src]
-
-        # 4) concat placement: multi-source routes become pre-allocated buffers their producers write into
-        placed = set()
-        copies = {}  # route index -> list of (src tensor, channel offset) that must be copied
-        for i, d in enumerate(defs):
-            if d['type'] != 'route' or len(d['layers']) == 1:
-                continue
-            srcs = [i + l if l < 0 else l for l in d['layers']]
+        # multi-source routes are buffers their producers write into
+        for i, parts in lay.concats.items():
             dst = tens[i]
             dst.buf = self._new_act(('cat', i), dst.C, dst.H, dst.W)
-            off = 0
-            for s in srcs:
-                st = tens[s]
-                if (id(st) not in placed and st.buf is None and off % 8 == 0 and st.dtype == torch.float16
-                        and st is not dst):
-                    st.buf, st.c0 = dst.buf, off
-                    placed.add(id(st))
-                else:
-                    copies.setdefault(i, []).append((st, off))
-                off += st.C
-        for i, d in enumerate(defs):  # grouped routes: upper half of the channels of the previous layer
-            if d['type'] == 'route' and 'groups' in d:
-                pass  # resolved at allocation time below (needs the source buffer)
+            for st, off, placed in parts:
+                if placed:
+                    st.buf = dst.buf
 
-        # 5) allocate what is left and emit the launch list
+        # allocate what is left and emit the launch list
         def alloc(t, i):
             if t.buf is None:
                 if t.dtype == torch.float16:
                     t.buf = self._new_act(i, t.C, t.H, t.W)
                 else:
-                    pitch = ((t.C + 3) // 4) * 4
-                    t.buf = self._take(('head', i, pitch, t.dtype), (B, t.H, t.W, pitch), t.dtype)
-                t.c0 = 0
+                    pc = pitch(t.C, t.dtype)
+                    t.buf = self._take(('head', i, pc, t.dtype), (B, t.H, t.W, pc), t.dtype)
             return t
 
         self.yolo = []
-        self.feature_views = []
         row_off = 0
         for i, (d, m) in enumerate(zip(defs, mods)):
             t = d['type']
@@ -299,12 +239,12 @@ class Plan:
                 conv, bn, act, slope = _block_parts(m)
                 if conv.groups != conv.in_channels or conv.out_channels != conv.in_channels:
                     raise NotImplementedError("only channel-multiplier-1 depthwise convolutions are supported")
-                self.steps.append(('dw', i, tens[i - 1], alloc(tens[i], i), conv, bn, act, slope))
+                self.steps.append(DwStep('dw', i, tens[i - 1], alloc(tens[i], i), conv, bn, act, slope))
             elif t == 'se':
                 fc = m[0].fc if isinstance(m, nn.Sequential) else m.fc
                 src = tens[i - 1]
                 ws = self._take(('se_ws', i), (B, 3 * src.C + fc[0].out_features), torch.float32)
-                self.steps.append(('se', i, src, alloc(tens[i], i), fc[0], fc[2], ws))
+                self.steps.append(SeStep('se', i, src, alloc(tens[i], i), fc[0], fc[2], ws))
             elif t == 'convolutional':
                 conv, bn, act, slope = _block_parts(m)
                 if conv.groups != 1:
@@ -312,48 +252,19 @@ class Plan:
                 out = alloc(tens[i], i)
                 res = None
                 if i + 1 < n and fused_into[i + 1] == i:
-                    l = defs[i + 1]['from'][0]
-                    res = tens[i + 1 + l if l < 0 else l]
+                    res = tens[sources(i + 1, defs[i + 1]['from'])[0]]
                 src = None if i == 0 else tens[i - 1]
-                self.steps.append(('conv', i, src, out, res, conv, bn, act, slope))
-            elif t == 'shortcut':
-                if fused_into[i] is not None:
-                    continue
-                frm = [i + l if l < 0 else l for l in d['from']]
-                if getattr(m, 'weight', False):
-                    raise NotImplementedError("weighted shortcut is not supported by the sm_90a engine yet")
-                out = alloc(tens[i], i)
-                cur = tens[i - 1]
-                for s in frm:
-                    # widths may differ (layers.py:57-72): the sum covers the first min(nx, na) channels, the rest of x
-                    # passes through
-                    self.steps.append(('add', cur, tens[s], out))
-                    cur = out
-            elif t == 'route':
-                if len(d['layers']) == 1:
-                    if 'groups' in d:
-                        src = tens[i - 1]
-                        g = tens[i]
-                        g.buf, g.c0 = src.buf, src.c0 + src.C // 2
-                    continue
-                for st, off in copies.get(i, []):
-                    self.steps.append(('copy', st, tens[i], off))
-            elif t == 'upsample':
-                self.steps.append(('upsample', tens[i - 1], alloc(tens[i], i), d['stride']))
-            elif t == 'maxpool':
-                k, s = d['size'], d['stride']
-                self.steps.append(('maxpool', tens[i - 1], alloc(tens[i], i), k, s, k == 2 and s == 1))
+                self.steps.append(ConvStep('conv', i, src, out, res, conv, bn, act, slope))
             elif t == 'yolo':
                 raw = tens[i - 1]
                 rows = m.na * raw.H * raw.W
                 self.yolo.append((m, raw, row_off, rows))
                 row_off += rows
+            else:
+                self.steps += pointwise_steps(lay, i, d, m, alloc)
         self.total_rows = row_off
-        # feature_out (models.py:542-543): every nn.Sequential block whose successor is not a YOLO layer
-        for i, m in enumerate(mods):
-            if m.__class__.__name__ == 'Sequential' and i + 1 < n and defs[i + 1]['type'] != 'yolo':
-                self.feature_views.append(tens[i] if (self.keep_features and tens[i] is not None) else None)
-        self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _, _, _) in self.yolo]
+        self.feature_views = [tens[i] if self.keep_features else None for i in feature_slots(model)]
+        self.anchors_px = [m.anchors.to(self.device).float().contiguous() for (m, _, _, _) in self.yolo]
 
     # ---------------------------------------------------------------------------------------------------------
     def _params_version(self):
@@ -375,26 +286,17 @@ class Plan:
             sw.version = ver
         packs = sw.packs
         for st in self.steps:
-            if st[0] == 'dw':
-                _, i, src, out, conv, bn, act, slope = st
-                key = self.wkey[i] = (i, 'dw')
-                if key in packs:
-                    continue
-                w = conv.weight.detach().float().contiguous()
-                if bn is not None:           # fold: y = conv * gamma/sqrt(var+eps) + (beta - mean*gamma/sqrt(var+eps))
-                    sc = (bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)).float()
-                    bi = (bn.bias.detach() - bn.running_mean * sc).float()
-                    if conv.bias is not None:
-                        bi = bi + conv.bias.detach().float() * sc
-                else:
-                    sc = None
-                    bi = conv.bias.detach().float().contiguous() if conv.bias is not None else None
-                packs[key] = (w, sc.contiguous() if sc is not None else None,
-                              bi.contiguous() if bi is not None else None)
+            if st.kind == 'dw':
+                key = self.wkey[st.i] = (st.i, 'dw')
+                if key not in packs:
+                    sc, bi = fold_bn(st.conv, st.bn)
+                    packs[key] = (st.conv.weight.detach().float().contiguous(),
+                                  sc.contiguous() if sc is not None else None,
+                                  bi.contiguous() if bi is not None else None)
                 continue
-            if st[0] != 'conv':
+            if st.kind != 'conv':
                 continue
-            _, i, src, out, res, conv, bn, act, slope = st
+            i, conv, bn = st.i, st.conv, st.bn
             layout = 'pair' if self._pair_packable(st) else 's2' if self._s2_pair_packable(st) else 'base'
             key = self.wkey[i] = (i, layout)
             if key in packs:
@@ -422,7 +324,7 @@ class Plan:
             elif layout == 's2':
                 _, bias_f, w32f = ops.pack_conv_weights(conv.weight.detach(), conv.bias.detach() if conv.bias is not None
                                                         else None, bnp, eps, want_fp32=True)
-                packs[key] = base + (('s2', ops.s2_pair_weights(w32f).half(), bias_f),)
+                packs[key] = base + ((ops.s2_pair_weights(w32f).half(), bias_f),)
 
     # ---- pixel-pair packing of the Cin = 32 3x3 layers --------------------------------------------------------------
     # With 32 input channels a tap of the im2col gather is a 64-byte row: one TMA request per pixel per tap, and the
@@ -434,7 +336,7 @@ class Plan:
     def _pair_packable(self, st):
         if os.environ.get('B2Y_PAIRPACK', '1') == '0':
             return False
-        _, i, src, out, res, conv, bn, act, slope = st
+        src, out, res, conv = st.src, st.out, st.res, st.conv
         if src is None or conv.kernel_size[0] != 3 or conv.stride[0] != 1 or conv.padding[0] != 1:
             return False
         if conv.in_channels != 32 or conv.out_channels > 128 or conv.out_channels % 8 or src.W % 2:
@@ -447,7 +349,7 @@ class Plan:
         read as pixel pairs makes it a 3 x 2 window with stride 2 x 1 over 128-byte rows (6 im2col boxes, not 9 halves)."""
         if os.environ.get('B2Y_PAIRPACK', '1') == '0':
             return False
-        _, i, src, out, res, conv, bn, act, slope = st
+        src, conv = st.src, st.conv
         if src is None or conv.kernel_size[0] != 3 or conv.stride[0] != 2 or conv.padding[0] != 1:
             return False
         if conv.in_channels != 32 or src.W % 2:
@@ -455,181 +357,62 @@ class Plan:
         return src.c0 == 0 and src.buf.shape[3] == src.C and src.dtype == torch.float16
 
     def _pair_pack(self, conv, bnp, eps):
-        O, I = conv.out_channels, conv.in_channels
         _, bias, w32 = ops.pack_conv_weights(conv.weight.detach(), conv.bias.detach() if conv.bias is not None else None,
                                              bnp, eps, want_fp32=True)
-        w2 = torch.zeros((2 * O, 2 * I, 3, 3), dtype=torch.float32, device=w32.device)
-        for o_sub in range(2):
-            for i_sub in range(2):
-                for kwp in range(3):
-                    s_ = 2 * (kwp - 1) + i_sub - o_sub + 1
-                    if 0 <= s_ <= 2:
-                        w2[o_sub * O:(o_sub + 1) * O, i_sub * I:(i_sub + 1) * I, :, kwp] = w32[:, :, :, s_]
-        wp2, _, _ = ops.pack_conv_weights(w2)
+        wp2, _, _ = ops.pack_conv_weights(ops.s1_pair_weights(w32))
         return wp2, torch.cat([bias, bias]).contiguous()
+
+    def _launch_conv(self, st, x):
+        src, out, res, conv, act, slope = st.src, st.out, st.res, st.conv, st.act, st.slope
+        wp, bias, w32, wstem = self._w(st.i)[:4]
+        layout = self.wkey[st.i][1]
+        k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+        if src is None:
+            if conv.in_channels > 4:
+                raise NotImplementedError("first layer with more than 4 input channels")
+            if wstem is not None and wstem.dim() == 2 and conv.out_channels <= 64:
+                # full-im2col weight layout: the fused kernel builds the A tile in smem (no workspace)
+                ops.stem_conv_fused(x, wstem, bias, k, s, p, act=act, slope=slope, out=out.view(),
+                                    x_div=256.0 if x.dtype == torch.uint8 else 1.0)
+                return
+            if x.dtype != torch.float32:
+                x = x.float() / 256.0 if x.dtype == torch.uint8 else x.float()
+            if wstem is not None:
+                if getattr(self, 'stem_ws', None) is None:
+                    self.stem_ws = self._stem_workspace(conv)
+                ops.stem_conv_tc(x, wstem, bias, conv.in_channels, k, s, p, act=act, slope=slope,
+                                 out=out.view(), workspace=self.stem_ws)
+            else:
+                ops.stem_conv(x, w32, bias, k, s, p, act=act, slope=slope, out=out.view())
+        elif layout == 's2':
+            wps2, bias_s2 = self._w(st.i)[4]
+            ops.conv2d(src.view(), wps2, bias_s2, k, s, p, act=act, slope=slope,
+                       residual=res.view() if res is not None else None, out=out.view(), w_layout=WLAYOUT_S2_PAIRS)
+        elif layout == 'pair':
+            wp2, bias2 = self._w(st.i)[4]
+            pairs = lambda t: t.buf.view(t.buf.shape[0], t.H, t.W // 2, 2 * t.C)
+            ops.conv2d(pairs(src), wp2, bias2, 3, 1, 1, act=act, slope=slope,
+                       residual=pairs(res) if res is not None else None, out=pairs(out))
+        else:
+            ops.conv2d(src.view_k(), wp, bias, k, s, p, act=act, slope=slope,
+                       residual=res.view() if res is not None else None, out=out.view())
 
     def _launch_all(self, x):
         for st in self.steps:
-            kind = st[0]
-            if kind == 'conv':
-                _, i, src, out, res, conv, bn, act, slope = st
-                wp, bias, w32, wstem = self._w(i)[:4]
-                k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-                if src is None:
-                    if conv.in_channels > 4:
-                        raise NotImplementedError("first layer with more than 4 input channels")
-                    if wstem is not None and wstem.dim() == 2 and conv.out_channels <= 64:
-                        # full-im2col weight layout: the fused kernel builds the A tile in smem (no workspace)
-                        ops.stem_conv_fused(x, wstem, bias, k, s, p, act=act, slope=slope, out=out.view(),
-                                            x_div=256.0 if x.dtype == torch.uint8 else 1.0)
-                    elif wstem is not None:
-                        if x.dtype != torch.float32:
-                            x = x.float() / 256.0 if x.dtype == torch.uint8 else x.float()
-                        if getattr(self, 'stem_ws', None) is None:
-                            self.stem_ws = self._stem_workspace(conv)
-                        ops.stem_conv_tc(x, wstem, bias, conv.in_channels, k, s, p, act=act, slope=slope,
-                                         out=out.view(), workspace=self.stem_ws)
-                    else:
-                        if x.dtype != torch.float32:
-                            x = x.float() / 256.0 if x.dtype == torch.uint8 else x.float()
-                        ops.stem_conv(x, w32, bias, k, s, p, act=act, slope=slope, out=out.view())
-                elif len(self._w(i)) == 5 and isinstance(self._w(i)[4][0], str):
-                    _, wps2, bias_s2 = self._w(i)[4]
-                    ops.conv2d(src.view(), wps2, bias_s2, k, s, p, act=act, slope=slope,
-                               residual=res.view() if res is not None else None, out=out.view(),
-                               w_layout=WLAYOUT_S2_PAIRS)
-                elif len(self._w(i)) == 5:
-                    wp2, bias2 = self._w(i)[4]
-                    pairs = lambda t: t.buf.view(t.buf.shape[0], t.H, t.W // 2, 2 * t.C)
-                    ops.conv2d(pairs(src), wp2, bias2, 3, 1, 1, act=act, slope=slope,
-                               residual=pairs(res) if res is not None else None, out=pairs(out))
-                else:
-                    ops.conv2d(src.view_k(), wp, bias, k, s, p, act=act, slope=slope,
-                               residual=res.view() if res is not None else None, out=out.view())
-            elif kind == 'dw':
-                _, i, src, out, conv, bn, act, slope = st
-                w, sc, bi = self._w(i)
-                ops.dwconv2d(src.view(), w, conv.kernel_size[0], conv.stride[0], conv.padding[0], scale=sc, bias=bi,
-                             act=act, slope=slope, out=out.view())
-            elif kind == 'se':
-                _, i, src, out, fc1, fc2, ws = st
-                ops.se_fwd(src.view(), fc1.weight.detach(), fc2.weight.detach(), out=out.view(), ws=ws)
-            elif kind == 'add':
-                xv, av, ov = st[1].view(), st[2].view(), st[3].view()
-                n = min(xv.shape[3], av.shape[3])
-                ops.add(xv[..., :n], av[..., :n], out=ov[..., :n])
-                if xv.shape[3] > n and st[1] is not st[3]:
-                    ops.copy_channels(xv[..., n:], ov[..., n:])
-            elif kind == 'copy':
-                _, srct, dst, off = st
-                ops.copy_channels(srct.view(), dst.buf[..., off:off + srct.C])
-            elif kind == 'upsample':
-                ops.upsample(st[1].view(), st[3], out=st[2].view())
-            elif kind == 'maxpool':
-                ops.maxpool(st[1].view(), st[3], st[4], tiny_pad=st[5], out=st[2].view())
+            if st.kind == 'conv':
+                self._launch_conv(st, x)
+            elif st.kind == 'dw':
+                conv = st.conv
+                w, sc, bi = self._w(st.i)
+                ops.dwconv2d(st.src.view(), w, conv.kernel_size[0], conv.stride[0], conv.padding[0], scale=sc, bias=bi,
+                             act=st.act, slope=st.slope, out=st.out.view())
+            elif st.kind == 'se':
+                ops.se_fwd(st.src.view(), st.fc1.weight.detach(), st.fc2.weight.detach(), out=st.out.view(), ws=st.ws)
+            else:
+                launch_pointwise(st)
         for (m, raw, row_off, rows), anc in zip(self.yolo, self.anchors_px):
-            ops_io = self.io
-            _, p = ops.yolo_decode(raw.buf, m.na, m.no, anc, m.stride, io=ops_io, row_offset=row_off)
+            _, p = ops.yolo_decode(raw.buf, m.na, m.no, anc, m.stride, io=self.io, row_offset=row_off)
             self.p_out.append(p)
-
-    # ---- measurement helpers (bench.py) -----------------------------------------------------------------------
-    def _launch_step(self, st, x):
-        saved = self.steps
-        self.steps = [st]
-        yolo = self.yolo
-        self.yolo = []
-        try:
-            self._launch_all(x)
-        finally:
-            self.steps, self.yolo = saved, yolo
-
-    def launches_per_forward(self):
-        return len(self.steps) + len(self.yolo) + (1 if getattr(self, 'stem_ws', None) is not None else 0)
-
-    def step_info(self, st):
-        """(label, algorithmic FLOPs, algorithmic HBM bytes) of one launch."""
-        kind = st[0]
-        B = self.B
-        if kind == 'conv':
-            _, i, src, out, res, conv, bn, act, slope = st
-            k = conv.kernel_size[0]
-            M = B * out.H * out.W
-            flops = 2.0 * M * conv.out_channels * conv.in_channels * k * k
-            in_hw = (self.H * self.W) if src is None else (src.H * src.W)
-            in_bytes = B * in_hw * conv.in_channels * (4 if src is None else 2)
-            out_bytes = M * conv.out_channels * (4 if out.dtype == torch.float32 else 2)
-            w_bytes = conv.out_channels * conv.in_channels * k * k * 2
-            res_bytes = M * conv.out_channels * 2 if res is not None else 0
-            label = "L%03d conv %dx%d s%d %d->%d @%dx%d %s%s" % (i, k, k, conv.stride[0], conv.in_channels,
-                                                                 conv.out_channels, out.H, out.W, act,
-                                                                 "+res" if res is not None else "")
-            return label, flops, in_bytes + out_bytes + w_bytes + res_bytes, src is None
-        t_in, t_out = st[1], (st[3] if kind == 'add' else st[2])
-        if kind == 'copy':
-            n = B * st[1].H * st[1].W * st[1].C * 2
-            return "copy C=%d @%dx%d" % (st[1].C, st[1].H, st[1].W), 0.0, 2 * n, False
-        n_in = B * t_in.H * t_in.W * t_in.C * 2
-        n_out = B * t_out.H * t_out.W * t_out.C * 2
-        if kind == 'add':
-            n_in *= 2
-        return "%s C=%d @%dx%d" % (kind, t_out.C, t_out.H, t_out.W), 0.0, n_in + n_out, False
-
-    def profile_layers(self, x, reps=10):
-        """Per-launch CUDA-event timing.  Each step is captured `reps` times back to back in its own CUDA graph and the
-        replay is timed (best of 3), so the CPU launch cost of eager calls (tensor-map encodes, ctypes) is excluded;
-        consecutive launches of one layer re-use its tensors, so layers whose working set fits the 50 MB L2 are
-        measured L2-warm (like in the real graph, where the producer layer just wrote them)."""
-        x = x.contiguous()
-        if self.param_version is None:
-            self.forward(x)
-        rows = []
-        self.io = torch.empty((self.B, self.total_rows, self.yolo[0][0].no), dtype=torch.float32, device=self.device)
-        for st in self.steps:
-            label, flops, nbytes, is_stem = self.step_info(st)
-            self._launch_step(st, x)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                for _ in range(reps):
-                    self._launch_step(st, x)
-            g.replay()
-            best = None
-            for _ in range(3):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                g.replay()
-                e1.record()
-                e1.synchronize()
-                ms = e0.elapsed_time(e1) / reps
-                best = ms if best is None else min(best, ms)
-            ms = best
-            rows.append({"label": label, "ms": ms, "tflops": flops / ms / 1e9 if ms > 0 else 0.0,
-                         "gbs": nbytes / ms / 1e6 if ms > 0 else 0.0, "flops": flops, "bytes": nbytes,
-                         "kind": "stem" if is_stem else st[0]})
-            del g
-        return rows
-
-    def time_tc_convs(self, x, iters=5):
-        """Time only the wgmma conv launches of one forward, back to back on the current stream.
-        Returns (ms per forward-worth of conv launches, algorithmic FLOPs of those launches, n launches)."""
-        x = x.contiguous().float()
-        if self.param_version is None:
-            self.forward(x)
-        convs = [st for st in self.steps if st[0] == 'conv' and st[2] is not None]
-        flops = sum(self.step_info(st)[1] for st in convs)
-        saved, yolo = self.steps, self.yolo
-        self.steps, self.yolo = convs, []
-        try:
-            self._launch_all(x)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(iters):
-                self._launch_all(x)
-            e1.record()
-            e1.synchronize()
-        finally:
-            self.steps, self.yolo = saved, yolo
-        return e0.elapsed_time(e1) / iters, flops, len(convs)
 
     def forward(self, x):
         model = self.model
@@ -794,7 +577,7 @@ class Engine:
             if model.training:
                 plan = TrainPlan(model, tuple(x.shape), x.device, keep, store, self.train_shared)
             else:
-                plan = Plan(model, tuple(x.shape), x.device, False, keep, store, self.eval_weights)
+                plan = Plan(model, tuple(x.shape), x.device, keep, store, self.eval_weights)
             self.plans[key] = plan
             if store.generation != gen:
                 self._drop_stale()

@@ -76,6 +76,21 @@ def s2_pair_weights(w_oihw):
     return out.contiguous()
 
 
+def s1_pair_weights(w_oihw):
+    """[O][I][3][3] -> [2O][2I][3][3]: the 3x3 / stride-1 / pad-1 filter over tensors viewed as pixel pairs
+    [B,H,W/2,2C].  Output sub-pixel o_sub and input sub-pixel i_sub of pair column kwp meet the original tap
+    s = 2(kwp-1) + i_sub - o_sub + 1; the other entries are zero."""
+    O, I = w_oihw.shape[:2]
+    out = torch.zeros((2 * O, 2 * I, 3, 3), dtype=torch.float32, device=w_oihw.device)
+    for o_sub in range(2):
+        for i_sub in range(2):
+            for kwp in range(3):
+                s = 2 * (kwp - 1) + i_sub - o_sub + 1
+                if 0 <= s <= 2:
+                    out[o_sub * O:(o_sub + 1) * O, i_sub * I:(i_sub + 1) * I, :, kwp] = w_oihw[:, :, :, s]
+    return out
+
+
 def conv2d(x, w_packed, bias, k, stride, pad, act="linear", slope=0.1, residual=None, out=None,
            out_dtype=torch.float16, stats=None, w_layout=0):
     """y = act(conv(x, w) + bias) [+ residual]; x NHWC fp16 view, w_packed [O][k][k][I] fp16."""

@@ -207,6 +207,7 @@ class QatRunner:
 
     def forward(self, x):
         from .engine import LazyFeatures
+        from .layout import feature_slots
         model = self.model
         defs, mods = model.module_defs, model.module_list
         dev = x.device
@@ -263,9 +264,7 @@ class QatRunner:
             else:
                 raise NotImplementedError("layer type '%s' in the QAT graph" % t)
             outs.append(h if model.routs[i] else None)
-        nfeat = sum(1 for j, mm in enumerate(mods) if mm.__class__.__name__ == 'Sequential' and j + 1 < len(defs)
-                    and defs[j + 1]['type'] != 'yolo')
-        feats = LazyFeatures([None] * nfeat)
+        feats = LazyFeatures([None] * len(feature_slots(model)))
         if model.training:
             return yolo_out, feats
         return torch.cat(io_list, 1), tuple(yolo_out), feats

@@ -23,6 +23,7 @@ import torch
 
 from . import ops
 from .engine import LazyFeatures
+from .layout import feature_slots, sources
 
 
 def _vote(values, scale_list, offset):
@@ -170,10 +171,9 @@ class QCalibPlan:
                     raise RuntimeError("quantized=3 needs shortcut_way 1 or 2 (models.py:275-305)")
                 if len(d['from']) != 1:
                     raise NotImplementedError("multi-source quantised shortcut")
-                l = d['from'][0]
-                outs[i] = self._shortcut(m, outs[i - 1], outs[i + l if l < 0 else l])
+                outs[i] = self._shortcut(m, outs[i - 1], outs[sources(i, d['from'])[0]])
             elif t == 'route':
-                srcs = [i + l if l < 0 else l for l in d['layers']]
+                srcs = sources(i, d['layers'])
                 if len(srcs) == 1:
                     if 'groups' in d:
                         raise NotImplementedError("grouped route in the PTQ graph")
@@ -189,6 +189,4 @@ class QCalibPlan:
                 yolo_out.append(p)
             else:
                 raise NotImplementedError("layer type '%s' in the PTQ graph" % t)
-        nfeat = sum(1 for j, mm in enumerate(mods) if mm.__class__.__name__ == 'Sequential' and j + 1 < len(defs)
-                    and defs[j + 1]['type'] != 'yolo')
-        return yolo_out, LazyFeatures([None] * nfeat)
+        return yolo_out, LazyFeatures([None] * len(feature_slots(model)))

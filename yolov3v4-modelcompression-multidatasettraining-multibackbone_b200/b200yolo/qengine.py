@@ -18,11 +18,8 @@ import os
 import torch
 
 from . import ops
-from .engine import _Tensor
+from .layout import _Tensor, infer_shapes, sources
 from .lib import OUT_F32, OUT_I8, WLAYOUT_S2_PAIRS, B2YError, call, ptr, stream_ptr
-
-_ACT_NAME = {'leaky': 'leaky', 'relu6': 'relu6', 'h_swish': 'h_swish', 'relu': 'relu', 'mish': 'mish',
-             'linear': 'linear'}
 
 
 def _pairs(t):
@@ -50,7 +47,10 @@ class QPlan:
         model, B, dev = self.model, self.B, self.device
         defs, mods = model.module_defs, model.module_list
         n = len(defs)
-        shapes, prev = [], (self.Cin, self.H, self.W)
+        shapes = infer_shapes(model, (self.Cin, self.H, self.W),
+                              ('convolutional', 'shortcut', 'route', 'upsample', 'yolo'),
+                              "layer type '%s' in the int8 graph (the reference cannot PTQ-calibrate maxpool cfgs either, "
+                              "models.py:537-539)")
         tens = [None] * n
         self.yolo = []
         row_off = 0
@@ -58,17 +58,14 @@ class QPlan:
         readers = set()
         for j, dj in enumerate(defs):
             if dj['type'] == 'route':
-                readers.update(j + l if l < 0 else l for l in dj['layers'])
+                readers.update(sources(j, dj['layers']))
             elif dj['type'] == 'shortcut':
-                readers.update(j + l if l < 0 else l for l in dj['from'])
+                readers.update(sources(j, dj['from']))
         for i, (d, m) in enumerate(zip(defs, mods)):
             t = d['type']
-            Cc, H, W = prev
+            Cc, H, W = shapes[i]
             if t == 'convolutional':
                 conv = m[0]
-                k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-                H, W = ops.conv_out_hw(H, W, k, s, p)
-                Cc = conv.out_channels
                 head = i + 1 < n and defs[i + 1]['type'] == 'yolo'
                 out = _Tensor(Cc, H, W, torch.float32 if head else torch.int8)
                 pitch = 256 if head else Cc
@@ -83,8 +80,7 @@ class QPlan:
                                        "residual adds otherwise, models.py:275-305)")
                 if len(d['from']) != 1 or getattr(m, 'weight', False):
                     raise NotImplementedError("weighted / multi-source quantised shortcut")
-                l = d['from'][0]
-                src = tens[i + l if l < 0 else l]
+                src = tens[sources(i, d['from'])[0]]
                 out = _Tensor(Cc, H, W, torch.int8)
                 out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
                 prev_step = self.steps[-1] if self.steps else None
@@ -99,42 +95,32 @@ class QPlan:
                     self.steps.append(('shortcut', i, tens[i - 1], src, out, m))
                 tens[i] = out
             elif t == 'route':
-                srcs = [i + l if l < 0 else l for l in d['layers']]
+                srcs = sources(i, d['layers'])
+                if 'groups' in d:
+                    raise NotImplementedError("grouped route in the int8 graph")
                 if len(srcs) == 1:
-                    if 'groups' in d:
-                        raise NotImplementedError("grouped route in the int8 graph")
                     tens[i] = tens[srcs[0]]
-                    Cc, H, W = tens[i].C, tens[i].H, tens[i].W
                 else:
-                    Cc = sum(tens[s].C for s in srcs)
-                    H, W = tens[srcs[0]].H, tens[srcs[0]].W
                     out = _Tensor(Cc, H, W, torch.int8)
                     out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
                     self.steps.append(('concat', i, [tens[s] for s in srcs], out, m))
                     tens[i] = out
             elif t == 'upsample':
-                s = d['stride']
-                H, W = H * s, W * s
                 out = _Tensor(Cc, H, W, torch.int8)
                 out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
-                self.steps.append(('upsample', i, tens[i - 1], out, s))
+                self.steps.append(('upsample', i, tens[i - 1], out, d['stride']))
                 tens[i] = out
             elif t == 'yolo':
                 raw = tens[i - 1]
                 rows = m.na * raw.H * raw.W
                 self.yolo.append((m, raw, row_off, rows))
                 row_off += rows
-            else:
-                raise NotImplementedError("layer type '%s' in the int8 graph (the reference cannot PTQ-calibrate "
-                                          "maxpool cfgs either, models.py:537-539)" % t)
-            prev = (Cc, H, W)
-            shapes.append(prev)
         self.total_rows = row_off
         self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _, _, _) in self.yolo]
 
     def _pack_qconv(self, src, conv, s_w):
         """int8 weight codes [O][kh][kw][I] + bias, in the pixel-pair forms for the two narrow (Cin = 32) 3x3 layers:
-        's1' = engine.py _pair_pack (the tensors viewed as [B,H,W/2,2C], doubled output channels), 's2' =
+        's1' = ops.s1_pair_weights (the tensors viewed as [B,H,W/2,2C], doubled output channels), 's2' =
         B2Y_WLAYOUT_S2_PAIRS.  q_weight holds code * s_w exactly, so the codes are recovered without rounding."""
         k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         bias = conv.q_bias.detach().float().contiguous()
@@ -143,13 +129,7 @@ class QPlan:
         lo, hi = -(1 << (conv.w_bits - 1)), (1 << (conv.w_bits - 1)) - 1
         pair_ok = os.environ.get('B2Y_PAIRPACK', '1') != '0' and k == 3 and p == 1 and I == 32 and src.W % 2 == 0
         if pair_ok and s == 1 and O <= 128 and O % 8 == 0:
-            w2 = torch.zeros((2 * O, 2 * I, 3, 3), dtype=torch.float32, device=qw.device)
-            for o_sub in range(2):
-                for i_sub in range(2):
-                    for kwp in range(3):
-                        s_ = 2 * (kwp - 1) + i_sub - o_sub + 1
-                        if 0 <= s_ <= 2:
-                            w2[o_sub * O:(o_sub + 1) * O, i_sub * I:(i_sub + 1) * I, :, kwp] = qw[:, :, :, s_]
+            w2 = ops.s1_pair_weights(qw)
             return ops.pack_qconv_weights(w2, s_w, conv.w_bits), torch.cat([bias, bias]).contiguous(), 's1'
         if pair_ok and s == 2:
             codes = (ops.s2_pair_weights(qw) / s_w).round().clamp(lo, hi).to(torch.int8).contiguous()
@@ -171,7 +151,7 @@ class QPlan:
                 bits_w, bits_a = conv.w_bits, conv.a_bits
                 if bits_w > 8 or bits_a > 8:
                     raise NotImplementedError("the int8 wgmma path covers <= 8 bit weights and activations")
-                act = _ACT_NAME[conv.activate]
+                act = conv.activate
                 slope = 0.25 if conv.maxabsscaler else 0.1
                 if src is None:
                     self.packed[i] = (conv.q_weight.detach().float().contiguous(), conv.q_bias.detach().float(), s_a,
@@ -189,7 +169,7 @@ class QPlan:
                 if conv.w_bits > 8 or conv.a_bits > 8:
                     raise NotImplementedError("the int8 wgmma path covers <= 8 bit weights and activations")
                 w8, bq, mode = self._pack_qconv(src, conv, s_w)
-                self.packed[i] = (w8, bq, scale_of[id(src)] * s_w, s_a, _ACT_NAME[conv.activate],
+                self.packed[i] = (w8, bq, scale_of[id(src)] * s_w, s_a, conv.activate,
                                   0.25 if conv.maxabsscaler else 0.1, conv.a_bits, mode)
                 scale_of[id(own)] = s_a
                 scale_of[id(out)] = _s(m.scale_sum)
@@ -207,7 +187,6 @@ class QPlan:
     def forward(self, x):
         """Eval forward of the INT8 graph; after one eager call the static launch sequence replays from a CUDA graph
         (the quantiser state is frozen in eval; call plan.invalidate() after re-calibrating)."""
-        import os
         if not self.prepared:
             self.prepare()
         x = x.contiguous().float()
@@ -341,6 +320,3 @@ class QPlan:
             m.nx, m.ny = raw.W, raw.H
             p_out.append(p)
         return io, tuple(p_out), []
-
-    def launches_per_forward(self):
-        return sum(len(st[2]) if st[0] == 'concat' else 1 for st in self.steps) + len(self.yolo)

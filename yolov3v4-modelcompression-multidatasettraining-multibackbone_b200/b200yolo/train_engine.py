@@ -24,7 +24,8 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import LazyFeatures, SlotStore, _Tensor, _block_parts
+from .engine import LazyFeatures, SlotStore, launch_pointwise, pointwise_steps
+from .layout import _Tensor, _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources
 from .lib import ACT, ConvDesc, OUT_F16, call, ptr, stream_ptr
 
 GDT = torch.bfloat16   # gradient tensors: bf16 (range of fp32) -- fp16 over/underflows across ~100 BN layers
@@ -49,6 +50,14 @@ class _ConvRec:
     def __init__(self):
         for k in self.__slots__:
             setattr(self, k, None)
+
+
+class _SeRec:
+    __slots__ = ('i', 'src', 'y', 'fc1', 'fc2', 'ws', 'ws_bwd')
+
+    def __init__(self, *fields):
+        for k, v in zip(self.__slots__, fields):
+            setattr(self, k, v)
 
 
 class TrainShared:
@@ -100,79 +109,19 @@ class TrainPlan:
     # ---------------------------------------------------------------------------------------------------------
     def _build(self):
         model, B, dev = self.model, self.B, self.device
-        defs, mods, routs = model.module_defs, model.module_list, model.routs
+        defs, mods = model.module_defs, model.module_list
         n = len(defs)
-        shapes, prev = [], (self.Cin, self.H, self.W)
-        for i, (d, m) in enumerate(zip(defs, mods)):
-            t = d['type']
-            Cc, H, W = prev
-            if t in ('convolutional', 'depthwise'):
-                conv = _block_parts(m)[0]
-                H, W = ops.conv_out_hw(H, W, conv.kernel_size[0], conv.stride[0], conv.padding[0])
-                Cc = conv.out_channels
-            elif t == 'se':
-                pass
-            elif t == 'maxpool':
-                k, s = d['size'], d['stride']
-                if k == 2 and s == 1:
-                    H, W = (H + 1 - k) // s + 1, (W + 1 - k) // s + 1
-                else:
-                    pd = (k - 1) // 2
-                    H, W = (H + 2 * pd - k) // s + 1, (W + 2 * pd - k) // s + 1
-            elif t == 'upsample':
-                H, W = H * d['stride'], W * d['stride']
-            elif t == 'route':
-                srcs = [i + l if l < 0 else l for l in d['layers']]
-                Cc = sum(shapes[s][0] for s in srcs)
-                if 'groups' in d:
-                    Cc //= 2
-                H, W = shapes[srcs[0]][1], shapes[srcs[0]][2]
-            elif t in ('shortcut', 'yolo'):
-                pass
-            else:
-                raise NotImplementedError("layer type '%s' is not supported by the sm_90a training engine yet" % t)
-            prev = (Cc, H, W)
-            shapes.append(prev)
-
-        is_head = [False] * n
-        fused_into = [None] * n   # shortcut i folded into the bn+act apply of conv i-1
-        for i, d in enumerate(defs):
-            if d['type'] == 'yolo' and i > 0 and defs[i - 1]['type'] == 'convolutional':
-                is_head[i - 1] = True
-            if d['type'] == 'shortcut' and i > 1:
-                frm = [i + l if l < 0 else l for l in d['from']]
-                if (not self.keep_features
-                        and len(frm) == 1 and defs[i - 1]['type'] == 'convolutional' and not routs[i - 1]
-                        and not getattr(mods[i], 'weight', False) and shapes[frm[0]] == shapes[i - 1]
-                        and _block_parts(mods[i - 1])[1] is not None):
-                    fused_into[i] = i - 1
-
-        tens = [None] * n
-        for i, d in enumerate(defs):
-            t = d['type']
-            if t == 'yolo' or (t == 'route' and len(d['layers']) == 1 and 'groups' not in d):
-                continue
-            Cc, H, W = shapes[i]
-            tens[i] = _Tensor(Cc, H, W, torch.float32 if is_head[i] else torch.float16)
-        self.pre_add = {}
-        for i in range(n):
-            if fused_into[i] is not None:
-                tens[fused_into[i]] = tens[i]
-        for i, d in enumerate(defs):
-            if d['type'] == 'route' and len(d['layers']) == 1 and 'groups' not in d:
-                l = d['layers'][0]
-                src = i + l if l < 0 else l
-                tens[i] = tens[src]
-
-        # concat placement (same policy as the inference plan); gradients mirror the placement
-        placed, copies = set(), {}
-        self.bufs = []   # (activation buffer, gradient buffer) pairs to keep alive
+        shapes = infer_shapes(model, (self.Cin, self.H, self.W),
+                              message="layer type '%s' is not supported by the sm_90a training engine yet")
+        # a shortcut is folded into the bn+act apply of the conv before it
+        lay = build_layout(model, shapes, self.keep_features, lambda i: _block_parts(mods[i])[1] is not None)
+        tens, is_head, fused_into = lay.tens, lay.is_head, lay.fused_into
 
         def new_buf(name, Cc, H, W, dtype=torch.float16):
             # fp16: MobileNet widths (24, 40, 72 ...) get a pitch rounded up to the MMA K granule, pad channels stay
             # zero forever (slots are zero-filled and the pitch depends on the width only)
-            pitch = _round_up(Cc, 4 if dtype != torch.float16 else 16)
-            return self._take((name, pitch, dtype), (B, H, W, pitch), dtype)
+            pc = pitch(Cc, dtype)
+            return self._take((name, pc, dtype), (B, H, W, pc), dtype)
 
         def zeros_later(shape, dtype):
             """placeholder (meta tensor) for a buffer that is carved out of the zero-at-start-of-backward arena"""
@@ -186,29 +135,19 @@ class TrainPlan:
             self.grad_of[id(t)] = g
             return g
 
-        for i, d in enumerate(defs):
-            if d['type'] != 'route' or len(d['layers']) == 1:
-                continue
-            srcs = [i + l if l < 0 else l for l in d['layers']]
+        # multi-source routes are buffers their producers write into; the gradients mirror the placement
+        for i, parts in lay.concats.items():
             dst = tens[i]
             dst.buf = new_buf(('cat', i), dst.C, dst.H, dst.W)
             gdst = make_grad(dst, zeros_later(dst.buf.shape, GDT))
-            off = 0
-            for s in srcs:
-                st = tens[s]
-                if id(st) not in placed and st.buf is None and off % 8 == 0 and st.dtype == torch.float16 \
-                        and st is not dst:
-                    st.buf, st.c0 = dst.buf, off
+            for st, off, placed in parts:
+                if placed:
+                    st.buf = dst.buf
                     make_grad(st, gdst.buf, off)
-                    placed.add(id(st))
-                else:
-                    copies.setdefault(i, []).append((st, off))
-                off += st.C
 
         def alloc(t, i):
             if t.buf is None:
                 t.buf = new_buf(('act', i), t.C if t.dtype == torch.float16 else HEAD_PAD, t.H, t.W, t.dtype)
-                t.c0 = 0
             if id(t) not in self.grad_of:
                 if t.dtype == torch.float16:
                     make_grad(t, zeros_later(t.buf.shape, GDT))
@@ -219,7 +158,6 @@ class TrainPlan:
             return t
 
         self.yolo = []
-        self.feature_views = []
         feat_idx = {}
         for i, (d, m) in enumerate(zip(defs, mods)):
             t = d['type']
@@ -228,10 +166,9 @@ class TrainPlan:
                 src = tens[i - 1]
                 out = alloc(tens[i], i)
                 cr = fc[0].out_features
-                rec = {'i': i, 'src': src, 'y': out, 'fc1': fc[0], 'fc2': fc[2],
-                       'ws': self._take(('se_ws', i), (B, 3 * src.C + cr), torch.float32),
-                       'ws_bwd': self._take(('se_ws_bwd', i), (B, 3 * src.C + cr), torch.float32)}
-                self.order.append(('se', rec))
+                self.order.append(('se', _SeRec(i, src, out, fc[0], fc[2],
+                                                self._take(('se_ws', i), (B, 3 * src.C + cr), torch.float32),
+                                                self._take(('se_ws_bwd', i), (B, 3 * src.C + cr), torch.float32))))
                 feat_idx[i] = out
             elif t in ('convolutional', 'depthwise'):
                 conv, bn, act, slope = _block_parts(m)
@@ -256,8 +193,7 @@ class TrainPlan:
                 r.src = None if i == 0 else tens[i - 1]
                 r.y = alloc(tens[i], i)
                 if i + 1 < n and fused_into[i + 1] == i:
-                    l = defs[i + 1]['from'][0]
-                    r.res = tens[i + 1 + l if l < 0 else l]
+                    r.res = tens[sources(i + 1, defs[i + 1]['from'])[0]]
                 if bn is not None:
                     # csrc/bn_train.cu: a thread owns 8 channels, a CTA of 256 threads at least one pixel row
                     if r.Cout % 8 != 0 or r.Cout > 2048:
@@ -278,36 +214,16 @@ class TrainPlan:
                     feat_idx[i] = r.y   # (a conv with a fused shortcut never materialises its pre-add output)
                 if r.depthwise:
                     r.dwg = zeros_later(tuple(conv.weight.shape), torch.float32)
-            elif t == 'shortcut':
-                if fused_into[i] is not None:
-                    continue
-                frm = [i + l if l < 0 else l for l in d['from']]
-                if getattr(m, 'weight', False):
-                    raise NotImplementedError("weighted shortcut is not supported yet")
-                out = alloc(tens[i], i)
-                self.order.append(('add', tens[i - 1], [tens[s] for s in frm], out))
-            elif t == 'route':
-                if len(d['layers']) == 1:
-                    if 'groups' in d:
-                        src, g = tens[i - 1], tens[i]
-                        g.buf, g.c0 = src.buf, src.c0 + src.C // 2
-                        gs = self.grad_of[id(src)]
-                        make_grad(g, gs.buf, gs.c0 + src.C // 2)
-                    continue
-                for st, off in copies.get(i, []):
-                    self.order.append(('copy', st, tens[i], off))
-            elif t == 'upsample':
-                self.order.append(('upsample', tens[i - 1], alloc(tens[i], i), d['stride']))
-            elif t == 'maxpool':
-                k, s = d['size'], d['stride']
-                self.order.append(('maxpool', tens[i - 1], alloc(tens[i], i), k, s, k == 2 and s == 1))
-                if m.__class__.__name__ == 'Sequential':
-                    feat_idx[i] = tens[i]
             elif t == 'yolo':
                 self.yolo.append((m, tens[i - 1]))
-        for i, m in enumerate(mods):
-            if m.__class__.__name__ == 'Sequential' and i + 1 < n and defs[i + 1]['type'] != 'yolo':
-                self.feature_views.append(feat_idx.get(i))
+            else:
+                self.order += pointwise_steps(lay, i, d, m, alloc)
+                if i in lay.grouped:
+                    gs = self.grad_of[id(lay.grouped[i])]
+                    make_grad(tens[i], gs.buf, gs.c0 + lay.grouped[i].C // 2)
+                if t == 'maxpool' and m.__class__.__name__ == 'Sequential':
+                    feat_idx[i] = tens[i]
+        self.feature_views = [feat_idx.get(i) for i in feature_slots(model)]
         self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _) in self.yolo]
         self.bn_counters = [r.bn.num_batches_tracked for r in self.convs if r.bn is not None]
         self._plan_grad_writes()
@@ -507,23 +423,20 @@ class TrainPlan:
                     write(G(r.src), r.conv.in_channels, ('dgrad', r.i), r.k >= r.s)
             elif kind == 'se':
                 e = st[1]
-                read(G(e['y']), G(e['y']).C)
-                write(G(e['src']), G(e['src']).C, ('se', idx), False)
+                read(G(e.y), G(e.y).C)
+                write(G(e.src), G(e.src).C, ('se', idx), False)
             elif kind == 'add':
-                _, first, others, out = st
-                go = G(out)
+                go = G(st.out)
                 read(go, go.C)
-                for j, t in enumerate([first] + list(others)):
+                for j, t in enumerate([st.first] + st.others):
                     write(G(t), min(G(t).C, go.C), ('add', idx, j), True)
             elif kind == 'copy':
-                _, srct, dst, off = st
-                gd = G(dst)
-                read(gd, srct.C, gd.c0 + off)
-                write(G(srct), srct.C, ('copy', idx), True)
+                gd = G(st.dst)
+                read(gd, st.src.C, gd.c0 + st.off)
+                write(G(st.src), st.src.C, ('copy', idx), True)
             elif kind in ('upsample', 'maxpool'):
-                src, out = st[1], st[2]
-                read(G(out), G(out).C)
-                write(G(src), G(src).C, (kind, idx), False)
+                read(G(st.out), G(st.out).C)
+                write(G(st.src), G(st.src).C, (kind, idx), False)
         self.dirty_grad_bufs = dirty
 
     def _grad_dst(self, param):
@@ -628,24 +541,9 @@ class TrainPlan:
                 self._conv_forward(r, x)
             elif kind == 'se':
                 e = st[1]
-                ops.se_fwd(e['src'].view(), e['fc1'].weight.detach(), e['fc2'].weight.detach(), out=e['y'].view(),
-                           ws=e['ws'])
-            elif kind == 'add':
-                cur = st[1]
-                for s in st[2]:                     # channel-sliced when the widths differ (layers.py:57-72)
-                    xv, av, ov = cur.view(), s.view(), st[3].view()
-                    n = min(xv.shape[3], av.shape[3])
-                    ops.add(xv[..., :n], av[..., :n], out=ov[..., :n])
-                    if xv.shape[3] > n and cur is not st[3]:
-                        ops.copy_channels(xv[..., n:], ov[..., n:])
-                    cur = st[3]
-            elif kind == 'copy':
-                _, srct, dst, off = st
-                ops.copy_channels(srct.view(), dst.buf[..., off:off + srct.C])
-            elif kind == 'upsample':
-                ops.upsample(st[1].view(), st[3], out=st[2].view())
-            elif kind == 'maxpool':
-                ops.maxpool(st[1].view(), st[3], st[4], tiny_pad=st[5], out=st[2].view())
+                ops.se_fwd(e.src.view(), e.fc1.weight.detach(), e.fc2.weight.detach(), out=e.y.view(), ws=e.ws)
+            else:
+                launch_pointwise(st)
         if self.bn_counters:
             torch._foreach_add_(self.bn_counters, 1)
 
@@ -732,13 +630,12 @@ class TrainPlan:
                 self._conv_backward(st[1], grads, S, inv)
             elif kind == 'se':
                 e = st[1]
-                ops.se_bwd(e['src'].view(), G(e['y']).view(), e['fc1'].weight.detach(), e['fc2'].weight.detach(),
-                           e['ws'], G(e['src']).view(), accumulate=True, dw1=self._grad_dst(e['fc1'].weight),
-                           dw2=self._grad_dst(e['fc2'].weight), grad_scale=inv, ws_bwd=e['ws_bwd'])
+                ops.se_bwd(e.src.view(), G(e.y).view(), e.fc1.weight.detach(), e.fc2.weight.detach(), e.ws,
+                           G(e.src).view(), accumulate=True, dw1=self._grad_dst(e.fc1.weight),
+                           dw2=self._grad_dst(e.fc2.weight), grad_scale=inv, ws_bwd=e.ws_bwd)
             elif kind == 'add':
-                _, first, others, out = st
-                go = G(out).view()
-                for j, s in enumerate([first] + list(others)):
+                go = G(st.out).view()
+                for j, s in enumerate([st.first] + st.others):
                     gs = G(s).view()
                     n = min(gs.shape[3], go.shape[3])      # sliced addends receive the matching gradient channels
                     if self.first_write.get(('add', idx, j)):
@@ -746,23 +643,24 @@ class TrainPlan:
                     else:
                         ops.add(gs[..., :n], go[..., :n], out=gs[..., :n])
             elif kind == 'copy':
-                _, srct, dst, off = st
-                gd = G(dst)
-                gs = G(srct).view()
+                gd = G(st.dst)
+                gs = G(st.src).view()
+                gslice = gd.buf[..., gd.c0 + st.off:gd.c0 + st.off + st.src.C]
                 if self.first_write.get(('copy', idx)):
-                    ops.copy_channels(gd.buf[..., gd.c0 + off:gd.c0 + off + srct.C], gs)
+                    ops.copy_channels(gslice, gs)
                 else:
-                    ops.add(gs, gd.buf[..., gd.c0 + off:gd.c0 + off + srct.C], out=gs)
+                    ops.add(gs, gslice, out=gs)
             elif kind == 'upsample':
-                _, src, out, s = st
-                gy, gx = G(out).view(), G(src).view()
+                src = st.src
+                gy, gx = G(st.out).view(), G(src).view()
                 call("b2y_upsample_nearest_bwd", ptr(gy), ops._pitch(gy), ptr(gx), ops._pitch(gx), self.B, src.H,
-                     src.W, src.C, int(s), ops._gdt(gy), stream_ptr())
+                     src.W, src.C, int(st.stride), ops._gdt(gy), stream_ptr())
             elif kind == 'maxpool':
-                _, src, out, k, s, tiny = st
-                gy, gx, xv = G(out).view(), G(src).view(), src.view()
+                src = st.src
+                gy, gx, xv = G(st.out).view(), G(src).view(), src.view()
                 call("b2y_maxpool_bwd", ptr(xv), ops._pitch(xv), ptr(gy), ops._pitch(gy), ptr(gx), ops._pitch(gx),
-                     self.B, src.H, src.W, src.C, int(k), int(s), 1 if tiny else 0, ops._gdt(gy), stream_ptr())
+                     self.B, src.H, src.W, src.C, int(st.k), int(st.s), 1 if st.tiny_pad else 0, ops._gdt(gy),
+                     stream_ptr())
         torch.cuda.current_stream().wait_stream(self.side_stream)          # join: every weight gradient is complete
         self._unpack_all()
         if self.shared.own_grads:
