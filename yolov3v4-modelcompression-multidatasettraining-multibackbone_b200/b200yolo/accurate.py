@@ -80,6 +80,9 @@ class AccurateRunner:
                 conv, bn, act, slope = _block_parts(m)
                 if conv.groups != 1:
                     raise NotImplementedError("grouped convolution in the accurate mode")
+                if conv.out_channels % 8 and not (i + 1 < len(defs) and defs[i + 1]['type'] == 'yolo'):
+                    raise NotImplementedError("layer %d: %d channels; the accurate mode needs multiples of 8 outside "
+                                              "the YOLO heads" % (i, conv.out_channels))
                 h = self._conv(i, conv, bn, act, slope, h)
             elif t == 'shortcut':
                 if getattr(m, 'weight', False):

@@ -9,7 +9,10 @@ by a static plan over NHWC fp16 buffers:
   * the launch sequence is captured once into a CUDA graph per input shape and replayed.
 
 Parameters stay in the nn.Module tree (fp32, NCHW) and are folded/packed on the device whenever they change.
-Shapes, folded shortcuts and the concat placement come from layout.py, which the training plan shares.
+Shapes, folded shortcuts and the concat placement come from layout.py, which the training plan shares.  Every fp16
+tensor is stored in whole 8-channel groups (layout.phys_width): a channel-pruned width such as 37 runs on the same
+kernels as 40, with zero weight rows and bias for the pad outputs and zero weight columns wherever an input channel is
+a pad or a gap between concat sources.
 """
 import collections
 import os
@@ -71,11 +74,27 @@ def launch_pointwise(st):
                 ops.copy_channels(xv[..., n:], ov[..., n:])
             cur = st.out
     elif st.kind == 'copy':
-        ops.copy_channels(st.src.view(), st.dst.buf[..., st.off:st.off + st.src.C])
+        ops.copy_channels(st.src.view(), st.dst.buf[..., st.off:st.off + st.src.Cp])
     elif st.kind == 'upsample':
         ops.upsample(st.src.view(), st.stride, out=st.out.view())
     elif st.kind == 'maxpool':
         ops.maxpool(st.src.view(), st.k, st.s, tiny_pad=st.tiny_pad, out=st.out.view())
+
+
+def _pad_rows(t, n, fill=0.0):
+    """t with n - len(t) entries of `fill` appended along dim 0 (the pad output channels of a weight)."""
+    if t is None or t.shape[0] == n:
+        return t
+    return torch.cat([t, t.new_full((n - t.shape[0],) + tuple(t.shape[1:]), fill)])
+
+
+def _scatter(t, dim, cmap, n):
+    """t with entry j along `dim` moved to position cmap[j] of a zero tensor of length n there (layout.Layout.chmap)."""
+    if t is None:
+        return None
+    shape = list(t.shape)
+    shape[dim] = n
+    return t.new_zeros(shape).index_copy_(dim, torch.as_tensor(cmap, device=t.device), t).contiguous()
 
 
 def fold_bn(conv, bn):
@@ -94,7 +113,8 @@ def fold_bn(conv, bn):
 class LazyFeatures(list):
     """feature_out of the reference API (models.py:542-543): one entry per conv block that does not feed a YOLO layer.
     Entries are materialised (NHWC fp16 -> NCHW fp32) on access; they alias engine buffers and are only valid
-    until the next forward."""
+    until the next forward.  An entry is the NHWC view of the logical channels, or (physical view, logical channel
+    index) for a tensor whose channels a concat placed with gaps."""
 
     def __init__(self, views):
         super().__init__([None] * len(views))
@@ -106,6 +126,8 @@ class LazyFeatures(list):
         v = self._views[i]
         if v is None:
             raise RuntimeError("feature_out[%d] was not kept: set model.keep_features = True before the forward" % i)
+        if isinstance(v, tuple):
+            return ops.nhwc_to_nchw(v[0]).index_select(1, v[1])
         return ops.nhwc_to_nchw(v)
 
     def __iter__(self):
@@ -209,14 +231,18 @@ class Plan:
         defs, mods = model.module_defs, model.module_list
         n = len(defs)
         shapes = infer_shapes(model, (self.Cin, self.H, self.W))
-        # inference folds a shortcut into the residual epilogue of the conv before it for multiples of 8 channels
-        lay = build_layout(model, shapes, self.keep_features, lambda i: shapes[i][0] % 8 == 0)
+        # inference folds a shortcut into the residual epilogue of the conv before it; the epilogue reads whole
+        # 8-channel groups, which every physical width is
+        lay = build_layout(model, shapes, self.keep_features, lambda i: True)
         tens, fused_into = lay.tens, lay.fused_into
+        self.chmap = lay.chmap
 
-        # multi-source routes are buffers their producers write into
+        # multi-source routes are buffers their producers write into; a conv reads a placed source through view_k, up to
+        # its next 16-channel boundary, which may lie past the concat's own width
         for i, parts in lay.concats.items():
             dst = tens[i]
-            dst.buf = self._new_act(('cat', i), dst.C, dst.H, dst.W)
+            width = max([dst.Cp] + [off + (st.Cp + 15) // 16 * 16 for st, off, placed in parts if placed])
+            dst.buf = self._new_act(('cat', i), width, dst.H, dst.W)
             for st, off, placed in parts:
                 if placed:
                     st.buf = dst.buf
@@ -225,9 +251,9 @@ class Plan:
         def alloc(t, i):
             if t.buf is None:
                 if t.dtype == torch.float16:
-                    t.buf = self._new_act(i, t.C, t.H, t.W)
+                    t.buf = self._new_act(i, t.Cp, t.H, t.W)
                 else:
-                    pc = pitch(t.C, t.dtype)
+                    pc = pitch(t.Cp, t.dtype)
                     t.buf = self._take(('head', i, pc, t.dtype), (B, t.H, t.W, pc), t.dtype)
             return t
 
@@ -243,7 +269,7 @@ class Plan:
             elif t == 'se':
                 fc = m[0].fc if isinstance(m, nn.Sequential) else m.fc
                 src = tens[i - 1]
-                ws = self._take(('se_ws', i), (B, 3 * src.C + fc[0].out_features), torch.float32)
+                ws = self._take(('se_ws', i), (B, 3 * src.Cp + fc[0].out_features), torch.float32)
                 self.steps.append(SeStep('se', i, src, alloc(tens[i], i), fc[0], fc[2], ws))
             elif t == 'convolutional':
                 conv, bn, act, slope = _block_parts(m)
@@ -263,8 +289,16 @@ class Plan:
             else:
                 self.steps += pointwise_steps(lay, i, d, m, alloc)
         self.total_rows = row_off
-        self.feature_views = [tens[i] if self.keep_features else None for i in feature_slots(model)]
+        self.feature_views = [self._logical(tens[i], lay.chmap[i]) if self.keep_features else None
+                              for i in feature_slots(model)]
         self.anchors_px = [m.anchors.to(self.device).float().contiguous() for (m, _, _, _) in self.yolo]
+
+    def _logical(self, t, cmap):
+        """(tensor, None) when its logical channels are the first C physical ones (the map is strictly increasing, so
+        it is the identity when it ends at C - 1), else (tensor, device index of its logical channels)."""
+        if cmap[-1] == t.C - 1:
+            return t, None
+        return t, torch.as_tensor(cmap, device=self.device)
 
     # ---------------------------------------------------------------------------------------------------------
     def _params_version(self):
@@ -286,13 +320,19 @@ class Plan:
             sw.version = ver
         packs = sw.packs
         for st in self.steps:
-            if st.kind == 'dw':
-                key = self.wkey[st.i] = (st.i, 'dw')
+            if st.kind in ('dw', 'se'):
+                # channel by channel over the input's physical channels: zero weights, scale and bias (squeeze-excite:
+                # zero fc1 columns and fc2 rows) for its pad and gap channels
+                key = self.wkey[st.i] = (st.i, st.kind)
                 if key not in packs:
-                    sc, bi = fold_bn(st.conv, st.bn)
-                    packs[key] = (st.conv.weight.detach().float().contiguous(),
-                                  sc.contiguous() if sc is not None else None,
-                                  bi.contiguous() if bi is not None else None)
+                    cmap, cp = self.chmap[st.i - 1], st.src.Cp
+                    if st.kind == 'dw':
+                        sc, bi = fold_bn(st.conv, st.bn)
+                        packs[key] = (_scatter(st.conv.weight.detach().float(), 0, cmap, cp),
+                                      _scatter(sc, 0, cmap, cp), _scatter(bi, 0, cmap, cp))
+                    else:
+                        packs[key] = (_scatter(st.fc1.weight.detach(), 1, cmap, cp),
+                                      _scatter(st.fc2.weight.detach(), 0, cmap, cp))
                 continue
             if st.kind != 'conv':
                 continue
@@ -308,12 +348,17 @@ class Plan:
                 eps = bn.eps
             base = packs.get((i, 'base'))
             if base is None:
-                stem = conv.in_channels <= 4
-                wsrc = conv.weight.detach()
-                if not stem and conv.in_channels % 16 != 0:      # zero columns for the padded K channels (view_k)
-                    wsrc = torch.nn.functional.pad(wsrc, (0, 0, 0, 0, 0, (-conv.in_channels) % 16))
-                wp, bias, w32 = ops.pack_conv_weights(wsrc, conv.bias.detach() if conv.bias is not None
-                                                      else None, bnp, eps, want_fp32=stem)
+                stem = st.src is None
+                # [Cp_out][K][kh][kw]: zero rows, bias and BatchNorm scale for the pad outputs (BatchNorm padded with
+                # gamma = beta = mean = 0, var = 1); the input columns go through the source's channel map, with zero
+                # columns for its pad and gap channels and up to the MMA K granule (view_k)
+                cp = st.out.Cp
+                wsrc = _pad_rows(conv.weight.detach(), cp)
+                if not stem:
+                    wsrc = _scatter(wsrc, 1, self.chmap[i - 1], (st.src.Cp + 15) // 16 * 16)
+                bnp_p = None if bnp is None else tuple(_pad_rows(t, cp, f) for t, f in zip(bnp, (0.0, 0.0, 0.0, 1.0)))
+                wp, bias, w32 = ops.pack_conv_weights(wsrc, _pad_rows(conv.bias.detach(), cp) if conv.bias is not None
+                                                      else None, bnp_p, eps, want_fp32=stem)
                 wstem = None
                 if stem and (conv.in_channels * conv.kernel_size[0] <= 16 or
                              conv.in_channels * conv.kernel_size[0] ** 2 <= 32):
@@ -341,7 +386,7 @@ class Plan:
             return False
         if conv.in_channels != 32 or conv.out_channels > 128 or conv.out_channels % 8 or src.W % 2:
             return False
-        full = lambda t: t.c0 == 0 and t.buf.shape[3] == t.C and t.dtype == torch.float16
+        full = lambda t: t.c0 == 0 and t.buf.shape[3] == t.C == t.Cp and t.dtype == torch.float16
         return full(src) and full(out) and (res is None or full(res))
 
     def _s2_pair_packable(self, st):
@@ -354,7 +399,8 @@ class Plan:
             return False
         if conv.in_channels != 32 or src.W % 2:
             return False
-        return src.c0 == 0 and src.buf.shape[3] == src.C and src.dtype == torch.float16
+        return (src.c0 == 0 and src.buf.shape[3] == src.C == src.Cp and st.out.C == st.out.Cp
+                and src.dtype == torch.float16)
 
     def _pair_pack(self, conv, bnp, eps):
         _, bias, w32 = ops.pack_conv_weights(conv.weight.detach(), conv.bias.detach() if conv.bias is not None else None,
@@ -370,7 +416,7 @@ class Plan:
         if src is None:
             if conv.in_channels > 4:
                 raise NotImplementedError("first layer with more than 4 input channels")
-            if wstem is not None and wstem.dim() == 2 and conv.out_channels <= 64:
+            if wstem is not None and wstem.dim() == 2 and out.Cp <= 64:
                 # full-im2col weight layout: the fused kernel builds the A tile in smem (no workspace)
                 ops.stem_conv_fused(x, wstem, bias, k, s, p, act=act, slope=slope, out=out.view(),
                                     x_div=256.0 if x.dtype == torch.uint8 else 1.0)
@@ -407,7 +453,8 @@ class Plan:
                 ops.dwconv2d(st.src.view(), w, conv.kernel_size[0], conv.stride[0], conv.padding[0], scale=sc, bias=bi,
                              act=st.act, slope=st.slope, out=st.out.view())
             elif st.kind == 'se':
-                ops.se_fwd(st.src.view(), st.fc1.weight.detach(), st.fc2.weight.detach(), out=st.out.view(), ws=st.ws)
+                w1, w2 = self._w(st.i)
+                ops.se_fwd(st.src.view(), w1, w2, out=st.out.view(), ws=st.ws)
             else:
                 launch_pointwise(st)
         for (m, raw, row_off, rows), anc in zip(self.yolo, self.anchors_px):
@@ -455,7 +502,8 @@ class Plan:
                 io, p = self.io.clone(), tuple(t.clone() for t in self.static_p)
         for (m, raw, _, _) in self.yolo:
             m.nx, m.ny = raw.W, raw.H
-        feats = LazyFeatures([None if t is None else t.view() for t in self.feature_views])
+        feats = LazyFeatures([None if f is None else f[0].buf[..., f[0].c0:f[0].c0 + f[0].C] if f[1] is None
+                              else (f[0].view(), f[1]) for f in self.feature_views])
         return io, p, feats
 
 

@@ -14,16 +14,24 @@ _ACT_OF_CLASS = {'LeakyReLU': 'leaky', 'Mish': 'mish', 'ReLU6': 'relu6', 'HardSw
 LAYER_TYPES = ('convolutional', 'depthwise', 'se', 'maxpool', 'upsample', 'route', 'shortcut', 'yolo')
 
 
-class _Tensor:
-    """Logical activation tensor: NHWC view = buffer[..., c0:c0+C]."""
-    __slots__ = ('C', 'H', 'W', 'buf', 'c0', 'dtype')
+def phys_width(C):
+    """Physical channel count of an fp16 activation with C logical channels: whole 8-channel groups (16 bytes), which
+    every elementwise, depthwise and squeeze-excite kernel and the 16-byte alignment of concat slots need.  Channels
+    C .. phys_width(C) - 1 hold zeros (see Layout.chmap)."""
+    return (C + 7) // 8 * 8
 
-    def __init__(self, C, H, W, dtype=torch.float16):
+
+class _Tensor:
+    """Activation tensor of C logical channels stored as Cp physical ones: NHWC view = buffer[..., c0:c0+Cp]."""
+    __slots__ = ('C', 'Cp', 'H', 'W', 'buf', 'c0', 'dtype')
+
+    def __init__(self, C, H, W, dtype=torch.float16, Cp=None):
         self.C, self.H, self.W, self.dtype = C, H, W, dtype
+        self.Cp = C if Cp is None else Cp
         self.buf, self.c0 = None, 0
 
     def view(self):
-        return self.buf[..., self.c0:self.c0 + self.C]
+        return self.buf[..., self.c0:self.c0 + self.Cp]
 
     def view_k(self):
         """View for a tensor-core consumer: the channel count rounded up to 16 (the MMA K granule is 16 fp16 elements).
@@ -31,11 +39,11 @@ class _Tensor:
         is a multiple of 16 and nobody ever writes the pad channels, the packed weights carry zero columns there (a
         tensor living inside a concat buffer may see its neighbour's channels instead of zeros: finite values times
         zero weights)."""
-        ck = (self.C + 15) // 16 * 16
-        if ck == self.C:
+        ck = (self.Cp + 15) // 16 * 16
+        if ck == self.Cp:
             return self.view()
         if self.c0 + ck > self.buf.shape[3]:
-            raise RuntimeError("activation buffer too narrow for the padded channel view (C=%d)" % self.C)
+            raise RuntimeError("activation buffer too narrow for the padded channel view (C=%d)" % self.Cp)
         return self.buf[..., self.c0:self.c0 + ck]
 
 
@@ -117,8 +125,57 @@ class Layout:
     concats     {multi-source route i: [(source tensor, channel offset, placed)]}: a placed source lives inside the
                 route's buffer (its c0 is the offset, the plan gives it the route's buffer), the others are copied
     grouped     {grouped route i: the tensor whose upper channel half it is}; its c0 is set, the plan gives it that
-                tensor's buffer"""
-    __slots__ = ('shapes', 'is_head', 'fused_into', 'tens', 'concats', 'grouped')
+                tensor's buffer
+    chmap       per layer (None for yolo layers): the physical channel, relative to the tensor's c0, of each logical
+                channel.  The identity except behind a multi-source route, whose sources sit at offsets that are sums
+                of physical widths, with zero channels between them; every layer that works channel by channel
+                (depthwise, squeeze-excite, max-pool, up-sample, shortcut) keeps its input's map.  A consumer of weights
+                scatters its input columns through it."""
+    __slots__ = ('shapes', 'is_head', 'fused_into', 'tens', 'concats', 'grouped', 'chmap')
+
+
+def _channel_maps(defs, shapes, is_head):
+    """(physical width, logical -> physical channel map) of every layer's output tensor, in layer order."""
+    n = len(defs)
+    cp, chmap = [None] * n, [None] * n
+    for i, d in enumerate(defs):
+        t, C = d['type'], shapes[i][0]
+        if t == 'yolo':
+            continue
+        if t == 'convolutional':
+            cp[i], chmap[i] = (C if is_head[i] else phys_width(C)), tuple(range(C))
+        elif t in ('depthwise', 'se', 'maxpool', 'upsample'):
+            cp[i], chmap[i] = cp[i - 1], chmap[i - 1]
+        elif t == 'shortcut':
+            cp[i], chmap[i] = cp[i - 1], chmap[i - 1]
+            for s in sources(i, d['from']):
+                k = min(C, shapes[s][0])
+                if chmap[s][:k] != chmap[i - 1][:k]:
+                    raise NotImplementedError("layer %d: shortcut over addends whose channels are placed differently "
+                                              "(one of them is a concat of widths that are not multiples of 8)" % i)
+                if shapes[s][0] > C and min(cp[s], cp[i]) > C:
+                    # the add covers whole 8-channel groups and would write the wider addend into the pad channels
+                    raise NotImplementedError("layer %d: shortcut whose addend is wider than its %d-channel input, "
+                                              "which is not a multiple of 8" % (i, C))
+        elif t == 'route':
+            srcs = sources(i, d['layers'])
+            if len(srcs) > 1:
+                off, m = 0, []
+                for s in srcs:
+                    m += [off + c for c in chmap[s]]
+                    off += cp[s]
+                cp[i], chmap[i] = off, tuple(m)
+            elif 'groups' in d:
+                src_map = chmap[i - 1]
+                half = len(src_map) // 2
+                p0 = src_map[half]
+                if len(src_map) % 2 or p0 % 8:
+                    raise NotImplementedError("layer %d: grouped route over %d channels: its upper half does not start "
+                                              "on an 8-channel boundary" % (i, len(src_map)))
+                cp[i], chmap[i] = cp[i - 1] - p0, tuple(c - p0 for c in src_map[half:])
+            else:
+                cp[i], chmap[i] = cp[srcs[0]], chmap[srcs[0]]
+    return cp, chmap
 
 
 def build_layout(model, shapes, keep_features, fuse_ok):
@@ -133,18 +190,22 @@ def build_layout(model, shapes, keep_features, fuse_ok):
     for i, d in enumerate(defs):
         if d['type'] == 'yolo' and i > 0 and defs[i - 1]['type'] == 'convolutional':
             is_head[i - 1] = True
+    cp, chmap = _channel_maps(defs, shapes, is_head)
+    lay.chmap = chmap
+    for i, d in enumerate(defs):
         if d['type'] == 'shortcut' and i > 1:
             frm = sources(i, d['from'])
             if (not keep_features  # feature_out must expose the conv output *before* the add
                     and len(frm) == 1 and defs[i - 1]['type'] == 'convolutional' and not routs[i - 1]
-                    and not getattr(mods[i], 'weight', False) and shapes[frm[0]] == shapes[i - 1] and fuse_ok(i - 1)):
+                    and not getattr(mods[i], 'weight', False) and shapes[frm[0]] == shapes[i - 1]
+                    and chmap[frm[0]] == chmap[i - 1] and cp[frm[0]] == cp[i - 1] and fuse_ok(i - 1)):
                 fused_into[i] = i - 1
 
     is_alias = lambda d: d['type'] == 'route' and len(d['layers']) == 1 and 'groups' not in d
     tens = lay.tens = [None] * n
     for i, d in enumerate(defs):
         if d['type'] != 'yolo' and not is_alias(d):
-            tens[i] = _Tensor(*shapes[i], torch.float32 if is_head[i] else torch.float16)
+            tens[i] = _Tensor(*shapes[i], torch.float32 if is_head[i] else torch.float16, Cp=cp[i])
     for i in range(n):
         if fused_into[i] is not None:
             tens[fused_into[i]] = tens[i]
@@ -157,8 +218,8 @@ def build_layout(model, shapes, keep_features, fuse_ok):
             alias[i] = src
             tens[i] = tens[src]
 
-    # concat placement: a source is written in place when it is fp16, not yet inside another concat, not a concat
-    # itself, and starts on a 16-byte boundary of the pixel row; otherwise it is copied
+    # concat placement at physical offsets: a source is written in place when it is fp16, not yet inside another
+    # concat, not a concat itself, and starts on a 16-byte boundary of the pixel row; otherwise it is copied
     lay.concats = {}
     taken = set()
     for i, d in enumerate(defs):
@@ -174,12 +235,12 @@ def build_layout(model, shapes, keep_features, fuse_ok):
                 st.c0 = off
                 taken.add(id(st))
             parts.append((st, off, placed))
-            off += st.C
+            off += st.Cp
         lay.concats[i] = parts
     lay.grouped = {}
     for i, d in enumerate(defs):
         if d['type'] == 'route' and len(d['layers']) == 1 and 'groups' in d:
             src = tens[i - 1]
-            tens[i].c0 = src.c0 + src.C // 2
+            tens[i].c0 = src.c0 + src.Cp - tens[i].Cp
             lay.grouped[i] = src
     return lay

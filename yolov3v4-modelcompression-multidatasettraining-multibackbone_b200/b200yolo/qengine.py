@@ -71,7 +71,8 @@ class QPlan:
                 pitch = 256 if head else Cc
                 out.buf = torch.empty((B, H, W, pitch), dtype=out.dtype, device=dev)
                 if not head and Cc % 16 != 0:
-                    raise NotImplementedError("int8 graph needs channel counts that are multiples of 16")
+                    raise NotImplementedError("layer %d: int8 graph needs channel counts that are multiples of 16 "
+                                              "(got %d)" % (i, Cc))
                 self.steps.append(('conv', i, None if i == 0 else tens[i - 1], out, conv, head))
                 tens[i] = out
             elif t == 'shortcut':
