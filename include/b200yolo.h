@@ -189,12 +189,14 @@ int b2y_yolo_decode(const float* raw, long long raw_pitch, float* p, float* io, 
  *   out[0]=sum(1-giou) out[1]=matches out[2]=sum BCE(cls) out[3]=sum BCE(obj) (fp32[4], overwritten)
  *   dp       fp32 same shape as p: d(lbox*w_box + lobj*w_obj + lcls*w_cls)/dp with the reference's
  *            'mean' reductions (NULL = forward only)
+ *   fl_gamma hyp['fl_gamma']: > 0 wraps the class and objectness BCE in the focal loss (utils/utils.py:333-360,
+ *            alpha 0.25); 0 = plain BCE.  Negative or NaN: B2Y_ERR_INVALID
  *   workspace: b2y_yolo_loss_workspace_bytes(...) bytes
  * ------------------------------------------------------------------------------------------------ */
 size_t b2y_yolo_loss_workspace_bytes(int batch, int na, int ny, int nx, int nt);
 int b2y_yolo_loss(const float* p, const float* targets, int nt, const float* anchors, int batch, int na, int no,
                   int ny, int nx, float iou_t, float gr, float cls_pw, float obj_pw, float w_box, float w_obj,
-                  float w_cls, float* out4, float* dp, void* workspace, void* stream);
+                  float w_cls, float fl_gamma, float* out4, float* dp, void* workspace, void* stream);
 /* build_targets only: writes up to na*nt matches in reference order (anchor-major, target-minor);
  *   idx int64 [4][na*nt] rows (b, a, gj, gi), tbox fp32 [na*nt][4], tcls int64 [na*nt], count int32[1] */
 int b2y_build_targets(const float* targets, int nt, const float* anchors, int na, int ny, int nx, float iou_t,

@@ -2,7 +2,7 @@
 
 The reference ships its cfg files under cfg/**; they are data, not code, and are not copied into this repo.
 This module re-creates the architectures (YOLOv3 / Darknet-53, YOLOv3-tiny, YOLOv4 / CSPDarknet-53 + SPP + PAN,
-YOLOv4-tiny) from their published structure so that tests and bench.py work on a box without /root/reference.
+YOLOv4-tiny, YOLOv2 / Darknet-19 and YOLOv2-tiny with one 5-anchor head) from their published structure so that tests and bench.py work on a box without /root/reference.
 tests/test_cfg_parity.py checks (when the reference is present) that the generated text parses to the same
 module definitions as the reference's own cfg files.
 """
@@ -10,6 +10,7 @@ module definitions as the reference's own cfg files.
 COCO_ANCHORS_V3 = "10,13, 16,30, 33,23, 30,61, 62,45, 59,119, 116,90, 156,198, 373,326"
 COCO_ANCHORS_V4 = "12, 16, 19, 36, 40, 28, 36, 75, 76, 55, 72, 146, 142, 110, 192, 243, 459, 401"
 TINY_ANCHORS = "10,14, 23,27, 37,58, 81,82, 135,169, 344,319"
+V2_ANCHORS = "7,12, 19,30, 45,61, 90,141, 240,279"
 
 
 class _Cfg:
@@ -213,7 +214,43 @@ def yolov3_mobilenet(classes=80):
     return c.text()
 
 
-ARCHS = {"yolov3": yolov3, "yolov3-tiny": yolov3_tiny, "yolov4": yolov4, "yolov3-mobilenet": yolov3_mobilenet}
+def _v2_head(c, classes):
+    """One stride-32 head over all five anchors: 5 * (classes + 5) filters (425 for 80 classes)."""
+    c.conv(5 * (classes + 5), 1, act="linear", bn=0)
+    c.yolo((0, 1, 2, 3, 4), V2_ANCHORS, classes, 5, (("random", 1),))
+
+
+def yolov2(classes=80):
+    """Darknet-19 (3x3 convs doubling the width per stage, 1x1 bottlenecks at half width between them, 2x2 max-pools)
+    with three 3x3 x 1024 convs before the head."""
+    c = _Cfg(_net(608, 608))
+    for stage, (filters, pairs) in enumerate(((32, 0), (64, 0), (128, 1), (256, 1), (512, 2), (1024, 2))):
+        c.conv(filters, 3)
+        for _ in range(pairs):
+            c.conv(filters // 2, 1)
+            c.conv(filters, 3)
+        if stage < 5:
+            c.maxpool(2, 2)
+    for _ in range(3):
+        c.conv(1024, 3)
+    _v2_head(c, classes)
+    return c.text()
+
+
+def yolov2_tiny(classes=80):
+    """Six 3x3 conv + 2x2 max-pool pairs (the last pool with stride 1), two 3x3 x 1024 convs, the head."""
+    c = _Cfg(_net())
+    for i, f in enumerate((16, 32, 64, 128, 256, 512)):
+        c.conv(f, 3)
+        c.maxpool(2, 2 if i < 5 else 1)
+    c.conv(1024, 3)
+    c.conv(1024, 3)
+    _v2_head(c, classes)
+    return c.text()
+
+
+ARCHS = {"yolov3": yolov3, "yolov3-tiny": yolov3_tiny, "yolov4": yolov4, "yolov3-mobilenet": yolov3_mobilenet,
+         "yolov2": yolov2, "yolov2-tiny": yolov2_tiny}
 
 
 def cfg_text(name, classes=80):

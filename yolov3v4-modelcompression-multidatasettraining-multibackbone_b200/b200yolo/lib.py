@@ -89,8 +89,8 @@ _PROTOS = {
     "b2y_nhwc_f16_to_nchw_f32": (i32, [vp, ll, vp, i32, i32, i32, i32, vp]),
     "b2y_yolo_decode": (i32, [vp, ll, vp, vp, ll, ll, i32, i32, i32, i32, i32, vp, f32, vp]),
     "b2y_yolo_loss_workspace_bytes": (sz, [i32, i32, i32, i32, i32]),
-    "b2y_yolo_loss": (i32, [vp, vp, i32, vp, i32, i32, i32, i32, i32, f32, f32, f32, f32, f32, f32, f32, vp, vp,
-                            vp, vp]),
+    "b2y_yolo_loss": (i32, [vp, vp, i32, vp, i32, i32, i32, i32, i32, f32, f32, f32, f32, f32, f32, f32, f32, vp,
+                            vp, vp, vp]),
     "b2y_build_targets": (i32, [vp, i32, vp, i32, i32, i32, f32, vp, vp, vp, vp, vp]),
     "b2y_qconv2d_fwd": (i32, [C.POINTER(QConvDesc), vp, vp, vp, vp, vp]),
     "b2y_qconv2d_shortcut_fwd": (i32, [C.POINTER(QConvDesc), vp, vp, vp, vp, ll, f32, f32, f32, f32, f32, f32, vp, vp]),

@@ -257,8 +257,10 @@ def yolo_decode(raw, na, no, anchors_px, stride, io=None, row_offset=0, want_p=T
     return io, p
 
 
-def yolo_loss_layer(p, targets, anchor_vec, iou_t, gr, cls_pw, obj_pw, w_box, w_obj, w_cls, want_grad=True):
-    """One yolo layer of compute_loss. Returns (out4 fp32[4] = [sum(1-giou), nb, sum bce cls, sum bce obj], dp)."""
+def yolo_loss_layer(p, targets, anchor_vec, iou_t, gr, cls_pw, obj_pw, w_box, w_obj, w_cls, want_grad=True,
+                    fl_gamma=0.0):
+    """One yolo layer of compute_loss. Returns (out4 fp32[4] = [sum(1-giou), nb, sum bce cls, sum bce obj], dp).
+    fl_gamma > 0: the class and objectness terms are focal-modulated BCE (alpha 0.25)."""
     B, na, ny, nx, no = p.shape
     p = p.contiguous()
     nt = int(targets.shape[0])
@@ -268,7 +270,8 @@ def yolo_loss_layer(p, targets, anchor_vec, iou_t, gr, cls_pw, obj_pw, w_box, w_
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=p.device)
     t = targets.contiguous().float() if nt else None
     call("b2y_yolo_loss", ptr(p), ptr(t), nt, ptr(anchor_vec), B, na, no, ny, nx, float(iou_t), float(gr),
-         float(cls_pw), float(obj_pw), float(w_box), float(w_obj), float(w_cls), ptr(out4), ptr(dp), ptr(ws),
+         float(cls_pw), float(obj_pw), float(w_box), float(w_obj), float(w_cls), float(fl_gamma), ptr(out4), ptr(dp),
+         ptr(ws),
          stream_ptr())
     return out4, dp
 

@@ -29,11 +29,17 @@ from .layout import _Tensor, _block_parts, build_layout, feature_slots, infer_sh
 from .lib import ACT, ConvDesc, OUT_F16, call, ptr, stream_ptr
 
 GDT = torch.bfloat16   # gradient tensors: bf16 (range of fp32) -- fp16 over/underflows across ~100 BN layers
-HEAD_PAD = 256  # head convs (255 filters) are run with 256 output channels (zero row) so that K % 16 == 0 in dgrad
 
 
 def _round_up(v, m):
     return (v + m - 1) // m * m
+
+
+def head_width(cout):
+    """Output channels a YOLO head conv runs with: Cout rounded up to the K granule (16) of the data-gradient GEMM,
+    at least 256.  The pad channels are zero rows of the weights and zero columns of the head gradient.  The 256 floor
+    keeps every head of up to 256 filters (255 for 80 classes, 18 for one) on the layout it has always had."""
+    return max(256, _round_up(cout, 16))
 
 
 def _widen(view, channels):
@@ -146,14 +152,15 @@ class TrainPlan:
                     make_grad(st, gdst.buf, off)
 
         def alloc(t, i):
+            hw = head_width(t.C)
             if t.buf is None:
-                t.buf = new_buf(('act', i), t.C if t.dtype == torch.float16 else HEAD_PAD, t.H, t.W, t.dtype)
+                t.buf = new_buf(('act', i), t.C if t.dtype == torch.float16 else hw, t.H, t.W, t.dtype)
             if id(t) not in self.grad_of:
                 if t.dtype == torch.float16:
                     make_grad(t, zeros_later(t.buf.shape, GDT))
                 else:  # head output: its gradient is directly the GEMM operand dZ -> fp16 (times a device-side scale)
-                    g = _Tensor(HEAD_PAD, t.H, t.W, torch.float16)
-                    g.buf = zeros_later((B, t.H, t.W, HEAD_PAD), torch.float16)
+                    g = _Tensor(hw, t.H, t.W, torch.float16)
+                    g.buf = zeros_later((B, t.H, t.W, hw), torch.float16)
                     self.grad_of[id(t)] = g
             return t
 
@@ -186,10 +193,10 @@ class TrainPlan:
                     raise NotImplementedError("first layer with more than 4 input channels")
                 r.Cout = conv.out_channels
                 # GEMM K granule: Cout is the K of the data-gradient GEMM, Cin the K of the forward / weight-gradient one
-                r.Cpad = HEAD_PAD if r.head else _round_up(r.Cout, 16)
+                r.Cpad = head_width(r.Cout) if r.head else _round_up(r.Cout, 16)
                 r.Ipad = _round_up(conv.in_channels, 16)
-                if r.head and (r.Cout > HEAD_PAD or bn is not None or act != 'linear'):
-                    raise NotImplementedError("unsupported YOLO head conv")
+                if r.head and (bn is not None or act != 'linear'):
+                    raise NotImplementedError("unsupported YOLO head conv: BatchNorm or a non-linear activation")
                 r.src = None if i == 0 else tens[i - 1]
                 r.y = alloc(tens[i], i)
                 if i + 1 < n and fused_into[i + 1] == i:
@@ -361,7 +368,7 @@ class TrainPlan:
             if r.stem:
                 w = r.conv.weight.detach()
                 if r.head:
-                    pad = torch.zeros((HEAD_PAD - r.Cout,) + tuple(w.shape[1:]), dtype=w.dtype, device=w.device)
+                    pad = torch.zeros((r.Cpad - r.Cout,) + tuple(w.shape[1:]), dtype=w.dtype, device=w.device)
                     w = torch.cat([w, pad], 0)
                 r.w32 = w.float().contiguous()
                 # tensor-core stem: full-im2col weight layout when the receptive field fits one 64-byte GEMM row
@@ -406,7 +413,7 @@ class TrainPlan:
         for (m, raw) in self.yolo:              # head gradients: written by yolo_grad_to_raw only where a loss exists
             g = G(raw)
             dirty.add(id(g.buf))
-            cov[id(g.buf)] = set(range(0, HEAD_PAD))
+            cov[id(g.buf)] = set(range(0, g.C))
         for idx in range(len(self.order) - 1, -1, -1):
             st = self.order[idx]
             kind = st[0]
@@ -558,7 +565,7 @@ class TrainPlan:
         if r.bn is None:
             bias = r.conv.bias.detach() if r.conv.bias is not None else None
             if r.head and bias is not None:
-                bias = torch.cat([bias, bias.new_zeros(HEAD_PAD - r.Cout)])
+                bias = torch.cat([bias, bias.new_zeros(r.Cpad - r.Cout)])
             out = self._zview(r)
             if r.stem:
                 ops.stem_conv(x, r.w32, bias, r.k, r.s, r.p, act=r.act, slope=r.slope, out=out)
@@ -620,7 +627,7 @@ class TrainPlan:
             g = self.grad_of[id(raw)]
             if dp is None:
                 continue
-            call("b2y_yolo_grad_to_raw", ptr(dp.contiguous().float()), ptr(g.buf), HEAD_PAD, self.B, m.na, m.no, raw.H,
+            call("b2y_yolo_grad_to_raw", ptr(dp.contiguous().float()), ptr(g.buf), g.C, self.B, m.na, m.no, raw.H,
                  raw.W, S, ptr(self.head_scale), ops._gdt(g.buf), stream_ptr())
         G = lambda t: self.grad_of[id(t)]
         for idx in range(len(self.order) - 1, -1, -1):

@@ -226,6 +226,25 @@ __device__ __forceinline__ float bce_logits(float x, float y, float pw, float* d
     return (1.f - y) * x + lw * sp;
 }
 
+// Focal modulation of one BCE element (FocalLoss, utils/utils.py:333-360, alpha = 0.25), applied only when gamma > 0:
+//   l = bce * af * m,   af = y*a + (1-y)*(1-a),   m = (1-p_t)^gamma,   p_t = y*s + (1-y)*(1-s),   s = sigmoid(x)
+// The reference differentiates this with autograd; here in closed form.  With d p_t/dx = (2y-1) * s*(1-s):
+//   dl/dx = af * [ bce' * m + bce * gamma * (1-p_t)^(gamma-1) * (-(2y-1) * s*(1-s)) ]
+// `bce` is the element's BCE value and *dx holds bce' on entry and dl/dx on return.  y may be fractional (objectness).
+// Saturated logits (s rounds to exactly 0 or 1, so 1-p_t = 0): the second term is taken as 0, its limit for x -> +-inf.
+// That equals the reference's gradient for gamma >= 1; for gamma < 1 the reference's autograd gives 0 * inf = NaN there.
+__device__ __forceinline__ float focal_modulate(float x, float y, float gamma, float bce, float* dx) {
+    const float s = sigmoid_f(x);
+    const float omp = 1.f - (y * s + (1.f - y) * (1.f - s));
+    const float af = y * 0.25f + (1.f - y) * 0.75f;
+    const float m = powf(omp, gamma);
+    if (dx != nullptr) {
+        const float dm = omp > 0.f ? gamma * powf(omp, gamma - 1.f) * (-(2.f * y - 1.f) * (s * (1.f - s))) : 0.f;
+        *dx = af * (*dx * m + bce * dm);
+    }
+    return bce * (af * m);
+}
+
 __device__ __forceinline__ float block_sum(float v, float* sh) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -266,8 +285,8 @@ __global__ void loss_assign_kernel(const float* __restrict__ targets, int nt, co
 // K2: per-match box + class loss and their gradients (atomicAdd into dp: duplicates accumulate)
 __global__ void loss_match_kernel(const float* __restrict__ p, const float* __restrict__ targets, int nt,
                                   const float* __restrict__ anchors, int B, int na, int no, int ny, int nx,
-                                  float iou_t, float cls_pw, float w_box, float w_cls, const int* __restrict__ nb_ptr,
-                                  float* __restrict__ out4, float* __restrict__ dp) {
+                                  float iou_t, float cls_pw, float w_box, float w_cls, float fl_gamma,
+                                  const int* __restrict__ nb_ptr, float* __restrict__ out4, float* __restrict__ dp) {
     __shared__ float sh[32];
     const int total = na * nt;
     const int nb = *nb_ptr;
@@ -300,7 +319,9 @@ __global__ void loss_match_kernel(const float* __restrict__ p, const float* __re
             for (int c = lane; c < nc; c += 32) {
                 const float y = (c == m.c) ? 1.f : 0.f;  // cp=1, cn=0 (utils.py:380)
                 float dx;
-                s_cls += bce_logits(ps[5 + c], y, cls_pw, dp ? &dx : nullptr);
+                float l = bce_logits(ps[5 + c], y, cls_pw, dp ? &dx : nullptr);
+                if (fl_gamma > 0.f) l = focal_modulate(ps[5 + c], y, fl_gamma, l, dp ? &dx : nullptr);
+                s_cls += l;
                 if (dp != nullptr) atomicAdd(dp + cell * no + 5 + c, w_cls * inv_cls * dx);
             }
         }
@@ -315,7 +336,7 @@ __global__ void loss_match_kernel(const float* __restrict__ p, const float* __re
 // K3: objectness BCE over every cell; tobj of a matched cell is recomputed from the winning candidate
 __global__ void loss_obj_kernel(const float* __restrict__ p, const float* __restrict__ targets, int nt,
                                 const float* __restrict__ anchors, int B, int na, int no, int ny, int nx, float iou_t,
-                                float gr, float obj_pw, float w_obj, const int* __restrict__ winner,
+                                float gr, float obj_pw, float w_obj, float fl_gamma, const int* __restrict__ winner,
                                 float* __restrict__ out4, float* __restrict__ dp) {
     __shared__ float sh[32];
     const long long cells = (long long)B * na * ny * nx;
@@ -332,7 +353,9 @@ __global__ void loss_obj_kernel(const float* __restrict__ p, const float* __rest
             tobj = (1.f - gr) + gr * fmaxf(giou, 0.f);  // utils.py:407
         }
         float dx;
-        s += bce_logits(p[cell * no + 4], tobj, obj_pw, dp ? &dx : nullptr);
+        float l = bce_logits(p[cell * no + 4], tobj, obj_pw, dp ? &dx : nullptr);
+        if (fl_gamma > 0.f) l = focal_modulate(p[cell * no + 4], tobj, fl_gamma, l, dp ? &dx : nullptr);
+        s += l;
         if (dp != nullptr) dp[cell * no + 4] = w_obj * inv_cells * dx;
     }
     const float r = block_sum(s, sh);
@@ -346,9 +369,11 @@ extern "C" size_t b2y_yolo_loss_workspace_bytes(int batch, int na, int ny, int n
 
 extern "C" int b2y_yolo_loss(const float* p, const float* targets, int nt, const float* anchors, int batch, int na,
                              int no, int ny, int nx, float iou_t, float gr, float cls_pw, float obj_pw, float w_box,
-                             float w_obj, float w_cls, float* out4, float* dp, void* workspace, void* stream) {
+                             float w_obj, float w_cls, float fl_gamma, float* out4, float* dp, void* workspace,
+                             void* stream) {
     if (!p || !anchors || !out4 || !workspace || batch <= 0 || na <= 0 || no < 5 || nt < 0) return B2Y_ERR_INVALID;
     if (nt > 0 && !targets) return B2Y_ERR_INVALID;
+    if (!(fl_gamma >= 0.f)) return B2Y_ERR_INVALID;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long cells = (long long)batch * na * ny * nx;
     int* nb = reinterpret_cast<int*>(workspace);
@@ -362,10 +387,10 @@ extern "C" int b2y_yolo_loss(const float* p, const float* targets, int nt, const
         loss_assign_kernel<<<grid_for(total, 256), 256, 0, st>>>(targets, nt, anchors, batch, na, ny, nx, iou_t, nb,
                                                                  winner);
         loss_match_kernel<<<grid_for((long long)total * 32, 128), 128, 0, st>>>(p, targets, nt, anchors, batch, na, no, ny, nx, iou_t,
-                                                                cls_pw, w_box, w_cls, nb, out4, dp);
+                                                                cls_pw, w_box, w_cls, fl_gamma, nb, out4, dp);
     }
     loss_obj_kernel<<<grid_for(cells, 256), 256, 0, st>>>(p, targets, nt, anchors, batch, na, no, ny, nx, iou_t, gr,
-                                                          obj_pw, w_obj, winner, out4, dp);
+                                                          obj_pw, w_obj, fl_gamma, winner, out4, dp);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }

@@ -50,7 +50,8 @@ def smooth_BCE(eps=0.1):
 
 
 class FocalLoss(nn.Module):
-    """Focal modulation of a BCEWithLogits criterion (inactive in the reference: hyp['fl_gamma'] == 0)."""
+    """Focal modulation of a BCEWithLogits criterion, active when hyp['fl_gamma'] > 0.  compute_loss runs it inside the
+    fused loss kernel (csrc/yolo.cu focal_modulate); this module is the tensor form for callers outside it."""
 
     def __init__(self, loss_fcn, gamma=1.5, alpha=0.25):
         super().__init__()
@@ -164,7 +165,7 @@ class _YoloLoss(torch.autograd.Function):
             cells = pi.numel() // pi.shape[-1]
             out4, dp = ops.yolo_loss_layer(pi.float(), targets, av, hyp['iou_t'], gr, hyp['cls_pw'], hyp['obj_pw'],
                                            hyp['giou'], hyp['obj'], hyp['cls'] if nc > 1 else 0.0,
-                                           want_grad=need_grad)
+                                           want_grad=need_grad, fl_gamma=hyp.get('fl_gamma', 0))
             nb = out4[1]
             has = (nb > 0).float()
             denom = nb.clamp(min=1.0)
@@ -192,12 +193,11 @@ class _YoloLoss(torch.autograd.Function):
 
 
 def compute_loss(p, targets, model):
-    """GIoU box + objectness + class loss of the YOLO head; returns (loss[1], cat(lbox, lobj, lcls, loss).detach())."""
+    """GIoU box + objectness + class loss of the YOLO head; returns (loss[1], cat(lbox, lobj, lcls, loss).detach()).
+    hyp['fl_gamma'] > 0 wraps the class and objectness BCE in the focal loss, as the reference does."""
     if not p[0].is_cuda:
         raise RuntimeError("compute_loss runs on the CUDA device only (no CPU fallback)")
     h = model.hyp
-    if h.get('fl_gamma', 0) > 0:
-        raise NotImplementedError("focal loss (hyp['fl_gamma'] > 0) is not part of the fused sm_90a loss")
     dev = p[0].device
     anchors = [_device_anchor_vec(m, dev) for m in _yolo_modules(model)]
     t = targets.to(dev).float()
