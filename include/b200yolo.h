@@ -315,6 +315,40 @@ int b2y_sgd_nesterov_ema(float* param, const float* grad, float* momentum_buf, f
 int b2y_l1_subgrad_ranges(float* grad, const float* param, const long long* ranges_dev, int n_ranges, float coeff,
                           void* stream);
 
+/* ---- grouped optimiser steps over the flat buffers (train.py:120-150 parameter groups, :356-365 burn-in) ----
+ * One CTA per tile of a device-resident tile table.  A tile is a run of elements of ONE parameter tensor, so its group
+ * (and whether the BatchNorm-L1 term applies, prune_utils.py:133-138) is uniform over the CTA.  flags: bits 0-1 the
+ * group index into B2YOptStep.group, bit 2 the L1 term.  At most B2Y_OPT_TILE elements per tile.  Every buffer is a
+ * flat fp32 buffer with the same element layout and a 16-byte-aligned base. */
+#define B2Y_OPT_MAX_GROUPS 4
+#define B2Y_OPT_TILE 4096
+#define B2Y_OPT_TILE_L1 4
+typedef struct {
+    long long start;
+    int len;
+    int flags;
+} B2YOptTile;
+typedef struct {
+    float lr, momentum, weight_decay;        /* SGD; Adam uses weight_decay (L2, added to the gradient) */
+    float one_minus_beta1, beta2, one_minus_beta2, eps; /* Adam; the complements are rounded from double on the host */
+    float step_size, bc2_sqrt; /* Adam: lr / (1 - beta1^t) and sqrt(1 - beta2^t), computed in double on the host */
+} B2YOptGroup;
+typedef struct {
+    B2YOptGroup group[B2Y_OPT_MAX_GROUPS];
+    float grad_scale; /* 1/world after the NCCL sum */
+    float l1_coeff;   /* s / grad_scale for tiles with B2Y_OPT_TILE_L1 (updateBN runs on the averaged gradient) */
+    float ema_decay;  /* ModelEMA d of this update, used when `ema` is not NULL */
+    int first_step;   /* SGD: the momentum buffer does not exist yet (torch: buf = grad) */
+} B2YOptStep;
+/* Nesterov SGD per group (torch.optim.SGD, nesterov=True, dampening=0); the per-element arithmetic is that of
+ * b2y_sgd_nesterov.  `ema` (optional): ema = d*ema + (1-d)*p_new (utils/torch_utils.py:171-183).  `hp` is read on the
+ * host and passed to the kernel by value. */
+int b2y_sgd_grouped(float* param, const float* grad, float* momentum_buf, float* ema, const B2YOptTile* tiles_dev,
+                    int n_tiles, const B2YOptStep* hp, void* stream);
+/* Adam per group (torch.optim.Adam, amsgrad=False, maximize=False, L2 weight decay); same tiles, EMA and L1 terms */
+int b2y_adam_grouped(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* ema,
+                     const B2YOptTile* tiles_dev, int n_tiles, const B2YOptStep* hp, void* stream);
+
 /* ---- bandwidth-oriented BatchNorm passes of the training step (csrc/bn_train.cu; models.py:100-113 under autograd) ----
  * save = fp32 [4][c]: batch mean, invstd, scale = gamma*invstd, shift = beta - mean*scale.
  * forward: derives them from the conv epilogue's channel sums (biased variance), updates the running statistics

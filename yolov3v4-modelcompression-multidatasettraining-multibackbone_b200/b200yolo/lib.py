@@ -32,6 +32,19 @@ class ConvDesc(C.Structure):
 
 WLAYOUT_DENSE, WLAYOUT_S2_PAIRS = 0, 1
 
+OPT_MAX_GROUPS, OPT_TILE, OPT_TILE_L1 = 4, 4096, 4
+
+
+class OptGroup(C.Structure):
+    _fields_ = [("lr", C.c_float), ("momentum", C.c_float), ("weight_decay", C.c_float),
+                ("one_minus_beta1", C.c_float), ("beta2", C.c_float), ("one_minus_beta2", C.c_float), ("eps", C.c_float),
+                ("step_size", C.c_float), ("bc2_sqrt", C.c_float)]
+
+
+class OptStep(C.Structure):
+    _fields_ = [("group", OptGroup * OPT_MAX_GROUPS), ("grad_scale", C.c_float), ("l1_coeff", C.c_float),
+                ("ema_decay", C.c_float), ("first_step", C.c_int)]
+
 
 class PackItem(C.Structure):
     _fields_ = [("w", C.c_void_p), ("w_fwd", C.c_void_p), ("w_dgrad", C.c_void_p),
@@ -132,6 +145,8 @@ _PROTOS = {
     "b2y_pack_conv_weights_multi": (i32, [vp, i32, i32, vp]),
     "b2y_unpack_wgrad_multi": (i32, [vp, i32, i32, vp]),
     "b2y_l1_subgrad_ranges": (i32, [vp, vp, vp, i32, f32, vp]),
+    "b2y_sgd_grouped": (i32, [vp, vp, vp, vp, vp, i32, C.POINTER(OptStep), vp]),
+    "b2y_adam_grouped": (i32, [vp, vp, vp, vp, vp, vp, i32, C.POINTER(OptStep), vp]),
     "b2y_kd_soft_rows": (i32, [vp, vp, ll, i32, i32, i32, f32, f32, vp, vp, vp]),
     "b2y_kd_box": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp, vp, vp, vp]),
     "b2y_letterbox_u8": (i32, [vp, i32, i32, i32, ll, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp]),

@@ -477,6 +477,30 @@ def sgd_nesterov(param, grad, buf, lr, momentum, weight_decay, grad_scale=1.0, f
          float(weight_decay), float(grad_scale), 1 if first_step else 0, stream_ptr())
 
 
+def _opt_check(tiles, *flat):
+    _require_cuda(tiles, *flat)
+    assert tiles.dtype == torch.int64 and tiles.dim() == 2 and tiles.shape[1] == 2 and tiles.is_contiguous()
+    n = flat[0].numel()
+    for t in flat:
+        if t is not None:
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n
+
+
+def sgd_grouped(param, grad, buf, tiles, hp, ema=None):
+    """Nesterov SGD per parameter group over flat buffers in one launch (csrc/train.cu opt_grouped_kernel).  `tiles` is
+    the int64 [n][2] device table of B2YOptTile rows, `hp` a lib.OptStep passed by value."""
+    _opt_check(tiles, param, grad, buf, ema)
+    call("b2y_sgd_grouped", ptr(param), ptr(grad), ptr(buf), ptr(ema), ptr(tiles), int(tiles.shape[0]), C.byref(hp),
+         stream_ptr())
+
+
+def adam_grouped(param, grad, exp_avg, exp_avg_sq, tiles, hp, ema=None):
+    """Adam per parameter group over flat buffers in one launch (torch.optim.Adam semantics, amsgrad=False)."""
+    _opt_check(tiles, param, grad, exp_avg, exp_avg_sq, ema)
+    call("b2y_adam_grouped", ptr(param), ptr(grad), ptr(exp_avg), ptr(exp_avg_sq), ptr(ema), ptr(tiles),
+         int(tiles.shape[0]), C.byref(hp), stream_ptr())
+
+
 def l1_subgrad_ranges(grad, param, ranges, coeff):
     """grad[off:off+len] += coeff * sign(param[off:off+len]) for each row (off, len) of the int64 device table `ranges`
     (BNOptimizer.updateBN, prune_utils.py:133-138)."""

@@ -1,5 +1,6 @@
 // Training-mode backward helpers on NHWC fp16 tensors (the per-channel (BatchNorm/bias) + activation gradient reduce,
-// the YOLO-head, upsample and max-pool gradients), and the fused SGD-Nesterov step over a flat fp32 parameter buffer.
+// the YOLO-head, upsample and max-pool gradients), the fused SGD-Nesterov step over a flat fp32 parameter buffer and the
+// per-parameter-group SGD / Adam steps over the same buffers.
 // Reference semantics: activation under autograd (models.py:100-113), optimizer train.py:135-144.  The BatchNorm
 // training passes of the conv layers are in bn_train.cu.
 #include "b200yolo.h"
@@ -235,19 +236,29 @@ extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const voi
 // SGD with Nesterov momentum (torch.optim.SGD semantics, train.py:135-144):
 //   g = grad*grad_scale + wd*p ; buf = first ? g : mu*buf + g ; p -= lr * (g + mu*buf)
 // ------------------------------------------------------------------------------------------------
+// The per-element arithmetic of the step, shared with the grouped kernel so that equal hyper-parameters give
+// bit-identical results.  `b` is the momentum buffer in (ignored when `first`) and out; returns the new weight.
+__device__ __forceinline__ float sgd_nesterov_elem(float w, float g, float& b, float lr, float mu, float wd, float gs,
+                                                   int first) {
+    const float grad = fmaf(wd, w, g * gs);
+    b = first ? grad : fmaf(mu, b, grad);
+    return w - lr * fmaf(mu, b, grad);
+}
+
+// ModelEMA.update (utils/torch_utils.py:171-183) fused into the optimiser pass: ema = d*ema + (1-d)*w_new
+__device__ __forceinline__ float ema_elem(float e, float wn, float d) { return fmaf(d, e, (1.f - d) * wn); }
+
 __global__ void sgd_nesterov_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf,
                                     long long n, float lr, float mu, float wd, float gs, int first,
                                     float* __restrict__ ema, float ema_decay) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
          i += (long long)gridDim.x * blockDim.x) {
         const float w = p[i];
-        const float grad = fmaf(wd, w, g[i] * gs);
-        const float b = first ? grad : fmaf(mu, buf[i], grad);
+        float b = first ? 0.f : buf[i];
+        const float wn = sgd_nesterov_elem(w, g[i], b, lr, mu, wd, gs, first);
         buf[i] = b;
-        const float wn = w - lr * fmaf(mu, b, grad);
         p[i] = wn;
-        // ModelEMA.update (utils/torch_utils.py:171-183) fused into the optimiser pass: ema = d*ema + (1-d)*w_new
-        if (ema != nullptr) ema[i] = fmaf(ema_decay, ema[i], (1.f - ema_decay) * wn);
+        if (ema != nullptr) ema[i] = ema_elem(ema[i], wn, ema_decay);
     }
 }
 
@@ -268,6 +279,140 @@ extern "C" int b2y_sgd_nesterov_ema(float* param, const float* grad, float* mome
         param, grad, momentum_buf, n, lr, momentum, weight_decay, grad_scale, first_step, ema, ema_decay);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Grouped optimiser steps (train.py:120-150 parameter groups, per-group burn-in at :356-365).  One CTA per tile of the
+// table; a tile lies inside one parameter tensor, so its group's hyper-parameters are uniform.  Its unaligned head and
+// tail (< 4 elements each) are scalar, the rest goes in 16-byte vectors, OPT_VEC of them per thread loaded before any is
+// updated.  HBM traffic per element: SGD reads p, g, buf and writes p, buf (20 B; 16 B on the first step, which does
+// not read buf); Adam reads p, g, m, v and writes p, m, v (28 B); the EMA adds 8 B.
+//
+// Order of operations per element (g is the NCCL sum of the per-rank gradients):
+//   1. g += (s / gs) * sign(w)  on L1 tiles -- BNOptimizer.updateBN on the averaged gradient (prune_utils.py:133-138)
+//   2. g  = g * gs              -- DDP's mean over ranks
+//   3. SGD:  g = g + wd*w ; buf = first ? g : mu*buf + g ; w -= lr * (g + mu*buf)          (sgd_nesterov_elem)
+//      Adam: g = g + wd*w                                   (grad.add(param, alpha=weight_decay))
+//            m = m + (1-b1)*(g - m)                         (exp_avg.lerp_(grad, 1-beta1))
+//            v = v*b2 + (1-b2)*g*g                          (exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1-beta2))
+//            w = w - step_size * m / (sqrt(v)/bc2_sqrt + eps)   step_size = lr/(1-b1^t), bc2_sqrt = sqrt(1-b2^t)
+//   4. ema = d*ema + (1-d)*w    -- ModelEMA.update on the new weight
+// ------------------------------------------------------------------------------------------------
+constexpr int OPT_THREADS = 256;
+constexpr int OPT_VEC = B2Y_OPT_TILE / (4 * OPT_THREADS);
+static_assert(OPT_VEC * 4 * OPT_THREADS == B2Y_OPT_TILE, "a tile is OPT_VEC float4 per thread");
+
+template <bool ADAM>
+__device__ __forceinline__ float opt_elem(float w, float g, float& s0, float& s1, const B2YOptGroup& G,
+                                          const B2YOptStep& hp, bool l1) {
+    if (l1) g = fmaf(hp.l1_coeff, (float)((w > 0.f) - (w < 0.f)), g);       // torch.sign: 0 at 0
+    if (!ADAM) return sgd_nesterov_elem(w, g, s0, G.lr, G.momentum, G.weight_decay, hp.grad_scale, hp.first_step);
+    const float gr = fmaf(G.weight_decay, w, g * hp.grad_scale);
+    s0 = fmaf(G.one_minus_beta1, gr - s0, s0);
+    s1 = fmaf(G.one_minus_beta2, gr * gr, s1 * G.beta2);
+    const float denom = sqrtf(s1) / G.bc2_sqrt + G.eps;
+    return w - G.step_size * (s0 / denom);
+}
+
+template <bool ADAM, bool EMA>
+__global__ void __launch_bounds__(OPT_THREADS)
+opt_grouped_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ s0, float* __restrict__ s1,
+                   float* __restrict__ ema, const B2YOptTile* __restrict__ tiles, const B2YOptStep hp) {
+    const B2YOptTile t = tiles[blockIdx.x];
+    const B2YOptGroup G = hp.group[t.flags & (B2Y_OPT_MAX_GROUPS - 1)];
+    const bool l1 = (t.flags & B2Y_OPT_TILE_L1) != 0;
+    const bool load_s0 = ADAM || !hp.first_step;
+    const long long s = t.start, e = s + t.len;
+    const long long a0 = min(e, (s + 3) & ~3LL), a1 = max(a0, e & ~3LL);   // [a0, a1): whole float4s
+    const int tid = threadIdx.x;
+
+    auto scalar = [&](long long i) {
+        float m0 = load_s0 ? s0[i] : 0.f, m1 = ADAM ? s1[i] : 0.f;
+        const float wn = opt_elem<ADAM>(p[i], g[i], m0, m1, G, hp, l1);
+        p[i] = wn;
+        s0[i] = m0;
+        if (ADAM) s1[i] = m1;
+        if (EMA) ema[i] = ema_elem(ema[i], wn, hp.ema_decay);
+    };
+    if (tid < a0 - s) scalar(s + tid);
+    if (tid < e - a1) scalar(a1 + tid);
+
+    float4* p4 = reinterpret_cast<float4*>(p);
+    const float4* g4 = reinterpret_cast<const float4*>(g);
+    float4* s04 = reinterpret_cast<float4*>(s0);
+    float4* s14 = reinterpret_cast<float4*>(s1);
+    float4* e4 = reinterpret_cast<float4*>(ema);
+    const long long v0 = a0 >> 2, nv = (a1 - a0) >> 2;
+    float4 vp[OPT_VEC], vg[OPT_VEC], va[OPT_VEC], vb[OPT_VEC], ve[OPT_VEC];
+#pragma unroll
+    for (int k = 0; k < OPT_VEC; ++k) {
+        const long long j = tid + k * OPT_THREADS;
+        if (j < nv) {
+            vp[k] = p4[v0 + j];
+            vg[k] = g4[v0 + j];
+            va[k] = load_s0 ? s04[v0 + j] : make_float4(0.f, 0.f, 0.f, 0.f);
+            if (ADAM) vb[k] = s14[v0 + j];
+            if (EMA) ve[k] = e4[v0 + j];
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < OPT_VEC; ++k) {
+        const long long j = tid + k * OPT_THREADS;
+        if (j < nv) {
+            float4 w = vp[k], a = va[k], b = ADAM ? vb[k] : make_float4(0.f, 0.f, 0.f, 0.f);
+            w.x = opt_elem<ADAM>(w.x, vg[k].x, a.x, b.x, G, hp, l1);
+            w.y = opt_elem<ADAM>(w.y, vg[k].y, a.y, b.y, G, hp, l1);
+            w.z = opt_elem<ADAM>(w.z, vg[k].z, a.z, b.z, G, hp, l1);
+            w.w = opt_elem<ADAM>(w.w, vg[k].w, a.w, b.w, G, hp, l1);
+            p4[v0 + j] = w;
+            s04[v0 + j] = a;
+            if (ADAM) s14[v0 + j] = b;
+            if (EMA) {
+                float4 em = ve[k];
+                em.x = ema_elem(em.x, w.x, hp.ema_decay);
+                em.y = ema_elem(em.y, w.y, hp.ema_decay);
+                em.z = ema_elem(em.z, w.z, hp.ema_decay);
+                em.w = ema_elem(em.w, w.w, hp.ema_decay);
+                e4[v0 + j] = em;
+            }
+        }
+    }
+}
+
+static bool opt_args_ok(const void* const* bufs, int nbufs, const B2YOptTile* tiles, int n_tiles, const B2YOptStep* hp) {
+    if (n_tiles < 0 || hp == nullptr || (n_tiles > 0 && tiles == nullptr)) return false;
+    for (int i = 0; i < nbufs; ++i)
+        if (bufs[i] == nullptr || (reinterpret_cast<uintptr_t>(bufs[i]) & 15) != 0) return false;
+    return true;
+}
+
+template <bool ADAM>
+static int opt_grouped_launch(float* param, const float* grad, float* s0, float* s1, float* ema,
+                              const B2YOptTile* tiles, int n_tiles, const B2YOptStep* hp, void* stream) {
+    if (n_tiles == 0) return B2Y_OK;
+    auto st = static_cast<cudaStream_t>(stream);
+    if (ema != nullptr)
+        opt_grouped_kernel<ADAM, true><<<n_tiles, OPT_THREADS, 0, st>>>(param, grad, s0, s1, ema, tiles, *hp);
+    else
+        opt_grouped_kernel<ADAM, false><<<n_tiles, OPT_THREADS, 0, st>>>(param, grad, s0, s1, nullptr, tiles, *hp);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_sgd_grouped(float* param, const float* grad, float* momentum_buf, float* ema,
+                               const B2YOptTile* tiles_dev, int n_tiles, const B2YOptStep* hp, void* stream) {
+    const void* bufs[] = {param, grad, momentum_buf};
+    if (!opt_args_ok(bufs, 3, tiles_dev, n_tiles, hp) || (reinterpret_cast<uintptr_t>(ema) & 15) != 0)
+        return B2Y_ERR_INVALID;
+    return opt_grouped_launch<false>(param, grad, momentum_buf, nullptr, ema, tiles_dev, n_tiles, hp, stream);
+}
+
+extern "C" int b2y_adam_grouped(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* ema,
+                                const B2YOptTile* tiles_dev, int n_tiles, const B2YOptStep* hp, void* stream) {
+    const void* bufs[] = {param, grad, exp_avg, exp_avg_sq};
+    if (!opt_args_ok(bufs, 4, tiles_dev, n_tiles, hp) || (reinterpret_cast<uintptr_t>(ema) & 15) != 0)
+        return B2Y_ERR_INVALID;
+    return opt_grouped_launch<true>(param, grad, exp_avg, exp_avg_sq, ema, tiles_dev, n_tiles, hp, stream);
 }
 
 // Network-slimming sparsity term of the BatchNorm scales (prune_utils.py:133-138, BNOptimizer.updateBN, called between
