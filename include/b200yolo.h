@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define B2Y_ABI_VERSION 2
+#define B2Y_ABI_VERSION 3
 
 /* status codes */
 #define B2Y_OK 0
@@ -302,18 +302,6 @@ int b2y_maxpool_bwd(const void* x, long long x_pitch, const void* dy, long long 
 /* weight gradient of the stem (in_c <= 4): x fp32 NCHW, dz fp16 NHWC -> dw OIHW fp32 (+= scale * ...) */
 int b2y_stem_conv_bwd_weight(const b2y_conv_desc* d, const float* x_nchw, const void* dz, float* dw_oihw,
                              float scale, int grad_dtype, void* stream);
-/* SGD + Nesterov momentum + weight decay over a flat fp32 buffer (train.py:135-144), grads pre-scaled by
- * grad_scale (1/world_size after the NCCL sum) */
-int b2y_sgd_nesterov(float* param, const float* grad, float* momentum_buf, long long n, float lr, float momentum,
-                     float weight_decay, float grad_scale, int first_step, void* stream);
-/* the same step with the model EMA (utils/torch_utils.py:171-183: ema = d*ema + (1-d)*w) updated in the same pass */
-int b2y_sgd_nesterov_ema(float* param, const float* grad, float* momentum_buf, float* ema, long long n, float lr,
-                         float momentum, float weight_decay, float grad_scale, int first_step, float ema_decay,
-                         void* stream);
-/* BatchNorm-scale L1 sparsity of network slimming (prune_utils.py:133-138 BNOptimizer.updateBN, train.py:444-445):
- * grad[off + i] += coeff * sign(param[off + i]) for every (off, len) pair of ranges_dev (int64 [n_ranges][2]) */
-int b2y_l1_subgrad_ranges(float* grad, const float* param, const long long* ranges_dev, int n_ranges, float coeff,
-                          void* stream);
 
 /* ---- grouped optimiser steps over the flat buffers (train.py:120-150 parameter groups, :356-365 burn-in) ----
  * One CTA per tile of a device-resident tile table.  A tile is a run of elements of ONE parameter tensor, so its group
@@ -340,9 +328,10 @@ typedef struct {
     float ema_decay;  /* ModelEMA d of this update, used when `ema` is not NULL */
     int first_step;   /* SGD: the momentum buffer does not exist yet (torch: buf = grad) */
 } B2YOptStep;
-/* Nesterov SGD per group (torch.optim.SGD, nesterov=True, dampening=0); the per-element arithmetic is that of
- * b2y_sgd_nesterov.  `ema` (optional): ema = d*ema + (1-d)*p_new (utils/torch_utils.py:171-183).  `hp` is read on the
- * host and passed to the kernel by value. */
+/* Nesterov SGD per group (torch.optim.SGD, nesterov=True, dampening=0, train.py:135-144), gradients scaled by
+ * grad_scale:  g = grad*grad_scale + wd*p ; buf = first_step ? g : mu*buf + g ; p -= lr * (g + mu*buf).
+ * `ema` (optional): ema = d*ema + (1-d)*p_new (utils/torch_utils.py:171-183).  `hp` is read on the host and passed to
+ * the kernel by value. */
 int b2y_sgd_grouped(float* param, const float* grad, float* momentum_buf, float* ema, const B2YOptTile* tiles_dev,
                     int n_tiles, const B2YOptStep* hp, void* stream);
 /* Adam per group (torch.optim.Adam, amsgrad=False, maximize=False, L2 weight decay); same tiles, EMA and L1 terms */

@@ -1,6 +1,6 @@
 """GPU: the grouped optimiser over FlatDataParallel's flat buffers (b200yolo/optim.py, csrc/train.cu opt_grouped_kernel)
 against dp.step and against torch.optim built by train.py's code (train.py:120-144, burn-in :356-365, LambdaLR :201).
-Gate: rtol 1e-5 / atol 1e-6 (the gate of tests/test_gpu_train_kernels.py::test_sgd_nesterov_matches_torch); each test
+Gate: rtol 1e-5 / atol 1e-6 (the gate of tests/test_gpu_train_kernels.py::test_sgd_grouped_matches_torch); each test
 prints its largest observed error."""
 import os
 import socket
@@ -94,6 +94,32 @@ def test_flat_sgd_bit_identical_to_dp_step():
     assert torch.equal(a.flat_mom, b.flat_mom)
     assert torch.equal(a.ema_param, b.ema_param)
     assert torch.equal(a.ema_buf, b.ema_buf)
+
+
+def test_flat_sgd_continues_the_momentum_of_dp_step():
+    """One dp.step() and then two steps of make_optimizer's FlatSGD (uniform hyper-parameters) on the same dp: the
+    FlatSGD continues the momentum dp.step left in flat_mom, bit for bit as three dp.step() calls."""
+    from b200yolo.optim import make_optimizer
+    from b200yolo.parallel import FlatDataParallel
+    dps = [FlatDataParallel(_model("yolov3-tiny")) for _ in range(2)]
+    hyp = dict(HYP, lr0=0.01)
+    gen = torch.Generator().manual_seed(9)
+    for i in range(3):
+        g = (torch.randn(dps[0].flat_grad.numel(), generator=gen) * 1e-2).cuda()
+        for dp in dps:
+            dp.flat_grad.copy_(g)
+        dps[0].step(lr=hyp['lr0'], momentum=hyp['momentum'], weight_decay=hyp['weight_decay'])
+        if i == 0:
+            dps[1].step(lr=hyp['lr0'], momentum=hyp['momentum'], weight_decay=hyp['weight_decay'])
+            opt = make_optimizer(dps[1], hyp)
+        else:
+            opt.step()
+    torch.cuda.synchronize()
+    a, b = dps
+    print("\n[dp.step then FlatSGD vs dp.step] max |diff| param %.3g mom %.3g"
+          % (float((a.flat_param - b.flat_param).abs().max()), float((a.flat_mom - b.flat_mom).abs().max())))
+    assert torch.equal(a.flat_param, b.flat_param)
+    assert torch.equal(a.flat_mom, b.flat_mom)
 
 
 def test_flat_sgd_burn_in_and_lambda_lr_match_torch_sgd():

@@ -238,8 +238,24 @@ def test_multi_tensor_pack_and_unpack_bit_exact(case):
         assert torch.equal(dst, ref_u), "unpacked weight gradient"
 
 
-def test_sgd_nesterov_matches_torch():
-    ops = _ops()
+def _sgd_grouped(p, g, buf, tiles, lr, momentum, weight_decay, grad_scale=1.0, first_step=False, ema=None,
+                 ema_decay=0.0, l1_coeff=0.0):
+    """One ops.sgd_grouped launch with a single parameter group; `tiles` lists (start, length, flags)."""
+    from b200yolo import lib
+    hp = lib.OptStep()
+    hp.group[0].lr, hp.group[0].momentum, hp.group[0].weight_decay = lr, momentum, weight_decay
+    hp.grad_scale, hp.l1_coeff, hp.ema_decay, hp.first_step = grad_scale, l1_coeff, ema_decay, int(first_step)
+    table = torch.tensor([(s, n | (f << 32)) for s, n, f in tiles], dtype=torch.int64, device="cuda")
+    _ops().sgd_grouped(p, g, buf, table, hp, ema=ema)
+
+
+def _whole(n):
+    """Tiles of at most OPT_TILE elements over one tensor of n elements."""
+    from b200yolo import lib
+    return [(s, min(lib.OPT_TILE, n - s), 0) for s in range(0, n, lib.OPT_TILE)]
+
+
+def test_sgd_grouped_matches_torch():
     g = torch.Generator().manual_seed(4)
     p0 = torch.randn(10007, generator=g)
     pt = torch.nn.Parameter(p0.clone())
@@ -249,7 +265,8 @@ def test_sgd_nesterov_matches_torch():
         gr = torch.randn(10007, generator=g)
         pt.grad = gr.clone()
         opt.step()
-        ops.sgd_nesterov(pc, (gr * 4).cuda(), buf, 0.01, 0.937, 5e-4, grad_scale=0.25, first_step=(step == 0))
+        _sgd_grouped(pc, (gr * 4).cuda(), buf, _whole(10007), 0.01, 0.937, 5e-4, grad_scale=0.25,
+                     first_step=(step == 0))
     np.testing.assert_allclose(pc.cpu().numpy(), pt.detach().numpy(), rtol=1e-5, atol=1e-6)
 
 
@@ -359,10 +376,9 @@ def test_data_movement_backward_kernels(gdt):
     assert torch.equal(raw[..., :255].cpu(), want) and float(raw[..., 255].abs().max()) == 0.0
 
 
-def test_fused_sgd_ema_matches_torch_and_model_ema():
+def test_sgd_grouped_ema_matches_torch_and_model_ema():
     """SURVEY 8(f3): SGD-Nesterov + ModelEMA (utils/torch_utils.py:171-183) in one pass over the flat buffer."""
     import math
-    ops = _ops()
     g = torch.Generator().manual_seed(8)
     n = 20011
     p0 = torch.randn(n, generator=g)
@@ -376,27 +392,30 @@ def test_fused_sgd_ema_matches_torch_and_model_ema():
         opt.step()
         d = 0.9999 * (1 - math.exp(-step / 2000))
         ema_ref.mul_(d).add_(pt.detach(), alpha=1 - d)
-        ops.sgd_nesterov(pc, gr.cuda(), buf, 0.01, 0.937, 5e-4, first_step=(step == 1), ema=ema, ema_decay=d)
+        _sgd_grouped(pc, gr.cuda(), buf, _whole(n), 0.01, 0.937, 5e-4, first_step=(step == 1), ema=ema, ema_decay=d)
     np.testing.assert_allclose(pc.cpu().numpy(), pt.detach().numpy(), rtol=1e-5, atol=1e-6)
     np.testing.assert_allclose(ema.cpu().numpy(), ema_ref.numpy(), rtol=1e-5, atol=1e-6)
 
 
-def test_bn_l1_sparsity_matches_update_bn():
-    """SURVEY 8(f3): BNOptimizer.updateBN (prune_utils.py:133-138, train.py:444-445) as one launch over a range table of
-    the flat buffers, and through FlatDataParallel.set_bn_sparsity + step() on the real yolov3-tiny module tree."""
-    ops = _ops()
+def test_bn_l1_tiles_match_update_bn():
+    """SURVEY 8(f3): BNOptimizer.updateBN (prune_utils.py:133-138, train.py:444-445) on the L1-flagged tiles of the
+    grouped optimiser, and through FlatDataParallel.set_bn_sparsity + step() on the real yolov3-tiny module tree."""
+    from b200yolo import lib
     g = torch.Generator().manual_seed(3)
     n = 5000
     p = torch.randn(n, generator=g)
     p[::17] = 0.0                                           # torch.sign(0) == 0
     gr = torch.randn(n, generator=g)
-    ranges = torch.tensor([[0, 32], [100, 1000], [4093, 907], [2000, 1]], dtype=torch.int64)
+    ranges = [(0, 32), (100, 1000), (4093, 907), (2000, 1)]
     want = gr.clone()
-    for off, ln in ranges.tolist():
+    for off, ln in ranges:
         want[off:off + ln] += 0.01 * torch.sign(p[off:off + ln])
-    gc = gr.clone().cuda()
-    ops.l1_subgrad_ranges(gc, p.cuda(), ranges.cuda(), 0.01)
-    assert torch.equal(gc.cpu(), want)
+    # the L1 ranges and the gaps between them as tiles; a first step without momentum or weight decay leaves g + L1 in buf
+    cuts = sorted({0, n} | {b for off, ln in ranges for b in (off, off + ln)})
+    tiles = [(a, b - a, lib.OPT_TILE_L1 if (a, b - a) in ranges else 0) for a, b in zip(cuts, cuts[1:])]
+    buf = torch.full((n,), float("nan"), device="cuda")
+    _sgd_grouped(p.cuda(), gr.cuda(), buf, tiles, 0.01, 0.0, 0.0, first_step=True, l1_coeff=0.01)
+    assert torch.equal(buf.cpu(), want)
 
     from b200yolo.parallel import FlatDataParallel
     from helpers import build_model

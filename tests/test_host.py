@@ -33,7 +33,7 @@ def test_c_abi_exports_every_declared_symbol():
     assert not binding.MISSING
     unbound = [n for n in declared if n not in binding.EXPORTS and n != "b2y_set_last_cuda_error"]
     assert not unbound, "declared in the header but not bound in b200yolo/lib.py: %s" % unbound
-    assert lib.b2y_abi_version() == 2
+    assert lib.b2y_abi_version() == 3
     assert binding.raw().b2y_strerror(-3).decode().startswith("unsupported")
 
 

@@ -91,9 +91,9 @@ def test_flat_data_parallel_gloo():
 
 
 def test_bn_sparsity_range_table_points_at_the_bn_scales():
-    """FlatDataParallel.set_bn_sparsity (BNOptimizer.updateBN, prune_utils.py:133-138): the (offset, length) rows handed to
-    b2y_l1_subgrad_ranges address exactly the BatchNorm scale vectors of the listed layers inside the flat buffers (the
-    kernel itself is checked on the GPU, tests/test_gpu_train_kernels.py)."""
+    """FlatDataParallel.set_bn_sparsity (BNOptimizer.updateBN, prune_utils.py:133-138): the host (offset, length) rows
+    from which the optimiser's tile table flags the L1 term address exactly the BatchNorm scale vectors of the listed
+    layers inside the flat buffers (the kernel itself is checked on the GPU, tests/test_gpu_train_kernels.py)."""
     from b200yolo.parallel import FlatDataParallel
     m = _real_model()
     dp = FlatDataParallel(m)

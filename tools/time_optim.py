@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Cost of one optimiser step over yolov4's flat buffers (FlatDataParallel, 64.4 M parameters), timed with CUDA events:
-  dp.step        -- FlatDataParallel.step, two launches of the single-group Nesterov kernel
+  dp.step        -- FlatDataParallel.step: FlatSGD over two groups (decayed conv weights, the rest), one launch
   FlatSGD        -- b200yolo.optim, train.py's three groups, one launch
   FlatAdam       -- the same for Adam
   torch SGD/Adam -- torch.optim (foreach, its default on CUDA) over the same parameter views, train.py's groups

@@ -127,8 +127,6 @@ _PROTOS = {
     "b2y_upsample_nearest_bwd": (i32, [vp, ll, vp, ll, i32, i32, i32, i32, i32, i32, vp]),
     "b2y_maxpool_bwd": (i32, [vp, ll, vp, ll, vp, ll, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b2y_stem_conv_bwd_weight": (i32, [C.POINTER(ConvDesc), vp, vp, vp, f32, i32, vp]),
-    "b2y_sgd_nesterov": (i32, [vp, vp, vp, ll, f32, f32, f32, f32, i32, vp]),
-    "b2y_sgd_nesterov_ema": (i32, [vp, vp, vp, vp, ll, f32, f32, f32, f32, i32, f32, vp]),
     "b2y_bn_train_fwd": (i32, [vp, ll, vp, vp, ll, vp, vp, f32, f32, vp, vp, vp, vp, ll, vp, ll, ll, i32, i32, f32, vp]),
     "b2y_bn_train_bwd_reduce": (i32, [vp, ll, vp, ll, vp, vp, vp, ll, i32, i32, f32, i32, vp]),
     "b2y_bn_train_bwd_apply": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, ll, ll, i32, i32, f32, i32, vp, vp, vp, vp, f32,
@@ -144,7 +142,6 @@ _PROTOS = {
     "b2y_layout_tile_i": (i32, [i32]),
     "b2y_pack_conv_weights_multi": (i32, [vp, i32, i32, vp]),
     "b2y_unpack_wgrad_multi": (i32, [vp, i32, i32, vp]),
-    "b2y_l1_subgrad_ranges": (i32, [vp, vp, vp, i32, f32, vp]),
     "b2y_sgd_grouped": (i32, [vp, vp, vp, vp, vp, i32, C.POINTER(OptStep), vp]),
     "b2y_adam_grouped": (i32, [vp, vp, vp, vp, vp, vp, i32, C.POINTER(OptStep), vp]),
     "b2y_kd_soft_rows": (i32, [vp, vp, ll, i32, i32, i32, f32, f32, vp, vp, vp]),

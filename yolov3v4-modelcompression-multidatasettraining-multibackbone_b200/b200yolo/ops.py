@@ -466,17 +466,6 @@ def se_bwd(x, dy, w1, w2, ws, dx, accumulate=False, dw1=None, dw2=None, grad_sca
     return dx, dw1, dw2
 
 
-def sgd_nesterov(param, grad, buf, lr, momentum, weight_decay, grad_scale=1.0, first_step=False, ema=None,
-                 ema_decay=0.0):
-    if ema is not None:
-        call("b2y_sgd_nesterov_ema", ptr(param), ptr(grad), ptr(buf), ptr(ema), param.numel(), float(lr),
-             float(momentum), float(weight_decay), float(grad_scale), 1 if first_step else 0, float(ema_decay),
-             stream_ptr())
-        return
-    call("b2y_sgd_nesterov", ptr(param), ptr(grad), ptr(buf), param.numel(), float(lr), float(momentum),
-         float(weight_decay), float(grad_scale), 1 if first_step else 0, stream_ptr())
-
-
 def _opt_check(tiles, *flat):
     _require_cuda(tiles, *flat)
     assert tiles.dtype == torch.int64 and tiles.dim() == 2 and tiles.shape[1] == 2 and tiles.is_contiguous()
@@ -499,14 +488,6 @@ def adam_grouped(param, grad, exp_avg, exp_avg_sq, tiles, hp, ema=None):
     _opt_check(tiles, param, grad, exp_avg, exp_avg_sq, ema)
     call("b2y_adam_grouped", ptr(param), ptr(grad), ptr(exp_avg), ptr(exp_avg_sq), ptr(ema), ptr(tiles),
          int(tiles.shape[0]), C.byref(hp), stream_ptr())
-
-
-def l1_subgrad_ranges(grad, param, ranges, coeff):
-    """grad[off:off+len] += coeff * sign(param[off:off+len]) for each row (off, len) of the int64 device table `ranges`
-    (BNOptimizer.updateBN, prune_utils.py:133-138)."""
-    _require_cuda(grad, param, ranges)
-    assert ranges.dtype == torch.int64 and ranges.dim() == 2 and ranges.shape[1] == 2 and ranges.is_contiguous()
-    call("b2y_l1_subgrad_ranges", ptr(grad), ptr(param), ptr(ranges), int(ranges.shape[0]), float(coeff), stream_ptr())
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -10,18 +10,20 @@ the burn-in loop, LambdaLR and MultiStepLR work on them unchanged.  step() reads
 host, packs them into a struct passed to the kernel by value, and launches csrc/train.cu opt_grouped_kernel once over a
 device-resident tile table (built on the first step, rebuilt only when the groups or the BatchNorm-L1 set change).  The
 gradient scale 1/world, the BatchNorm-L1 term (FlatDataParallel.set_bn_sparsity) and the model EMA
-(FlatDataParallel.enable_ema) are applied in the same pass, as FlatDataParallel.step does.
+(FlatDataParallel.enable_ema) are applied in the same pass.  FlatDataParallel.step is a FlatSGD step over two groups.
 
 Per-parameter state ('momentum_buffer', 'exp_avg', 'exp_avg_sq') are views of flat state buffers in the parameter
 layout; state_dict() returns copies that load into a torch.optim.SGD / Adam built by train.py's code, and
 load_state_dict() copies a torch optimiser's state into the flat views.  FlatSGD keeps its momentum in
-FlatDataParallel.flat_mom, the buffer FlatDataParallel.step uses: drive a FlatDataParallel with one of the two.
+FlatDataParallel.flat_mom, and whether that holds one in FlatDataParallel.has_momentum, so FlatDataParallel.step and
+every FlatSGD over the same FlatDataParallel continue one momentum.
 """
 from collections import defaultdict
 
 import torch
 
 from . import lib, ops
+from .parallel import _is_decay_param
 
 
 def train_param_groups(dp, quantized=-1):
@@ -33,10 +35,10 @@ def train_param_groups(dp, quantized=-1):
     for k, v in dict(dp.module.named_parameters()).items():
         if id(v) not in flat:
             raise ValueError("parameter %s is not in the FlatDataParallel buffers (requires_grad=False?)" % k)
-        if '.bias' in k:
-            pg2.append(v)
-        elif 'Conv2d.weight' in k:
+        if _is_decay_param(k):
             pg1.append(v)
+        elif '.bias' in k:
+            pg2.append(v)
         elif 'scale' in k and quantized == 2:
             pg3.append(v)
         else:
@@ -60,23 +62,21 @@ class _FlatOptimizer:
         """int64 [n][2] device table of B2YOptTile rows {start, len | flags << 32}: tiles of at most OPT_TILE elements
         inside one parameter tensor, cut at multiples of OPT_TILE so that every tile but a tensor's first starts
         16-byte aligned."""
-        dp = self.dp
-        l1 = getattr(dp, '_l1', None)
+        l1 = self.dp._l1
         if self._tiles is not None and self._tiles_l1 is l1:
             return self._tiles
-        self._tiles = build_tile_table(dp, self.param_groups)
+        self._tiles = build_tile_table(self.dp, self.param_groups)
         self._tiles_l1 = l1
         return self._tiles
 
     def _step_common(self):
-        """The fields of lib.OptStep that do not depend on the algorithm; advances the EMA counter like dp.step."""
+        """The fields of lib.OptStep that do not depend on the algorithm; advances the EMA counter."""
         dp = self.dp
         hp = lib.OptStep()
         gs = 1.0 / float(dp.world)
         hp.grad_scale = gs
-        l1 = getattr(dp, '_l1', None)
-        if l1 is not None:
-            hp.l1_coeff = l1[1] / gs          # updateBN runs on the averaged gradient, the kernel scales after it
+        if dp._l1 is not None:
+            hp.l1_coeff = dp._l1[1] / gs          # updateBN runs on the averaged gradient, the kernel scales after it
         ema = getattr(dp, 'ema_param', None)
         d = 0.0
         if ema is not None:
@@ -146,10 +146,7 @@ def build_tile_table(dp, param_groups):
             owner[id(p)] = gi
     if len(owner) != len(dp.params) or any(id(p) not in owner for p in dp.params):
         raise ValueError("the parameter groups must hold exactly the FlatDataParallel's parameters")
-    l1 = getattr(dp, '_l1', None)
-    l1_rows = {}
-    if l1 is not None:
-        l1_rows = {off: ln for off, ln in l1[0].cpu().tolist()}
+    l1_rows = dict(dp._l1[0].tolist()) if dp._l1 is not None else {}
     T = lib.OPT_TILE
     rows, off = [], 0
     for p in dp.params:
@@ -176,7 +173,7 @@ class FlatSGD(_FlatOptimizer, torch.optim.SGD):
 
     def __init__(self, dp, params, lr, momentum=0.0, dampening=0, weight_decay=0, nesterov=True):
         self._flat_init(dp)
-        self._has_buf = False
+        self._bound = False
         torch.optim.SGD.__init__(self, params, lr=lr, momentum=momentum, dampening=dampening,
                                  weight_decay=weight_decay, nesterov=nesterov)
 
@@ -187,10 +184,10 @@ class FlatSGD(_FlatOptimizer, torch.optim.SGD):
 
     def _launch(self, tiles, hp, ema):
         dp = self.dp
-        hp.first_step = 0 if self._has_buf else 1
+        hp.first_step = 0 if dp.has_momentum else 1
         ops.sgd_grouped(dp.flat_param, dp.flat_grad, dp.flat_mom, tiles, hp, ema=ema)
-        if not self._has_buf:
-            self._has_buf = True
+        dp.has_momentum = True
+        if not self._bound:
             self._bind_state()
 
     def _bind_state(self):
@@ -198,15 +195,17 @@ class FlatSGD(_FlatOptimizer, torch.optim.SGD):
         for p in self.dp.params:
             self.state[p]['momentum_buffer'] = self.dp.flat_mom[off:off + p.numel()].view_as(p)
             off += p.numel()
+        self._bound = True
 
     def _reset_state(self):
-        self._has_buf = False
+        self.dp.has_momentum = False
+        self._bound = False
 
     def _load_state(self, per_param):
         if any(s.get('momentum_buffer') is None for s in per_param):
             raise ValueError("optimizer state without a momentum_buffer")
         self._copy_flat(self.dp.flat_mom, [s['momentum_buffer'] for s in per_param])
-        self._has_buf = True
+        self.dp.has_momentum = True
         self._bind_state()
 
 

@@ -6,7 +6,7 @@ DDP's bucketed all-reduce (SUM, then / world) overlapped with backward, rank-0 b
 
 Here all parameters live in one flat fp32 buffer and all gradients in another (the training plan writes weight
 gradients straight into their slice), so the exchange step is exactly one `all_reduce(flat_grad, SUM)` over
-NCCL/NVLink and the 1/world factor is folded into the fused SGD-Nesterov kernel.  Semantics kept from DDP:
+NCCL/NVLink and the 1/world factor is folded into the fused optimiser kernel.  Semantics kept from DDP:
   * reduced gradient = mean over ranks of the per-rank gradients (each rank's loss uses its own shard),
   * BatchNorm statistics are per replica; running buffers follow rank 0 (broadcast before each forward),
   * parameters are broadcast from rank 0 at construction.
@@ -62,7 +62,9 @@ class FlatDataParallel:
                 self.flat_buf[off:off + n].copy_(b.detach().reshape(-1).float())
                 b.data = self.flat_buf[off:off + n].view_as(b)
                 off += n
-        self.steps = 0
+        self.has_momentum = False        # flat_mom holds a momentum buffer: set by the SGD step or a loaded state
+        self._l1 = None
+        self._sgd = None
         if self.world > 1:
             dist.broadcast(self.flat_param, src=0, group=self.pg)           # N2: parameters from rank 0
             self._broadcast_buffers()
@@ -135,9 +137,9 @@ class FlatDataParallel:
 
     def set_bn_sparsity(self, prune_idx, s):
         """Network-slimming sparsity training (train.py -sr --s, :444-445; prune_utils.py:133-138 BNOptimizer.updateBN):
-        from now on step() adds s * sign(gamma) to the (averaged) gradient of the BatchNorm scale of every
-        module_list[idx] in prune_idx -- one launch over a range table of the flat buffers, before the fused optimiser.
-        s = 0 or an empty list switches it off."""
+        from now on the optimiser step adds s * sign(gamma) to the (averaged) gradient of the BatchNorm scale of every
+        module_list[idx] in prune_idx, in the same launch as the update.  Kept on the host: an int64 CPU table of the
+        (offset, length) rows of those scales in the flat buffers, and s.  s = 0 or an empty list switches it off."""
         offsets, off = {}, 0
         for p in self.params:
             offsets[id(p)] = off
@@ -146,34 +148,17 @@ class FlatDataParallel:
         for idx in (prune_idx if s else []):
             bn = self.module.module_list[idx][1]
             rows.append((offsets[id(bn.weight)], bn.weight.numel()))
-        self._l1 = (torch.tensor(rows, dtype=torch.int64, device=self.flat_param.device).reshape(-1, 2).contiguous(),
-                    float(s)) if rows else None
+        self._l1 = (torch.tensor(rows, dtype=torch.int64).reshape(-1, 2), float(s)) if rows else None
 
     def step(self, lr, momentum=0.937, weight_decay=0.000484, nesterov=True):
-        """Fused SGD-Nesterov (+ EMA when enabled) over the flat buffers (two launches: decayed conv weights, the rest)."""
-        from . import ops
+        """Nesterov SGD with one lr and momentum, weight decay on the 'Conv2d.weight' parameters only: a
+        b200yolo.optim.FlatSGD step over two groups, those parameters and the rest (+ BatchNorm-L1 and EMA when enabled),
+        in one launch."""
         assert nesterov, "the fused kernel implements the reference's nesterov=True configuration"
-        first = self.steps == 0
-        gs = 1.0 / float(self.world)
-        nd = self.n_decay
-        ema = getattr(self, 'ema_param', None)
-        d = 0.0
-        if ema is not None:
-            self.ema_updates += 1
-            d = self._ema_decay(self.ema_updates)
-        l1 = getattr(self, '_l1', None)
-        if l1 is not None:
-            # updateBN runs after DDP has averaged the gradients: s * sign(w) is NOT divided by world -> pre-multiply
-            ops.l1_subgrad_ranges(self.flat_grad, self.flat_param, l1[0], l1[1] / gs)
-        if nd:
-            ops.sgd_nesterov(self.flat_param[:nd], self.flat_grad[:nd], self.flat_mom[:nd], lr, momentum, weight_decay,
-                             grad_scale=gs, first_step=first, ema=ema[:nd] if ema is not None else None, ema_decay=d)
-        if nd < self.flat_param.numel():
-            ops.sgd_nesterov(self.flat_param[nd:], self.flat_grad[nd:], self.flat_mom[nd:], lr, momentum, 0.0,
-                             grad_scale=gs, first_step=first, ema=ema[nd:] if ema is not None else None, ema_decay=d)
-        if ema is not None and self.ema_buf is not None:
-            ops.axpby(self.flat_buf, self.ema_buf, 1.0 - d, d)         # running statistics: ema = d*ema + (1-d)*buf
-        self.steps += 1
-        eng = self.module.__dict__.get('_engine')
-        if eng is not None:
-            eng.weights_changed()            # weights changed through the flat buffer: re-pack on the next forward
+        if self._sgd is None:
+            from .optim import FlatSGD
+            nd = sum(map(_is_decay_param, self.names))        # the decayed parameters come first in the flat layout
+            self._sgd = FlatSGD(self, [{'params': self.params[:nd]}, {'params': self.params[nd:]}], lr, momentum)
+        for group, wd in zip(self._sgd.param_groups, (weight_decay, 0.0)):
+            group.update(lr=lr, momentum=momentum, weight_decay=wd)
+        self._sgd.step()

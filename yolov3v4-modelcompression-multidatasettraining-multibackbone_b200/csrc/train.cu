@@ -233,55 +233,6 @@ extern "C" int b2y_bn_act_bwd_reduce(const void* x, long long x_pitch, const voi
 }
 
 // ------------------------------------------------------------------------------------------------
-// SGD with Nesterov momentum (torch.optim.SGD semantics, train.py:135-144):
-//   g = grad*grad_scale + wd*p ; buf = first ? g : mu*buf + g ; p -= lr * (g + mu*buf)
-// ------------------------------------------------------------------------------------------------
-// The per-element arithmetic of the step, shared with the grouped kernel so that equal hyper-parameters give
-// bit-identical results.  `b` is the momentum buffer in (ignored when `first`) and out; returns the new weight.
-__device__ __forceinline__ float sgd_nesterov_elem(float w, float g, float& b, float lr, float mu, float wd, float gs,
-                                                   int first) {
-    const float grad = fmaf(wd, w, g * gs);
-    b = first ? grad : fmaf(mu, b, grad);
-    return w - lr * fmaf(mu, b, grad);
-}
-
-// ModelEMA.update (utils/torch_utils.py:171-183) fused into the optimiser pass: ema = d*ema + (1-d)*w_new
-__device__ __forceinline__ float ema_elem(float e, float wn, float d) { return fmaf(d, e, (1.f - d) * wn); }
-
-__global__ void sgd_nesterov_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf,
-                                    long long n, float lr, float mu, float wd, float gs, int first,
-                                    float* __restrict__ ema, float ema_decay) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-         i += (long long)gridDim.x * blockDim.x) {
-        const float w = p[i];
-        float b = first ? 0.f : buf[i];
-        const float wn = sgd_nesterov_elem(w, g[i], b, lr, mu, wd, gs, first);
-        buf[i] = b;
-        p[i] = wn;
-        if (ema != nullptr) ema[i] = ema_elem(ema[i], wn, ema_decay);
-    }
-}
-
-extern "C" int b2y_sgd_nesterov(float* param, const float* grad, float* momentum_buf, long long n, float lr,
-                                float momentum, float weight_decay, float grad_scale, int first_step, void* stream) {
-    if (!param || !grad || !momentum_buf || n < 0) return B2Y_ERR_INVALID;
-    sgd_nesterov_kernel<<<grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        param, grad, momentum_buf, n, lr, momentum, weight_decay, grad_scale, first_step, nullptr, 0.f);
-    B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
-}
-
-extern "C" int b2y_sgd_nesterov_ema(float* param, const float* grad, float* momentum_buf, float* ema, long long n,
-                                    float lr, float momentum, float weight_decay, float grad_scale, int first_step,
-                                    float ema_decay, void* stream) {
-    if (!param || !grad || !momentum_buf || !ema || n < 0) return B2Y_ERR_INVALID;
-    sgd_nesterov_kernel<<<grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        param, grad, momentum_buf, n, lr, momentum, weight_decay, grad_scale, first_step, ema, ema_decay);
-    B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
 // Grouped optimiser steps (train.py:120-150 parameter groups, per-group burn-in at :356-365).  One CTA per tile of the
 // table; a tile lies inside one parameter tensor, so its group's hyper-parameters are uniform.  Its unaligned head and
 // tail (< 4 elements each) are scalar, the rest goes in 16-byte vectors, OPT_VEC of them per thread loaded before any is
@@ -291,7 +242,7 @@ extern "C" int b2y_sgd_nesterov_ema(float* param, const float* grad, float* mome
 // Order of operations per element (g is the NCCL sum of the per-rank gradients):
 //   1. g += (s / gs) * sign(w)  on L1 tiles -- BNOptimizer.updateBN on the averaged gradient (prune_utils.py:133-138)
 //   2. g  = g * gs              -- DDP's mean over ranks
-//   3. SGD:  g = g + wd*w ; buf = first ? g : mu*buf + g ; w -= lr * (g + mu*buf)          (sgd_nesterov_elem)
+//   3. SGD:  g = g + wd*w ; buf = first ? g : mu*buf + g ; w -= lr * (g + mu*buf)
 //      Adam: g = g + wd*w                                   (grad.add(param, alpha=weight_decay))
 //            m = m + (1-b1)*(g - m)                         (exp_avg.lerp_(grad, 1-beta1))
 //            v = v*b2 + (1-b2)*g*g                          (exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1-beta2))
@@ -306,13 +257,19 @@ template <bool ADAM>
 __device__ __forceinline__ float opt_elem(float w, float g, float& s0, float& s1, const B2YOptGroup& G,
                                           const B2YOptStep& hp, bool l1) {
     if (l1) g = fmaf(hp.l1_coeff, (float)((w > 0.f) - (w < 0.f)), g);       // torch.sign: 0 at 0
-    if (!ADAM) return sgd_nesterov_elem(w, g, s0, G.lr, G.momentum, G.weight_decay, hp.grad_scale, hp.first_step);
     const float gr = fmaf(G.weight_decay, w, g * hp.grad_scale);
+    if (!ADAM) {                                                            // s0 = buf (ignored on the first step)
+        s0 = hp.first_step ? gr : fmaf(G.momentum, s0, gr);
+        return w - G.lr * fmaf(G.momentum, s0, gr);
+    }
     s0 = fmaf(G.one_minus_beta1, gr - s0, s0);
     s1 = fmaf(G.one_minus_beta2, gr * gr, s1 * G.beta2);
     const float denom = sqrtf(s1) / G.bc2_sqrt + G.eps;
     return w - G.step_size * (s0 / denom);
 }
+
+// ModelEMA.update (utils/torch_utils.py:171-183) fused into the optimiser pass: ema = d*ema + (1-d)*w_new
+__device__ __forceinline__ float ema_elem(float e, float wn, float d) { return fmaf(d, e, (1.f - d) * wn); }
 
 template <bool ADAM, bool EMA>
 __global__ void __launch_bounds__(OPT_THREADS)
@@ -413,28 +370,6 @@ extern "C" int b2y_adam_grouped(float* param, const float* grad, float* exp_avg,
     if (!opt_args_ok(bufs, 4, tiles_dev, n_tiles, hp) || (reinterpret_cast<uintptr_t>(ema) & 15) != 0)
         return B2Y_ERR_INVALID;
     return opt_grouped_launch<true>(param, grad, exp_avg, exp_avg_sq, ema, tiles_dev, n_tiles, hp, stream);
-}
-
-// Network-slimming sparsity term of the BatchNorm scales (prune_utils.py:133-138, BNOptimizer.updateBN, called between
-// backward and optimizer.step at train.py:444-445): grad += coeff * sign(w) on a table of [offset, length] ranges of
-// the flat buffers.  One CTA per range (a BatchNorm layer: 32 .. 1024 scales).
-__global__ void l1_subgrad_ranges_kernel(float* __restrict__ g, const float* __restrict__ p,
-                                         const long long* __restrict__ ranges, float coeff) {
-    const long long off = ranges[2 * blockIdx.x], len = ranges[2 * blockIdx.x + 1];
-    for (long long i = threadIdx.x; i < len; i += blockDim.x) {
-        const float w = p[off + i];
-        const float sgn = (float)((w > 0.f) - (w < 0.f));           // torch.sign: 0 at 0
-        g[off + i] = fmaf(coeff, sgn, g[off + i]);
-    }
-}
-
-extern "C" int b2y_l1_subgrad_ranges(float* grad, const float* param, const long long* ranges_dev, int n_ranges,
-                                     float coeff, void* stream) {
-    if (!grad || !param || n_ranges < 0 || (n_ranges > 0 && !ranges_dev)) return B2Y_ERR_INVALID;
-    if (n_ranges == 0) return B2Y_OK;
-    l1_subgrad_ranges_kernel<<<n_ranges, 128, 0, static_cast<cudaStream_t>(stream)>>>(grad, param, ranges_dev, coeff);
-    B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
