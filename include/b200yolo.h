@@ -198,9 +198,10 @@ int b2y_yolo_loss(const float* p, const float* targets, int nt, const float* anc
                   int ny, int nx, float iou_t, float gr, float cls_pw, float obj_pw, float w_box, float w_obj,
                   float w_cls, float fl_gamma, float* out4, float* dp, void* workspace, void* stream);
 /* build_targets only: writes up to na*nt matches in reference order (anchor-major, target-minor);
- *   idx int64 [4][na*nt] rows (b, a, gj, gi), tbox fp32 [na*nt][4], tcls int64 [na*nt], count int32[1] */
-int b2y_build_targets(const float* targets, int nt, const float* anchors, int na, int ny, int nx, float iou_t,
-                      long long* idx, float* tbox, long long* tcls, int* count, void* stream);
+ *   idx int64 [4][na*nt] rows (b, a, gj, gi), tbox fp32 [na*nt][4], tcls int64 [na*nt], count int32[1].
+ *   Candidates with b outside [0, batch) or a cell off the ny x nx grid are dropped, as b2y_yolo_loss drops them. */
+int b2y_build_targets(const float* targets, int nt, const float* anchors, int batch, int na, int ny, int nx,
+                      float iou_t, long long* idx, float* tbox, long long* tcls, int* count, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Quantisation (power-of-two scale fake-quant, BN fold, INT8 conv):

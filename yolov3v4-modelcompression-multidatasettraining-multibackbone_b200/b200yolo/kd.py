@@ -58,7 +58,7 @@ class _KD(torch.autograd.Function):
                 scales.append(k)
                 s, t, ds = _soft(ps, pt, 4, k, layer_acc[i:i + 1], want)
                 B, na, ny, nx, no = s.shape
-                idx, tbox, _ = ops.build_targets_layer(targets, av, ny, nx, iou_t)
+                idx, tbox, _ = ops.build_targets_layer(targets, av, B, ny, nx, iou_t)
                 nb = int(idx.shape[1])
                 reg_nb += nb
                 if nb:

@@ -104,7 +104,7 @@ _PROTOS = {
     "b2y_yolo_loss_workspace_bytes": (sz, [i32, i32, i32, i32, i32]),
     "b2y_yolo_loss": (i32, [vp, vp, i32, vp, i32, i32, i32, i32, i32, f32, f32, f32, f32, f32, f32, f32, f32, vp,
                             vp, vp, vp]),
-    "b2y_build_targets": (i32, [vp, i32, vp, i32, i32, i32, f32, vp, vp, vp, vp, vp]),
+    "b2y_build_targets": (i32, [vp, i32, vp, i32, i32, i32, i32, f32, vp, vp, vp, vp, vp]),
     "b2y_qconv2d_fwd": (i32, [C.POINTER(QConvDesc), vp, vp, vp, vp, vp]),
     "b2y_qconv2d_shortcut_fwd": (i32, [C.POINTER(QConvDesc), vp, vp, vp, vp, ll, f32, f32, f32, f32, f32, f32, vp, vp]),
     "b2y_fakequant_f32": (i32, [vp, vp, ll, f32, f32, f32, vp]),

@@ -276,7 +276,9 @@ def yolo_loss_layer(p, targets, anchor_vec, iou_t, gr, cls_pw, obj_pw, w_box, w_
     return out4, dp
 
 
-def build_targets_layer(targets, anchor_vec, ny, nx, iou_t):
+def build_targets_layer(targets, anchor_vec, batch, ny, nx, iou_t):
+    """One yolo layer of build_targets -> (idx int64 [4, n] = (b, a, gj, gi), tbox fp32 [n, 4], tcls int64 [n]), in the
+    reference's order (anchor-major, target-minor).  Candidates outside the batch or the ny x nx grid are dropped."""
     nt = int(targets.shape[0])
     na = int(anchor_vec.shape[0])
     cap = max(1, na * nt)
@@ -286,8 +288,8 @@ def build_targets_layer(targets, anchor_vec, ny, nx, iou_t):
     tcls = torch.zeros((cap,), dtype=torch.int64, device=dev)
     count = torch.zeros((1,), dtype=torch.int32, device=dev)
     t = targets.contiguous().float() if nt else None
-    call("b2y_build_targets", ptr(t), nt, ptr(anchor_vec), na, ny, nx, float(iou_t), ptr(idx), ptr(tbox), ptr(tcls),
-         ptr(count), stream_ptr())
+    call("b2y_build_targets", ptr(t), nt, ptr(anchor_vec), int(batch), na, ny, nx, float(iou_t), ptr(idx), ptr(tbox),
+         ptr(tcls), ptr(count), stream_ptr())
     n = int(count.item())
     return idx[:, :n], tbox[:n], tcls[:n]
 

@@ -143,22 +143,26 @@ struct Match {
     float tx, ty, tw, th;  // tbox: (frac x, frac y, w, h) in grid units
 };
 
+// A candidate whose image index b lies outside [0, B) or whose cell (gi, gj) lies off the grid (x or y == 1.0 after
+// the .long() truncation, a negative image index) is dropped, by the loss and by build_targets alike: the reference
+// would raise an IndexError at pi[b, a, gj, gi], and writing or reading such a cell here would go out of bounds.
 __device__ __forceinline__ Match match_candidate(const float* __restrict__ targets, const float* __restrict__ anchors,
-                                                 int a, int j, int nx, int ny, float iou_t) {
+                                                 int a, int j, int B, int nx, int ny, float iou_t) {
     Match m;
     const float* t = targets + (long long)j * 6;
     // t = targets * gain, gain = (1,1,nx,ny,nx,ny)  (utils.py:742-743)
     const float gx = t[2] * (float)nx, gy = t[3] * (float)ny;
     const float gw = t[4] * (float)nx, gh = t[5] * (float)ny;
     const float aw = anchors[a * 2], ah = anchors[a * 2 + 1];
-    // wh_iou (utils.py:325-330)
-    const float inter = fminf(aw, gw) * fminf(ah, gh);
-    const float iou = inter / (aw * ah + gw * gh - inter);
-    m.ok = iou > iou_t;
+    // wh_iou (utils.py:325-330): each prod(2) rounded on its own, as torch does.  Contracting aw*ah + gw*gh into one FMA
+    // moves the denominator by an ulp, which flips the `> iou_t` decision of a candidate whose IoU sits at the threshold.
+    const float inter = __fmul_rn(fminf(aw, gw), fminf(ah, gh));
+    const float iou = inter / __fsub_rn(__fadd_rn(__fmul_rn(aw, ah), __fmul_rn(gw, gh)), inter);
     m.b = (int)t[0];  // .long() truncation (utils.py:761,764)
     m.c = (int)t[1];
     m.gi = (int)gx;
     m.gj = (int)gy;
+    m.ok = iou > iou_t && m.b >= 0 && m.b < B && m.gi >= 0 && m.gi < nx && m.gj >= 0 && m.gj < ny;
     m.tx = gx - floorf(gx);
     m.ty = gy - floorf(gy);
     m.tw = gw;
@@ -270,8 +274,8 @@ __global__ void loss_assign_kernel(const float* __restrict__ targets, int nt, co
     int local = 0;
     for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < total; k += gridDim.x * blockDim.x) {
         const int a = k / nt, j = k - a * nt;
-        const Match m = match_candidate(targets, anchors, a, j, nx, ny, iou_t);
-        if (m.ok && m.b >= 0 && m.b < B && m.gi >= 0 && m.gi < nx && m.gj >= 0 && m.gj < ny) {
+        const Match m = match_candidate(targets, anchors, a, j, B, nx, ny, iou_t);
+        if (m.ok) {
             local++;
             const long long cell = (((long long)m.b * na + a) * ny + m.gj) * nx + m.gi;
             atomicMax(winner + cell, k);
@@ -300,8 +304,8 @@ __global__ void loss_match_kernel(const float* __restrict__ p, const float* __re
     const int warps = (gridDim.x * blockDim.x) >> 5;
     for (int k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < total; k += warps) {
         const int a = k / nt, j = k - a * nt;
-        const Match m = match_candidate(targets, anchors, a, j, nx, ny, iou_t);
-        if (!(m.ok && m.b >= 0 && m.b < B && m.gi >= 0 && m.gi < nx && m.gj >= 0 && m.gj < ny)) continue;   // warp-uniform
+        const Match m = match_candidate(targets, anchors, a, j, B, nx, ny, iou_t);
+        if (!m.ok) continue;   // warp-uniform
         const long long cell = (((long long)m.b * na + a) * ny + m.gj) * nx + m.gi;
         const float* ps = p + cell * no;
         if (lane == 0) {
@@ -348,7 +352,7 @@ __global__ void loss_obj_kernel(const float* __restrict__ p, const float* __rest
         float tobj = 0.f;
         if (k >= 0) {
             const int a = k / nt, j = k - a * nt;
-            const Match m = match_candidate(targets, anchors, a, j, nx, ny, iou_t);
+            const Match m = match_candidate(targets, anchors, a, j, B, nx, ny, iou_t);
             const float giou = giou_fwd_bwd(p + cell * no, anchors[a * 2], anchors[a * 2 + 1], m, nullptr);
             tobj = (1.f - gr) + gr * fmaxf(giou, 0.f);  // utils.py:407
         }
@@ -399,7 +403,7 @@ extern "C" int b2y_yolo_loss(const float* p, const float* targets, int nt, const
 // build_targets as a standalone op: ordered (anchor-major, target-minor) compaction in one CTA
 // ------------------------------------------------------------------------------------------------
 __global__ void build_targets_kernel(const float* __restrict__ targets, int nt, const float* __restrict__ anchors,
-                                     int na, int ny, int nx, float iou_t, long long* __restrict__ idx,
+                                     int B, int na, int ny, int nx, float iou_t, long long* __restrict__ idx,
                                      float* __restrict__ tbox, long long* __restrict__ tcls,
                                      int* __restrict__ count) {
     __shared__ int warp_tot[32];
@@ -414,7 +418,7 @@ __global__ void build_targets_kernel(const float* __restrict__ targets, int nt, 
         int a = 0;
         if (k < total) {
             a = k / nt;
-            m = match_candidate(targets, anchors, a, k - a * nt, nx, ny, iou_t);
+            m = match_candidate(targets, anchors, a, k - a * nt, B, nx, ny, iou_t);
         }
         const unsigned bal = __ballot_sync(0xffffffffu, m.ok);
         const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -447,13 +451,13 @@ __global__ void build_targets_kernel(const float* __restrict__ targets, int nt, 
     if (threadIdx.x == 0) *count = base;
 }
 
-extern "C" int b2y_build_targets(const float* targets, int nt, const float* anchors, int na, int ny, int nx,
-                                 float iou_t, long long* idx, float* tbox, long long* tcls, int* count,
+extern "C" int b2y_build_targets(const float* targets, int nt, const float* anchors, int batch, int na, int ny,
+                                 int nx, float iou_t, long long* idx, float* tbox, long long* tcls, int* count,
                                  void* stream) {
-    if (!anchors || !idx || !tbox || !tcls || !count || nt < 0 || na <= 0) return B2Y_ERR_INVALID;
+    if (!anchors || !idx || !tbox || !tcls || !count || nt < 0 || batch <= 0 || na <= 0) return B2Y_ERR_INVALID;
     if (nt > 0 && !targets) return B2Y_ERR_INVALID;
-    build_targets_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(targets, nt, anchors, na, ny, nx, iou_t,
-                                                                            idx, tbox, tcls, count);
+    build_targets_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(targets, nt, anchors, batch, na, ny, nx,
+                                                                            iou_t, idx, tbox, tcls, count);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }

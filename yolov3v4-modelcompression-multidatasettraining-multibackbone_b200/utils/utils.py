@@ -135,8 +135,8 @@ def build_targets(p, targets, model):
     tcls, tbox, indices, av = [], [], [], []
     for i, layer in enumerate(_yolo_modules(model)):
         anchors = _device_anchor_vec(layer, targets.device)
-        ny, nx = int(p[i].shape[2]), int(p[i].shape[3])
-        idx, box, cls = ops.build_targets_layer(targets, anchors, ny, nx, model.hyp['iou_t'])
+        B, ny, nx = int(p[i].shape[0]), int(p[i].shape[2]), int(p[i].shape[3])
+        idx, box, cls = ops.build_targets_layer(targets, anchors, B, ny, nx, model.hyp['iou_t'])
         if cls.numel():
             assert int(cls.max()) < model.nc, \
                 'Model accepts %g classes labeled from 0-%g, however you labelled a class %g. ' \
