@@ -347,6 +347,15 @@ int b2y_bn_train_fwd(const void* z, long long z_pitch, const float* stat_sum, co
                      const float* gamma, const float* beta, float eps, float momentum, float* running_mean,
                      float* running_var, float* save, const void* residual, long long res_pitch, void* y,
                      long long y_pitch, long long pixels, int c, int act, float slope, void* stream);
+/* The same at a channel-pruned width: z, y, the residual, the statistics and `save` are c wide (c % 8 == 0), the
+ * BatchNorm has c_logical channels (c - 8 < c_logical <= c).  Channels c_logical .. c-1 get y = 0 (scale and shift 0,
+ * the residual's pad is zero); gamma, beta and the running statistics are read and written at [0, c_logical) only, and
+ * `save` entries of the pad channels are not written.  b2y_bn_train_fwd is this with c_logical = c. */
+int b2y_bn_train_fwd_lw(const void* z, long long z_pitch, const float* stat_sum, const float* stat_sqsum,
+                        long long count, const float* gamma, const float* beta, float eps, float momentum,
+                        float* running_mean, float* running_var, float* save, const void* residual, long long res_pitch,
+                        void* y, long long y_pitch, long long pixels, int c, int c_logical, int act, float slope,
+                        void* stream);
 /* sums = fp32 [2][c] (caller zeroes): S1 = sum du, S2 = sum du*xhat with du = dy*act'(z*scale+shift) */
 int b2y_bn_train_bwd_reduce(const void* z, long long z_pitch, const void* dy, long long dy_pitch, const float* save,
                             float* sums, float* du_absmax /* optional atomicMax of |du|, caller zeroes */,
@@ -367,6 +376,9 @@ typedef struct b2y_pack_item {
     void* w_dgrad;      /* fp16 [phase][in_c][tap][out_c_pad] (see b2y_pack_dgrad_weights) or NULL */
     int O, Opad, I, k, stride, pad;
     int tile_begin, Ipad; /* Ipad = row length of w_fwd (in_c rounded up to the MMA K granule of 16) */
+    const int* col_map; /* device int [in_c]: the w_fwd column of each input channel, or NULL for the identity.  With a
+                         * map, the columns no input channel maps to are left untouched (zero in a zero-filled buffer):
+                         * the pad channels of a channel-pruned source and the gaps between the sources of a concat */
 } b2y_pack_item;
 typedef struct b2y_unpack_item {
     const float* src;   /* packed weight gradient fp32 [out_c_pad][k][k][in_c_pad] */

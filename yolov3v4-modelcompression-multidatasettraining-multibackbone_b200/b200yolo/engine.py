@@ -598,7 +598,11 @@ class Engine:
                 self._accurate = AccurateRunner(model)
             return self._accurate.forward(x)
         keep = bool(model.keep_features)
-        key = (tuple(x.shape), bool(model.training), x.device.index, keep, x.dtype)
+        # a train-mode forward that records no graph (torch.no_grad(), or frozen parameters) only needs the batch
+        # statistics and the running-statistics update: the forward-only plan, which runs channel-pruned widths too
+        # (adaptive BatchNorm recalibration of pruned candidates, EagleEye_*_prune.py)
+        fwd_only = model.training and not (torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()))
+        key = (tuple(x.shape), bool(model.training), x.device.index, keep, x.dtype) + (('stats',) if fwd_only else ())
         if model.training:
             from .train_engine import TrainPlan, TrainShared
             if self.train_store is None:
@@ -609,7 +613,7 @@ class Engine:
                 self.eval_store = SlotStore(x.device)
             store = self.eval_store
         plan = self.plans.get(key)
-        owner = store.pinned_by()
+        owner = None if fwd_only else store.pinned_by()      # the forward-only plan's slots are its own
         if owner is not None and owner is not plan:
             # a training forward of another shape still waits for its backward and owns the shared slots: this step
             # runs on a plan with private storage, which is not cached
@@ -623,7 +627,7 @@ class Engine:
                 self.plans.pop(next(iter(self.plans)))
             gen = store.generation
             if model.training:
-                plan = TrainPlan(model, tuple(x.shape), x.device, keep, store, self.train_shared)
+                plan = TrainPlan(model, tuple(x.shape), x.device, keep, store, self.train_shared, forward_only=fwd_only)
             else:
                 plan = Plan(model, tuple(x.shape), x.device, keep, store, self.eval_weights)
             self.plans[key] = plan

@@ -49,7 +49,7 @@ class OptStep(C.Structure):
 class PackItem(C.Structure):
     _fields_ = [("w", C.c_void_p), ("w_fwd", C.c_void_p), ("w_dgrad", C.c_void_p),
                 ("O", C.c_int), ("Opad", C.c_int), ("I", C.c_int), ("k", C.c_int), ("stride", C.c_int),
-                ("pad", C.c_int), ("tile_begin", C.c_int), ("Ipad", C.c_int)]
+                ("pad", C.c_int), ("tile_begin", C.c_int), ("Ipad", C.c_int), ("col_map", C.c_void_p)]
 
 
 class UnpackItem(C.Structure):
@@ -128,6 +128,8 @@ _PROTOS = {
     "b2y_maxpool_bwd": (i32, [vp, ll, vp, ll, vp, ll, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b2y_stem_conv_bwd_weight": (i32, [C.POINTER(ConvDesc), vp, vp, vp, f32, i32, vp]),
     "b2y_bn_train_fwd": (i32, [vp, ll, vp, vp, ll, vp, vp, f32, f32, vp, vp, vp, vp, ll, vp, ll, ll, i32, i32, f32, vp]),
+    "b2y_bn_train_fwd_lw": (i32, [vp, ll, vp, vp, ll, vp, vp, f32, f32, vp, vp, vp, vp, ll, vp, ll, ll, i32, i32, i32,
+                                  f32, vp]),
     "b2y_bn_train_bwd_reduce": (i32, [vp, ll, vp, ll, vp, vp, vp, ll, i32, i32, f32, i32, vp]),
     "b2y_bn_train_bwd_apply": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, ll, ll, i32, i32, f32, i32, vp, vp, vp, vp, f32,
                                      vp]),

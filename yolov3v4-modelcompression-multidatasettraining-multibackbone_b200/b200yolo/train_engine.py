@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import LazyFeatures, SlotStore, launch_pointwise, pointwise_steps
+from .engine import LazyFeatures, SlotStore, _pad_rows, launch_pointwise, pointwise_steps
 from .layout import _Tensor, _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources
 from .lib import ACT, ConvDesc, OUT_F16, call, ptr, stream_ptr
 
@@ -51,7 +51,7 @@ def _widen(view, channels):
 class _ConvRec:
     __slots__ = ('i', 'conv', 'bn', 'act', 'slope', 'src', 'z', 'y', 'res', 'head', 'stem', 'k', 's', 'p', 'Cout',
                  'Cpad', 'w16', 'wT', 'stats', 'ones', 'zeros', 'w32', 'aux_row', 'wstem', 'save', 'sums', 'dw',
-                 'depthwise', 'Ipad', 'dwg')
+                 'depthwise', 'Ipad', 'dwg', 'col_map', 'wdw', 'cidx')
 
     def __init__(self):
         for k in self.__slots__:
@@ -59,9 +59,11 @@ class _ConvRec:
 
 
 class _SeRec:
-    __slots__ = ('i', 'src', 'y', 'fc1', 'fc2', 'ws', 'ws_bwd')
+    __slots__ = ('i', 'src', 'y', 'fc1', 'fc2', 'ws', 'ws_bwd', 'w1', 'w2', 'cidx')
 
     def __init__(self, *fields):
+        for k in self.__slots__:
+            setattr(self, k, None)
         for k, v in zip(self.__slots__, fields):
             setattr(self, k, v)
 
@@ -69,12 +71,14 @@ class _SeRec:
 class TrainShared:
     """Training state of one model that does not depend on the input shape, shared by its plans of every shape: the
     packed fp16 weights and data-gradient slabs (`w16`, `wT`) and the stem's packed weights, keyed by layer index, with
-    their pack tables; the OIHW fp32 gradient outputs of the plain-autograd path; and the side stream of the weight
+    their pack tables; the forward-only plans' input-column maps (`col_maps`), which those tables point to and so must
+    live as long as they do; the OIHW fp32 gradient outputs of the plain-autograd path; and the side stream of the weight
     gradients, so that one split-K workspace (`stream_ws`, keyed by stream) serves every plan."""
 
     def __init__(self, device):
         self.device = device
         self.w16, self.wT, self.wstem = {}, {}, {}
+        self.col_maps = {}
         self.pack_tables = {}
         self.own_grads = {}
         self.side_stream = None
@@ -94,10 +98,17 @@ class _Pin:
 
 
 class TrainPlan:
-    def __init__(self, model, x_shape, device, keep_features=False, store=None, shared=None):
+    """forward_only: the plan of a train-mode forward that records no graph (batch statistics, running-statistics update,
+    no backward).  It runs every width the eval plan runs: activations bound at their physical widths (layout.phys_width),
+    weights packed with zero pad rows and input columns scattered through the source's channel map, the BatchNorm apply
+    told the logical width.  It holds no backward state, and its slots are its own (named ('fo', ...)), so a
+    gradient-free forward between a training forward and its backward leaves everything that step saved untouched."""
+
+    def __init__(self, model, x_shape, device, keep_features=False, store=None, shared=None, *, forward_only=False):
         self.model = model
         self.device = device
         self.keep_features = bool(keep_features)
+        self.forward_only = bool(forward_only)
         self.B, self.Cin, self.H, self.W = x_shape
         self.store = store if store is not None else SlotStore(device)
         self.shared = shared if shared is not None else TrainShared(device)
@@ -108,6 +119,8 @@ class TrainPlan:
         self._build()
 
     def _take(self, name, shape, dtype):
+        if self.forward_only:
+            name = ('fo',) + tuple(name)
         t = self.store.take(name, shape, dtype)
         self.held[name] = self.store.versions[name]
         return t
@@ -122,6 +135,13 @@ class TrainPlan:
         # a shortcut is folded into the bn+act apply of the conv before it
         lay = build_layout(model, shapes, self.keep_features, lambda i: _block_parts(mods[i])[1] is not None)
         tens, is_head, fused_into = lay.tens, lay.is_head, lay.fused_into
+        self.layout = lay
+        fo = self.forward_only
+        # the width a buffer is bound at: the physical one in the forward-only plan (the same as the logical one for every
+        # width the training plan accepts)
+        width = (lambda t: t.Cp) if fo else (lambda t: t.C)
+        cidx = lambda i: torch.as_tensor(lay.chmap[i], dtype=torch.long, device=dev)
+        z_later = []        # forward-only: BatchNorm convs whose z lives in the one shared scratch slot
 
         def new_buf(name, Cc, H, W, dtype=torch.float16):
             # fp16: MobileNet widths (24, 40, 72 ...) get a pitch rounded up to the MMA K granule, pad channels stay
@@ -144,17 +164,24 @@ class TrainPlan:
         # multi-source routes are buffers their producers write into; the gradients mirror the placement
         for i, parts in lay.concats.items():
             dst = tens[i]
-            dst.buf = new_buf(('cat', i), dst.C, dst.H, dst.W)
-            gdst = make_grad(dst, zeros_later(dst.buf.shape, GDT))
+            # a conv reads a placed source through view_k, up to its next 16-channel boundary, which may lie past the
+            # concat's own width when a physical width is 8 mod 16 (as in the eval plan)
+            wcat = max([width(dst)] + [off + _round_up(width(st), 16) for st, off, placed in parts if placed]) if fo \
+                else dst.C
+            dst.buf = new_buf(('cat', i), wcat, dst.H, dst.W)
+            gdst = None if fo else make_grad(dst, zeros_later(dst.buf.shape, GDT))
             for st, off, placed in parts:
                 if placed:
                     st.buf = dst.buf
-                    make_grad(st, gdst.buf, off)
+                    if not fo:
+                        make_grad(st, gdst.buf, off)
 
         def alloc(t, i):
             hw = head_width(t.C)
             if t.buf is None:
-                t.buf = new_buf(('act', i), t.C if t.dtype == torch.float16 else hw, t.H, t.W, t.dtype)
+                t.buf = new_buf(('act', i), width(t) if t.dtype == torch.float16 else hw, t.H, t.W, t.dtype)
+            if fo:
+                return t
             if id(t) not in self.grad_of:
                 if t.dtype == torch.float16:
                     make_grad(t, zeros_later(t.buf.shape, GDT))
@@ -173,9 +200,17 @@ class TrainPlan:
                 src = tens[i - 1]
                 out = alloc(tens[i], i)
                 cr = fc[0].out_features
-                self.order.append(('se', _SeRec(i, src, out, fc[0], fc[2],
-                                                self._take(('se_ws', i), (B, 3 * src.C + cr), torch.float32),
-                                                self._take(('se_ws_bwd', i), (B, 3 * src.C + cr), torch.float32))))
+                if fo:
+                    # fc1 columns / fc2 rows scattered to the input's physical channels (zero for pads and gaps)
+                    e = _SeRec(i, src, out, fc[0], fc[2], self._take(('se_ws', i), (B, 3 * src.Cp + cr), torch.float32))
+                    e.w1 = torch.zeros((cr, src.Cp), dtype=torch.float32, device=dev)
+                    e.w2 = torch.zeros((src.Cp, cr), dtype=torch.float32, device=dev)
+                    e.cidx = cidx(i - 1)
+                    self.order.append(('se', e))
+                else:
+                    self.order.append(('se', _SeRec(i, src, out, fc[0], fc[2],
+                                                    self._take(('se_ws', i), (B, 3 * src.C + cr), torch.float32),
+                                                    self._take(('se_ws_bwd', i), (B, 3 * src.C + cr), torch.float32))))
                 feat_idx[i] = out
             elif t in ('convolutional', 'depthwise'):
                 conv, bn, act, slope = _block_parts(m)
@@ -195,13 +230,34 @@ class TrainPlan:
                 # GEMM K granule: Cout is the K of the data-gradient GEMM, Cin the K of the forward / weight-gradient one
                 r.Cpad = head_width(r.Cout) if r.head else _round_up(r.Cout, 16)
                 r.Ipad = _round_up(conv.in_channels, 16)
+                if fo and not r.head:
+                    r.Cpad = tens[i].Cp           # no data-gradient GEMM: the output's physical width
+                if fo and i > 0:
+                    # the forward GEMM's K: the source's physical width up to the MMA K granule (_Tensor.view_k)
+                    r.Ipad = _round_up(tens[i - 1].Cp, 16)
+                    if not r.depthwise and lay.chmap[i - 1] != tuple(range(conv.in_channels)):
+                        # shared, not plan-owned: the cached pack table (keyed by the weight pointers) holds its pointer
+                        key = ('fo', i, lay.chmap[i - 1])
+                        if key not in self.shared.col_maps:
+                            self.shared.col_maps[key] = torch.as_tensor(lay.chmap[i - 1], dtype=torch.int32, device=dev)
+                        r.col_map = self.shared.col_maps[key]
                 if r.head and (bn is not None or act != 'linear'):
                     raise NotImplementedError("unsupported YOLO head conv: BatchNorm or a non-linear activation")
                 r.src = None if i == 0 else tens[i - 1]
                 r.y = alloc(tens[i], i)
                 if i + 1 < n and fused_into[i + 1] == i:
                     r.res = tens[sources(i + 1, defs[i + 1]['from'])[0]]
-                if bn is not None:
+                if bn is not None and fo:
+                    # the BatchNorm apply works on the first Cout of Cp channels: a depthwise layer behind a gapped
+                    # concat would have its channels elsewhere
+                    if lay.chmap[i] != tuple(range(r.Cout)):
+                        raise NotImplementedError("layer %d: BatchNorm over channels a concat placed with gaps" % i)
+                    if r.y.Cp > 2048:
+                        raise NotImplementedError("layer %d: BatchNorm of more than 2048 channels (got %d)" % (i, r.Cout))
+                    r.z = _Tensor(r.Cout, r.y.H, r.y.W, Cp=r.y.Cp)
+                    z_later.append(r)
+                    r.stats = zeros_later((2, r.y.Cp), torch.float32)
+                elif bn is not None:
                     # csrc/bn_train.cu: a thread owns 8 channels, a CTA of 256 threads at least one pixel row
                     if r.Cout % 8 != 0 or r.Cout > 2048:
                         raise NotImplementedError("layer %d: BatchNorm training needs a multiple of 8 channels, at most "
@@ -219,20 +275,28 @@ class TrainPlan:
                 self.order.append(('conv', r))
                 if not is_head[i] and r.res is None:
                     feat_idx[i] = r.y   # (a conv with a fused shortcut never materialises its pre-add output)
-                if r.depthwise:
+                if r.depthwise and fo:
+                    # fp32 weights scattered to the input's physical channels, re-made by every pack
+                    r.wdw = torch.zeros((r.y.Cp,) + tuple(conv.weight.shape[1:]), dtype=torch.float32, device=dev)
+                    r.cidx = cidx(i - 1)
+                elif r.depthwise:
                     r.dwg = zeros_later(tuple(conv.weight.shape), torch.float32)
             elif t == 'yolo':
                 self.yolo.append((m, tens[i - 1]))
             else:
                 self.order += pointwise_steps(lay, i, d, m, alloc)
-                if i in lay.grouped:
+                if i in lay.grouped and not fo:
                     gs = self.grad_of[id(lay.grouped[i])]
                     make_grad(tens[i], gs.buf, gs.c0 + lay.grouped[i].C // 2)
                 if t == 'maxpool' and m.__class__.__name__ == 'Sequential':
                     feat_idx[i] = tens[i]
         self.feature_views = [feat_idx.get(i) for i in feature_slots(model)]
+        self.feature_maps = [lay.chmap[i] for i in feature_slots(model)]
         self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _) in self.yolo]
         self.bn_counters = [r.bn.num_batches_tracked for r in self.convs if r.bn is not None]
+        if fo:
+            self._build_forward_only(z_later)
+            return
         self._plan_grad_writes()
         # ---- arenas ------------------------------------------------------------------------------------------------
         # Everything that has to be zero when a pass starts is carved out of ONE allocation per pass, cleared by ONE
@@ -333,6 +397,96 @@ class TrainPlan:
         self.runs = 0
         self.fwd_graph = self.bwd_graph = None
         self.bwd_key = None
+
+    def _build_forward_only(self, z_later):
+        """The buffers of the forward-only plan: its forward arena (the BatchNorm channel sums), ONE z slot for every
+        layer (the BatchNorm apply consumes z right after its conv), one `save` scratch, the packed forward weights."""
+        B, dev = self.B, self.device
+        fwd_req = [r for r in self.convs if r.stats is not None]
+        offs, total = [], 0
+        for r in fwd_req:
+            offs.append(total)
+            total += _round_up(r.stats.numel() * 4, 256)
+        self.fwd_arena = self._take(('fwd_arena',), (max(total, 256),), torch.uint8)
+        for r, off in zip(fwd_req, offs):
+            r.stats = self.fwd_arena[off:off + r.stats.numel() * 4].view(torch.float32).view(r.stats.shape)
+        if z_later:
+            zpix = lambda r: B * r.z.H * r.z.W * pitch(r.z.Cp, torch.float16)
+            zbuf = self._take(('z',), (max(zpix(r) for r in z_later),), torch.float16)
+            save = torch.empty(4 * max(r.z.Cp for r in z_later), dtype=torch.float32, device=dev)
+            for r in z_later:
+                r.z.buf = zbuf[:zpix(r)].view(B, r.z.H, r.z.W, pitch(r.z.Cp, torch.float16))
+                r.save = save[:4 * r.z.Cp].view(4, r.z.Cp)
+        self.params = [p for p in self.model.parameters()]
+        for r in self.convs:
+            if not r.stem and not r.depthwise:
+                key = ('fo', r.i)
+                if key not in self.shared.w16:
+                    # zero-filled once: pad rows, pad / gap columns and the K pad are never written
+                    self.shared.w16[key] = torch.zeros((r.Cpad, r.k, r.k, r.Ipad), dtype=torch.float16, device=dev)
+                r.w16 = self.shared.w16[key]
+        self.static_x = self._take(('x',), (B, self.Cin, self.H, self.W), torch.float32)
+        st = self.convs[0]
+        if st.stem and st.bn is not None and not st.head and st.conv.in_channels * st.k * st.k <= 32:
+            d = ops.make_conv_desc((B, self.H, self.W, st.conv.in_channels), st.conv.in_channels, st.Cpad, st.k, st.s,
+                                   st.p, st.Cpad)
+            self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,), torch.float16)
+        # feature_out entries at the logical widths: a slice when the logical channels are the first C physical ones,
+        # else (physical view, device index of the logical channels), as the eval plan gives them
+        self.fo_features = []
+        for t, cmap in zip(self.feature_views, self.feature_maps):
+            if t is None:
+                self.fo_features.append(None)
+            elif cmap[-1] == t.C - 1:
+                self.fo_features.append(t.buf[..., t.c0:t.c0 + t.C])
+            else:
+                self.fo_features.append((t.view(), torch.as_tensor(cmap, device=dev)))
+        self.runs = 0
+        self.fwd_graph = self.bwd_graph = None
+
+    def _pack_forward_only(self):
+        """fp32 master weights -> the forward-only plan's operands: ONE table-driven launch for the fp16 forward layout
+        (no data-gradient slabs; input columns through the source's channel map), the stem, and the fp32 depthwise /
+        squeeze-excite weights scattered to their input's physical channels."""
+        from .lib import PackItem, raw
+        body = [r for r in self.convs if not r.stem and not r.depthwise]
+        key = ('fo',) + tuple(r.conv.weight.data_ptr() for r in body)
+        table = self.shared.pack_tables.get(key)
+        if table is None and body:
+            items, tiles = [], 0
+            for r in body:
+                O, I, k = r.conv.weight.shape[0], r.conv.weight.shape[1], r.k
+                w = r.conv.weight.detach()
+                assert w.is_contiguous() and w.dtype == torch.float32
+                ti = int(raw().b2y_layout_tile_i(k))
+                if ti <= 0:
+                    raise NotImplementedError("kernel size %d is not supported by the training engine" % k)
+                items.append(PackItem(w.data_ptr(), r.w16.data_ptr(), None, O, r.Cpad, I, k, r.s, r.p, tiles, r.Ipad,
+                                      r.col_map.data_ptr() if r.col_map is not None else None))
+                tiles += ((r.Cpad + 31) // 32) * ((I + ti - 1) // ti)
+            arr = (PackItem * len(items))(*items)
+            host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
+            table = self.shared.pack_tables[key] = (host.to(self.device), len(items), tiles)
+        if body:
+            tab, n, tiles = table
+            call("b2y_pack_conv_weights_multi", ptr(tab), n, tiles, stream_ptr())
+        for r in self.convs:
+            if r.stem:
+                r.w32 = _pad_rows(r.conv.weight.detach().float(), r.Cpad).contiguous()
+                if r.conv.weight.shape[1] * r.k * r.k <= 32 and not r.head:
+                    key = ('fo', r.i)
+                    if key not in self.shared.wstem:
+                        self.shared.wstem[key] = torch.empty((r.Cpad, 32), dtype=torch.float16, device=self.device)
+                    r.wstem = ops.pack_stem_weights(r.w32, out=self.shared.wstem[key])
+                else:
+                    r.wstem = None
+            elif r.depthwise:
+                r.wdw.index_copy_(0, r.cidx, r.conv.weight.detach())
+        for st in self.order:
+            if st[0] == 'se':
+                e = st[1]
+                e.w1.index_copy_(1, e.cidx, e.fc1.weight.detach())
+                e.w2.index_copy_(0, e.cidx, e.fc2.weight.detach())
 
     # ---------------------------------------------------------------------------------------------------------
     def _params_version(self):
@@ -536,7 +690,7 @@ class TrainPlan:
         model = self.model
         ver = self._params_version()
         if force_pack or ver != self.param_version:
-            self._pack()
+            self._pack_forward_only() if self.forward_only else self._pack()
             self.param_version = None if force_pack else ver
         x = x.contiguous().float()
         self.x = x
@@ -548,7 +702,8 @@ class TrainPlan:
                 self._conv_forward(r, x)
             elif kind == 'se':
                 e = st[1]
-                ops.se_fwd(e.src.view(), e.fc1.weight.detach(), e.fc2.weight.detach(), out=e.y.view(), ws=e.ws)
+                w1, w2 = (e.w1, e.w2) if self.forward_only else (e.fc1.weight.detach(), e.fc2.weight.detach())
+                ops.se_fwd(e.src.view(), w1, w2, out=e.y.view(), ws=e.ws)
             else:
                 launch_pointwise(st)
         if self.bn_counters:
@@ -564,8 +719,8 @@ class TrainPlan:
     def _conv_forward(self, r, x):
         if r.bn is None:
             bias = r.conv.bias.detach() if r.conv.bias is not None else None
-            if r.head and bias is not None:
-                bias = torch.cat([bias, bias.new_zeros(r.Cpad - r.Cout)])
+            if (r.head or self.forward_only) and bias is not None:
+                bias = _pad_rows(bias, r.Cpad)
             out = self._zview(r)
             if r.stem:
                 ops.stem_conv(x, r.w32, bias, r.k, r.s, r.p, act=r.act, slope=r.slope, out=out)
@@ -582,20 +737,29 @@ class TrainPlan:
             ops.stem_conv(x, r.w32, None, r.k, r.s, r.p, act='linear', out=z)
             # channel sums of the stem output: the reduce kernel with u = z, dy = z gives (sum z, sum z*z)
             if r.ones is None:
-                r.ones = torch.ones(r.Cout, dtype=torch.float32, device=self.device)
-                r.zeros = torch.zeros(r.Cout, dtype=torch.float32, device=self.device)
+                r.ones = torch.ones(z.shape[3], dtype=torch.float32, device=self.device)
+                r.zeros = torch.zeros(z.shape[3], dtype=torch.float32, device=self.device)
             B_, H_, W_, C_ = z.shape
             call("b2y_bn_act_bwd_reduce", ptr(z), ops._pitch(z), ptr(z), ops._pitch(z), ptr(r.ones), ptr(r.zeros),
                  ptr(r.zeros), ptr(r.ones), ptr(r.stats[1]), ptr(r.stats[0]), None, B_ * H_ * W_, C_, 0, 0.0, 0,
                  stream_ptr())
         elif r.depthwise:
-            ops.dwconv2d(r.src.view(), r.conv.weight.detach(), r.k, r.s, r.p, out=z, stats=(r.stats[0], r.stats[1]))
+            w = r.wdw if self.forward_only else r.conv.weight.detach()
+            ops.dwconv2d(r.src.view(), w, r.k, r.s, r.p, out=z, stats=(r.stats[0], r.stats[1]))
         else:
-            ops.conv2d(r.src.view_k(), r.w16[:r.Cout], None, r.k, r.s, r.p, out=z, stats=(r.stats[0], r.stats[1]))
+            ops.conv2d(r.src.view_k(), r.w16[:z.shape[3]], None, r.k, r.s, r.p, out=z, stats=(r.stats[0], r.stats[1]))
         bn = r.bn
         count = z.shape[0] * z.shape[1] * z.shape[2]
         res = r.res.view() if r.res is not None else None
         y = r.y.view()
+        if self.forward_only:
+            # z, y and the statistics are Cp wide; gamma, beta and the running statistics are the module's own Cout
+            call("b2y_bn_train_fwd_lw", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
+                 ptr(bn.weight.detach()), ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum),
+                 ptr(bn.running_mean), ptr(bn.running_var), ptr(r.save), ptr(res),
+                 ops._pitch(res) if res is not None else 0, ptr(y), ops._pitch(y), int(count), z.shape[3], r.Cout,
+                 ACT[r.act], float(r.slope), stream_ptr())
+            return
         call("b2y_bn_train_fwd", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
              ptr(bn.weight.detach()), ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum),
              ptr(bn.running_mean), ptr(bn.running_var), ptr(r.save), ptr(res),
@@ -754,6 +918,8 @@ class TrainPlan:
     def run(self, x):
         """autograd entry: returns (yolo_out list, feature_out).  While the step's backward is pending (autograd
         recorded it), the plan's slot store is pinned: the engine runs plans of other shapes on private storage."""
+        if self.forward_only:
+            return self._run_forward_only(x)
         outs = _DarknetTrain.apply(self, x, *self.params)
         if outs[0].grad_fn is not None:
             outs[0].grad_fn.b2y_pin = _Pin(self.store, self)   # released by backward or when the graph is freed
@@ -761,6 +927,14 @@ class TrainPlan:
         object.__setattr__(self.model, '_b2y_epoch', getattr(self.model, '_b2y_epoch', 0) + 1)
         feats = LazyFeatures([None if t is None else t.view() for t in self.feature_views])
         return list(outs), feats
+
+
+    def _run_forward_only(self, x):
+        """(yolo_out list, feature_out) of a train-mode forward without autograd; feature_out at the logical widths."""
+        with torch.no_grad():
+            outs = self.forward_graphed(x)
+        object.__setattr__(self.model, '_b2y_epoch', getattr(self.model, '_b2y_epoch', 0) + 1)
+        return list(outs), LazyFeatures(self.fo_features)
 
 
 class _DarknetTrain(torch.autograd.Function):

@@ -66,7 +66,7 @@ bn_train_fwd_kernel(const __half* __restrict__ z, long long zp, const float* __r
                     const float* __restrict__ s2, const float* __restrict__ gamma, const float* __restrict__ beta,
                     float count, float eps, float momentum, float* __restrict__ rmean, float* __restrict__ rvar,
                     float* __restrict__ save, const __half* __restrict__ res, long long rp, __half* __restrict__ y,
-                    long long yp, long long pixels, int CV, int PPB, int act_rt, float slope) {
+                    long long yp, long long pixels, int CV, int PPB, int act_rt, float slope, int c_logical) {
     pdl_wait();                     // launched as a programmatic dependent (launch_pdl): the statistics / z come from
     pdl_launch_dependents();        // the previous kernel
     const int tid = threadIdx.x;
@@ -77,6 +77,10 @@ bn_train_fwd_kernel(const __half* __restrict__ z, long long zp, const float* __r
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int c = cv * 8 + j;
+        if (c >= c_logical) {       // pad channel of a pruned width: y = act(0) (+ a zero residual pad) = 0
+            sc[j] = sh[j] = 0.f;
+            continue;
+        }
         const float mean = __ldg(s1 + c) / count;
         const float var = fmaxf(__ldg(s2 + c) / count - mean * mean, 0.f);      // biased: used for normalisation
         const float invstd = 1.f / sqrtf(var + eps);
@@ -332,13 +336,14 @@ inline bool shape_ok(int c, long long p0, long long p1, long long p2 = 8) {
 
 }  // namespace
 
-extern "C" int b2y_bn_train_fwd(const void* z, long long z_pitch, const float* stat_sum, const float* stat_sqsum,
-                                long long count, const float* gamma, const float* beta, float eps, float momentum,
-                                float* running_mean, float* running_var, float* save, const void* residual,
-                                long long res_pitch, void* y, long long y_pitch, long long pixels, int c, int act,
-                                float slope, void* stream) {
+extern "C" int b2y_bn_train_fwd_lw(const void* z, long long z_pitch, const float* stat_sum, const float* stat_sqsum,
+                                   long long count, const float* gamma, const float* beta, float eps, float momentum,
+                                   float* running_mean, float* running_var, float* save, const void* residual,
+                                   long long res_pitch, void* y, long long y_pitch, long long pixels, int c,
+                                   int c_logical, int act, float slope, void* stream) {
     if (!z || !y || !stat_sum || !stat_sqsum || !save || count <= 0 || pixels <= 0) return B2Y_ERR_INVALID;
     if (!shape_ok(c, z_pitch, y_pitch, residual ? res_pitch : 8)) return B2Y_ERR_UNSUPPORTED;
+    if (c_logical < 1 || c_logical > c || c - c_logical >= 8) return B2Y_ERR_INVALID;
     const Geo g = geo_for(c);
     const int grid = wave_grid(pixels, g.PPB, 2);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -346,10 +351,19 @@ extern "C" int b2y_bn_train_fwd(const void* z, long long z_pitch, const float* s
         launch_pdl(bn_train_fwd_kernel<decltype(A)::value, 4>, dim3(grid), dim3(256), 0, st, 
             reinterpret_cast<const __half*>(z), z_pitch, stat_sum, stat_sqsum, gamma, beta, (float)count, eps, momentum,
             running_mean, running_var, save, reinterpret_cast<const __half*>(residual), res_pitch,
-            reinterpret_cast<__half*>(y), y_pitch, pixels, g.CV, g.PPB, act, slope);
+            reinterpret_cast<__half*>(y), y_pitch, pixels, g.CV, g.PPB, act, slope, c_logical);
     });
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
+}
+
+extern "C" int b2y_bn_train_fwd(const void* z, long long z_pitch, const float* stat_sum, const float* stat_sqsum,
+                                long long count, const float* gamma, const float* beta, float eps, float momentum,
+                                float* running_mean, float* running_var, float* save, const void* residual,
+                                long long res_pitch, void* y, long long y_pitch, long long pixels, int c, int act,
+                                float slope, void* stream) {
+    return b2y_bn_train_fwd_lw(z, z_pitch, stat_sum, stat_sqsum, count, gamma, beta, eps, momentum, running_mean,
+                               running_var, save, residual, res_pitch, y, y_pitch, pixels, c, c, act, slope, stream);
 }
 
 extern "C" int b2y_bn_train_bwd_reduce(const void* z, long long z_pitch, const void* dy, long long dy_pitch,

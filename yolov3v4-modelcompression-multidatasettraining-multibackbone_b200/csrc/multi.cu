@@ -105,7 +105,19 @@ pack_multi_kernel(const b2y_pack_item* __restrict__ items, int n_items) {
     // ---- forward layout [o][tap][i]: runs of ni halves, two per lane ----
     if (it.w_fwd != nullptr) {
         __half* wf = reinterpret_cast<__half*>(it.w_fwd);
-        if ((ni & 1) == 0) {
+        if (it.col_map != nullptr) {
+            // input column i goes to physical column col_map[i] (a channel-pruned source: its pad channels and the gaps
+            // of a concat keep the zeros the caller filled the buffer with)
+            for (int ol = warp; ol < TO; ol += 8) {
+                const int o = o0 + ol;
+                if (o >= it.Opad) break;
+                for (int j = lane; j < k2 * ni; j += 32) {
+                    const int tap = j / ni, il = j - tap * ni;
+                    wf[((long long)o * k2 + tap) * it.Ipad + __ldg(it.col_map + i0 + il)] =
+                        __float2half_rn(tile[ol][il * k2 + tap]);
+                }
+            }
+        } else if ((ni & 1) == 0) {
             const int npair = ni >> 1;
             const int sh = (npair & (npair - 1)) == 0 ? 31 - __clz(npair) : -1;
             for (int ol = warp; ol < TO; ol += 8) {
