@@ -366,6 +366,17 @@ int b2y_bn_train_bwd_apply(const void* z, long long z_pitch, const void* dy, lon
                            const float* save, const float* sums, void* dz, long long dz_pitch, long long pixels, int c,
                            int act, float slope, int grad_dtype, const float* du_absmax, float* scale_out,
                            float* dgamma_out, float* dbeta_out, float grad_out_scale, void* stream);
+/* fp32 NHWC BatchNorm + activation of the float depthwise blocks of a google-QAT graph (models.py:183-197 under
+ * quantized=1): z, y dense [pixels][c], any c.  training = 1: batch statistics (biased variance) normalise, the running
+ * statistics are updated with the unbiased variance and `momentum`; training = 0: the running statistics normalise.
+ * save = fp32 [4][c] as above.  Sums over pixels are taken in a fixed order in double: two runs give the same bits. */
+int b2y_bn_f32_fwd(const float* z, long long pixels, int c, const float* gamma, const float* beta, float eps,
+                   float momentum, float* running_mean, float* running_var, int training, float* save, float* y, int act,
+                   float slope, void* stream);
+/* dz = gamma*invstd*(du - S1/N - xhat*S2/N) (training) or gamma*invstd*du (eval), du = dy*act'(z*scale+shift);
+ * dbeta = S1 = sum du, dgamma = S2 = sum du*xhat (overwritten).  coef = fp32 [3][c] scratch. */
+int b2y_bn_f32_bwd(const float* z, const float* dy, long long pixels, int c, const float* gamma, const float* save,
+                   int training, float* coef, float* dz, float* dgamma, float* dbeta, int act, float slope, void* stream);
 
 /* ---- table-driven layout kernels (csrc/multi.cu): one launch for ALL convolutions of a model ----
  * Tiles: 32 output channels x b2y_layout_tile_i(k) input channels x k*k taps; tile_begin = running sum of
@@ -412,6 +423,19 @@ int b2y_se_fwd(const void* x, long long x_pitch, const float* w1, const float* w
 int b2y_se_bwd(const void* x, long long x_pitch, const void* dy, long long dy_pitch, const float* w1, const float* w2,
                const float* ws, float* ws_bwd /* fp32 [batch][3c + cr] */, void* dx, long long dx_pitch, int accumulate,
                float* dw1, float* dw2, float grad_scale, int batch, int hw, int c, int cr, int grad_dtype, void* stream);
+/* fp32 versions for the float depthwise / SE layers of a google-QAT graph: dense NHWC fp32 (pitch = c), any c, sums over
+ * pixels in a fixed order (two runs give the same bits).
+ * z = dwconv(x, w) + bias[c] (bias optional) */
+int b2y_dwconv_fwd_f32(const b2y_conv_desc* d, const float* x, const float* w, const float* bias, float* z, void* stream);
+/* dx = dwconv^T(dz, w) and dw[c][k][k] = sum_pixels dz * x, both overwritten; either may be NULL */
+int b2y_dwconv_bwd_f32(const b2y_conv_desc* d, const float* x, const float* dz, const float* w, float* dx, float* dw,
+                       void* stream);
+/* ws layout as b2y_se_fwd */
+int b2y_se_fwd_f32(const float* x, const float* w1, const float* w2, float* y, int batch, int hw, int c, int cr, float* ws,
+                   void* stream);
+/* dx = dy*s + dmean/hw, dw1 [cr][c], dw2 [c][cr] (all overwritten) */
+int b2y_se_bwd_f32(const float* x, const float* dy, const float* w1, const float* w2, const float* ws, float* ws_bwd,
+                   float* dx, float* dw1, float* dw2, int batch, int hw, int c, int cr, void* stream);
 
 /* ---- quantisation-aware training pieces (csrc/quant.cu) ----
  * straight-through backward of b2y_fakequant_f32 (google.py:81-92, 124-143): dx = g * [lo <= round(x/s) <= hi] * gain */

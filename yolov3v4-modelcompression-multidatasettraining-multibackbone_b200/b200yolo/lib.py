@@ -138,6 +138,12 @@ _PROTOS = {
     "b2y_dwconv_bwd_weight": (i32, [C.POINTER(ConvDesc), vp, vp, vp, f32, vp, vp]),
     "b2y_se_fwd": (i32, [vp, ll, vp, vp, vp, ll, i32, i32, i32, i32, vp, vp]),
     "b2y_se_bwd": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, vp, ll, i32, vp, vp, f32, i32, i32, i32, i32, i32, vp]),
+    "b2y_dwconv_fwd_f32": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, vp]),
+    "b2y_dwconv_bwd_f32": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp]),
+    "b2y_se_fwd_f32": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp]),
+    "b2y_se_bwd_f32": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "b2y_bn_f32_fwd": (i32, [vp, ll, i32, vp, vp, f32, f32, vp, vp, i32, vp, vp, i32, f32, vp]),
+    "b2y_bn_f32_bwd": (i32, [vp, vp, ll, i32, vp, vp, i32, vp, vp, vp, vp, i32, f32, vp]),
     "b2y_fakequant_bwd_f32": (i32, [vp, vp, vp, ll, f32, f32, f32, f32, vp]),
     "b2y_tpsq_fwd_f32": (i32, [vp, vp, ll, f32, i32, vp]),
     "b2y_tpsq_bwd_f32": (i32, [vp, vp, vp, vp, ll, f32, i32, vp]),

@@ -12,10 +12,12 @@ per-channel [C]-sized fold arithmetic.
 Exactness: fake-quantised activations and weights are int8 codes times a power of two, exact in fp16, and their products
 / fp32 partial sums are exact, so the quantised conv equals the reference's fp32 F.conv2d on the same values.
 """
+import ctypes
+
 import torch
 
 from . import ops
-from .lib import call, ptr, stream_ptr
+from .lib import ConvDesc, call, ptr, stream_ptr
 
 
 def _pow2_scale(g):
@@ -198,6 +200,102 @@ def search_pow2(scale_value):
     return ce if abs(ce - v) < abs(fl - v) else fl
 
 
+def _dw_desc(x, C, k, s, p):
+    B, H, W, _ = x.shape
+    Ho, Wo = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
+    return ConvDesc(B, H, W, C, C, C, k, s, p, Ho, Wo, C, 0, 0.0, 0, 0, 0), (B, Ho, Wo, C)
+
+
+class DepthwiseBlockFn(torch.autograd.Function):
+    """The float [depthwise] block of a google-QAT graph (reference models.py:175-197 under quantized=1): z =
+    Conv2d(groups=C)(x), y = act(BatchNorm2d(z)), batch statistics in training (running statistics updated in place),
+    running statistics in eval.  fp32 NHWC in both directions on the kernels of depthwise.cu / bn_train.cu."""
+
+    @staticmethod
+    def forward(ctx, x, w, gamma, beta, rmean, rvar, k, s, p, act, slope, training, momentum, eps):
+        C = x.shape[3]
+        x = x.contiguous()
+        wk = w.detach().contiguous()
+        d, shape = _dw_desc(x, C, k, s, p)
+        z = torch.empty(shape, dtype=torch.float32, device=x.device)
+        call("b2y_dwconv_fwd_f32", ctypes.byref(d), ptr(x), ptr(wk), None, ptr(z), stream_ptr())
+        y = torch.empty_like(z)
+        save = torch.empty((4, C), dtype=torch.float32, device=x.device)
+        call("b2y_bn_f32_fwd", ptr(z), z.numel() // C, C, ptr(gamma.detach()), ptr(beta.detach()), float(eps),
+             float(momentum), ptr(rmean), ptr(rvar), int(training), ptr(save), ptr(y), ops.ACT[act], float(slope),
+             stream_ptr())
+        ctx.save_for_backward(x, wk, gamma.detach(), z, save)
+        ctx.geom = (d, int(training), ops.ACT[act], float(slope))
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, wk, gamma, z, save = ctx.saved_tensors
+        d, training, act, slope = ctx.geom
+        C = z.shape[3]
+        gy = gy.contiguous().float()
+        dz = torch.empty_like(z)
+        coef = torch.empty((3, C), dtype=torch.float32, device=z.device)
+        dgamma = torch.empty(C, dtype=torch.float32, device=z.device)
+        dbeta = torch.empty_like(dgamma)
+        call("b2y_bn_f32_bwd", ptr(z), ptr(gy), z.numel() // C, C, ptr(gamma), ptr(save), training, ptr(coef), ptr(dz),
+             ptr(dgamma), ptr(dbeta), act, slope, stream_ptr())
+        dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        dw = torch.empty_like(wk)
+        call("b2y_dwconv_bwd_f32", ctypes.byref(d), ptr(x), ptr(dz), ptr(wk), ptr(dx), ptr(dw), stream_ptr())
+        return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None, None
+
+
+def depthwise_block(block, d, x, training):
+    """module tree Sequential(DepthWise2d, BatchNorm2d[, activation]) of models._conv_block -> NHWC fp32 output"""
+    conv = block[0]
+    if len(block) < 2 or block[1].__class__.__name__ != 'BatchNorm2d':
+        raise NotImplementedError("depthwise block without BatchNorm in the QAT graph")
+    bn = block[1]
+    k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+    if training and bn.momentum is None:
+        raise NotImplementedError("cumulative-average BatchNorm in the QAT graph")
+    slope = block[2].negative_slope if d['activation'] == 'leaky' else 0.1
+    y = DepthwiseBlockFn.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, k, s, p,
+                               d['activation'] if len(block) > 2 else 'linear', slope, training, bn.momentum, bn.eps)
+    if training:
+        bn.num_batches_tracked.add_(1)
+    return y
+
+
+class SEFn(torch.autograd.Function):
+    """SE (utils/layers.py:154-166) over NHWC fp32: y = x * hsigmoid(W2 relu(W1 mean_hw(x)))"""
+
+    @staticmethod
+    def forward(ctx, x, w1, w2):
+        B, H, W, C = x.shape
+        Cr = w1.shape[0]
+        x = x.contiguous()
+        w1d, w2d = w1.detach().contiguous(), w2.detach().contiguous()
+        y = torch.empty_like(x)
+        ws = torch.empty(B * (3 * C + Cr), dtype=torch.float32, device=x.device)
+        call("b2y_se_fwd_f32", ptr(x), ptr(w1d), ptr(w2d), ptr(y), B, H * W, C, Cr, ptr(ws), stream_ptr())
+        ctx.save_for_backward(x, w1d, w2d, ws)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, w1, w2, ws = ctx.saved_tensors
+        B, H, W, C = x.shape
+        Cr = w1.shape[0]
+        gy = gy.contiguous().float()
+        dx = torch.empty_like(x)
+        dw1, dw2 = torch.empty_like(w1), torch.empty_like(w2)
+        wsb = torch.empty(B * (3 * C + Cr), dtype=torch.float32, device=x.device)
+        call("b2y_se_bwd_f32", ptr(x), ptr(gy), ptr(w1), ptr(w2), ptr(ws), ptr(wsb), ptr(dx), ptr(dw1), ptr(dw2), B,
+             H * W, C, Cr, stream_ptr())
+        return dx, dw1, dw2
+
+
+def se_layer(se, x):
+    return SEFn.apply(x, se.fc[0].weight, se.fc[2].weight)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 class QatRunner:
     """Executes the module list of a quantized=1 / 2 Darknet (training or eval) over NHWC fp32 tensors."""
@@ -218,6 +316,10 @@ class QatRunner:
             t = d['type']
             if t == 'convolutional':
                 h = m[0](h)
+            elif t == 'depthwise':
+                h = depthwise_block(m, d, h, model.training)
+            elif t == 'se':
+                h = se_layer(m.se, h)
             elif t == 'shortcut':
                 name = m.__class__.__name__
                 if name == 'Shortcut':           # TPSQ graphs keep the plain layers (models.py:275-305)

@@ -334,6 +334,126 @@ inline bool shape_ok(int c, long long p0, long long p1, long long p2 = 8) {
     return c > 0 && c % 8 == 0 && c / 8 <= 256 && p0 % 8 == 0 && p1 % 8 == 0 && p2 % 8 == 0;
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// fp32 NHWC BatchNorm + activation of the google-QAT graph's float depthwise blocks (b200yolo/qat.py), any C, dense.
+// save [4][C] = mean, invstd, scale, shift: the batch statistics in training, the running ones in eval.  Sums over pixels
+// go through chunk_reduce (common.cuh, fixed order, double).
+struct BnF32StatOp {
+    const float* z;
+    int C;
+    __device__ void operator()(int, long long p, int c, float (&v)[2]) const {
+        const float t = __ldg(z + p * C + c);
+        v[0] = t;
+        v[1] = t * t;
+    }
+};
+__global__ void __launch_bounds__(256) bn_f32_stat_kernel(BnF32StatOp op, long long rows, double* part) {
+    chunk_reduce<2>(op, rows, op.C, part);
+}
+
+// training: batch mean / biased variance for the normalisation, running statistics updated with the unbiased variance
+// (nn.BatchNorm2d); eval: the running statistics
+__global__ void bn_f32_finalize_kernel(const double* __restrict__ part, long long count, const float* __restrict__ gamma,
+                                       const float* __restrict__ beta, float eps, float momentum,
+                                       float* __restrict__ rmean, float* __restrict__ rvar, float* __restrict__ save,
+                                       int C, int training) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    float mean, var;
+    if (training) {
+        double s1 = 0.0, s2 = 0.0;
+        for (int ch = 0; ch < F32_CHUNKS; ++ch) {
+            s1 += part[((long long)ch * 2) * C + c];
+            s2 += part[((long long)ch * 2 + 1) * C + c];
+        }
+        const double m = s1 / (double)count;
+        const double vb = fmax(s2 / (double)count - m * m, 0.0);
+        mean = (float)m;
+        var = (float)vb;
+        const float unbiased = count > 1 ? (float)(vb * ((double)count / (double)(count - 1))) : var;
+        rmean[c] = (1.f - momentum) * rmean[c] + momentum * mean;
+        rvar[c] = (1.f - momentum) * rvar[c] + momentum * unbiased;
+    } else {
+        mean = rmean[c];
+        var = rvar[c];
+    }
+    const float invstd = 1.f / sqrtf(var + eps);
+    const float sc = gamma[c] * invstd;
+    save[c] = mean;
+    save[C + c] = invstd;
+    save[2 * C + c] = sc;
+    save[3 * C + c] = beta[c] - mean * sc;
+}
+
+__global__ void __launch_bounds__(256)
+bn_f32_apply_kernel(const float* __restrict__ z, const float* __restrict__ save, float* __restrict__ y, int C,
+                    long long total, int act, float slope) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % C);
+        y[idx] = apply_act(fmaf(__ldg(z + idx), __ldg(save + 2 * C + c), __ldg(save + 3 * C + c)), act, slope);
+    }
+}
+
+// backward sums: S1 = sum du, S2 = sum du * (z - mean), du = dy * act'(z * scale + shift)
+struct BnF32BwdOp {
+    const float* z;
+    const float* dy;
+    const float* save;
+    int C, act;
+    float slope;
+    __device__ void operator()(int, long long p, int c, float (&v)[2]) const {
+        const float t = __ldg(z + p * C + c);
+        const float du = __ldg(dy + p * C + c) * act_grad(fmaf(t, __ldg(save + 2 * C + c), __ldg(save + 3 * C + c)), act, slope);
+        v[0] = du;
+        v[1] = du * (t - __ldg(save + c));
+    }
+};
+__global__ void __launch_bounds__(256) bn_f32_bwd_stat_kernel(BnF32BwdOp op, long long rows, double* part) {
+    chunk_reduce<2>(op, rows, op.C, part);
+}
+
+// sums [2][C] in fp32 (dbeta, dgamma) and the double coefficients of dz = A du + Bx z + Cc per channel
+__global__ void bn_f32_bwd_finalize_kernel(const double* __restrict__ part, long long count,
+                                           const float* __restrict__ gamma, const float* __restrict__ save,
+                                           float* __restrict__ coef, float* __restrict__ dgamma,
+                                           float* __restrict__ dbeta, int C, int training) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double s1 = 0.0, s2 = 0.0;
+    for (int ch = 0; ch < F32_CHUNKS; ++ch) {
+        s1 += part[((long long)ch * 2) * C + c];
+        s2 += part[((long long)ch * 2 + 1) * C + c];
+    }
+    const double is = save[C + c], mean = save[c];
+    dbeta[c] = (float)s1;
+    dgamma[c] = (float)(s2 * is);
+    const double A = (double)gamma[c] * is;
+    if (training) {   // dz = A (du - S1/N - xhat * (S2 * invstd) / N),  xhat = (z - mean) invstd
+        const double db = s1 / (double)count, dg = s2 * is * is / (double)count;
+        coef[c] = (float)A;
+        coef[C + c] = (float)(-A * dg);
+        coef[2 * C + c] = (float)(A * (mean * dg - db));
+    } else {          // running statistics are constants: dz = A du
+        coef[c] = (float)A;
+        coef[C + c] = 0.f;
+        coef[2 * C + c] = 0.f;
+    }
+}
+
+__global__ void __launch_bounds__(256)
+bn_f32_bwd_apply_kernel(const float* __restrict__ z, const float* __restrict__ dy, const float* __restrict__ save,
+                        const float* __restrict__ coef, float* __restrict__ dz, int C, long long total, int act,
+                        float slope) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % C);
+        const float t = __ldg(z + idx);
+        const float du = __ldg(dy + idx) * act_grad(fmaf(t, __ldg(save + 2 * C + c), __ldg(save + 3 * C + c)), act, slope);
+        dz[idx] = fmaf(__ldg(coef + c), du, fmaf(__ldg(coef + C + c), t, __ldg(coef + 2 * C + c)));
+    }
+}
+
 }  // namespace
 
 extern "C" int b2y_bn_train_fwd_lw(const void* z, long long z_pitch, const float* stat_sum, const float* stat_sqsum,
@@ -414,6 +534,42 @@ extern "C" int b2y_bn_train_bwd_apply(const void* z, long long z_pitch, const vo
                 sums, reinterpret_cast<__half*>(dz), dz_pitch, pixels, g.CV, g.PPB, act, slope, du_absmax, scale_out,
                 dgamma_out, dbeta_out, grad_out_scale);
     });
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_bn_f32_fwd(const float* z, long long pixels, int c, const float* gamma, const float* beta, float eps,
+                              float momentum, float* running_mean, float* running_var, int training, float* save,
+                              float* y, int act, float slope, void* stream) {
+    if (!z || !gamma || !beta || !running_mean || !running_var || !save || !y || pixels <= 0 || c <= 0)
+        return B2Y_ERR_INVALID;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* part = nullptr;
+    if (training) {
+        part = chunk_ws(st, 1, 2, c);
+        if (part == nullptr) return B2Y_ERR_CUDA;
+        bn_f32_stat_kernel<<<chunk_grid(c, 1), dim3(32, 8), 0, st>>>(BnF32StatOp{z, c}, pixels, part);
+    }
+    bn_f32_finalize_kernel<<<(c + 127) / 128, 128, 0, st>>>(part, pixels, gamma, beta, eps, momentum, running_mean,
+                                                             running_var, save, c, training);
+    bn_f32_apply_kernel<<<grid_1d(pixels * c), 256, 0, st>>>(z, save, y, c, pixels * c, act, slope);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_bn_f32_bwd(const float* z, const float* dy, long long pixels, int c, const float* gamma,
+                              const float* save, int training, float* coef /* [3][c] */, float* dz, float* dgamma,
+                              float* dbeta, int act, float slope, void* stream) {
+    if (!z || !dy || !gamma || !save || !coef || !dz || !dgamma || !dbeta || pixels <= 0 || c <= 0)
+        return B2Y_ERR_INVALID;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* part = chunk_ws(st, 1, 2, c);
+    if (part == nullptr) return B2Y_ERR_CUDA;
+    bn_f32_bwd_stat_kernel<<<chunk_grid(c, 1), dim3(32, 8), 0, st>>>(BnF32BwdOp{z, dy, save, c, act, slope}, pixels,
+                                                                      part);
+    bn_f32_bwd_finalize_kernel<<<(c + 127) / 128, 128, 0, st>>>(part, pixels, gamma, save, coef, dgamma, dbeta, c,
+                                                                 training);
+    bn_f32_bwd_apply_kernel<<<grid_1d(pixels * c), 256, 0, st>>>(z, dy, save, coef, dz, c, pixels * c, act, slope);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }

@@ -438,3 +438,65 @@ static inline int acc_finalize(double* acc, float* dst, long long n, cudaStream_
 // `st`, on the same terms as stream_acc: the weight gradient stores its split-K partial tiles there and reduces them in
 // a fixed order (wgrad_tc.cu).
 float* stream_ws(cudaStream_t st, long long n);
+
+// Fixed-order per-channel reduction of the fp32 NHWC paths (QAT depthwise, BatchNorm, squeeze-excite): a CTA of 32
+// channels x 8 pixel rows sums K values per (row, channel) over its chunk of the rows in double, the 8 rows are then added
+// in order, and the chunk's total goes to part[((group * chunks + chunk) * K + k) * C + c].  chunk_sum_kernel adds the
+// chunks in order.  No atomics, so two runs give the same bits.  grid = (ceil(C / 32), F32_CHUNKS, groups), block (32, 8).
+namespace b2y {
+constexpr int F32_CHUNKS = 128;
+
+template <int K, typename Op>
+__device__ __forceinline__ void chunk_reduce(const Op& op, long long rows, int C, double* __restrict__ part) {
+    __shared__ double red[K][8][33];
+    const int c = blockIdx.x * 32 + threadIdx.x;
+    const long long per = (rows + gridDim.y - 1) / gridDim.y;
+    const long long r0 = (long long)blockIdx.y * per;
+    const long long r1 = r0 + per < rows ? r0 + per : rows;
+    double acc[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) acc[k] = 0.0;
+    if (c < C) {
+        for (long long r = r0 + threadIdx.y; r < r1; r += 8) {
+            float v[K];
+            op(blockIdx.z, r, c, v);
+#pragma unroll
+            for (int k = 0; k < K; ++k) acc[k] += (double)v[k];
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < K; ++k) red[k][threadIdx.y][threadIdx.x] = acc[k];
+    __syncthreads();
+    if (threadIdx.y == 0 && c < C) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            double s = 0.0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) s += red[k][j][threadIdx.x];
+            part[(((long long)blockIdx.z * gridDim.y + blockIdx.y) * K + k) * C + c] = s;
+        }
+    }
+}
+
+// out[g][i] = alpha * sum_{chunk} part[g][chunk][i]   (i < n = K * C), chunks added in order
+template <int UNUSED = 0>
+__global__ void chunk_sum_kernel(const double* __restrict__ part, float* __restrict__ out, long long n, int groups,
+                                 float alpha) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n * groups;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const long long g = idx / n, i = idx % n;
+        double s = 0.0;
+        for (int ch = 0; ch < F32_CHUNKS; ++ch) s += part[(g * F32_CHUNKS + ch) * n + i];
+        out[idx] = (float)(s * alpha);
+    }
+}
+
+inline dim3 chunk_grid(int c, int groups) { return dim3((unsigned)((c + 31) / 32), F32_CHUNKS, (unsigned)groups); }
+inline double* chunk_ws(cudaStream_t st, long long groups, int K, int c) {
+    return reinterpret_cast<double*>(stream_ws(st, 2LL * groups * F32_CHUNKS * K * c));
+}
+inline int grid_1d(long long n) {
+    long long g = (n + 255) / 256;
+    return (int)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
+}
+}  // namespace b2y

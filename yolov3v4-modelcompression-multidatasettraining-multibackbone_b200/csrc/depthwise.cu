@@ -424,6 +424,122 @@ inline int set_smem(K kern, size_t bytes, unsigned long long& mask) {
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// fp32 NHWC versions for the google-QAT graph (b200yolo/qat.py), whose depthwise blocks and SE layers stay in float
+// (reference models.py:115-197 under quantized=1).  Dense tensors (pitch = C), any C: MobileNet's widths 24, 40, 72, 120,
+// 184 and 200 are not multiples of 16.  One thread per (pixel, channel), consecutive threads on consecutive channels;
+// every reduction over pixels goes through chunk_reduce (common.cuh), so two runs give the same bits.
+
+// z[n,yo,xo,c] = bias[c] + sum_{r,s} x[n, yo*st-pad+r, xo*st-pad+s, c] * w[c][r][s]
+__global__ void __launch_bounds__(256)
+dwconv_f32_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                      float* __restrict__ z, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo,
+                      long long total) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % C);
+        const long long pix = idx / C;
+        const int xo = (int)(pix % Wo), yo = (int)((pix / Wo) % Ho);
+        const long long n = pix / ((long long)Wo * Ho);
+        const float* wc = w + (long long)c * k * k;
+        float acc = 0.f;
+        for (int r = 0; r < k; ++r) {
+            const int yi = yo * stride - pad + r;
+            if (yi < 0 || yi >= H) continue;
+            for (int s = 0; s < k; ++s) {
+                const int xi = xo * stride - pad + s;
+                if (xi < 0 || xi >= W) continue;
+                acc = fmaf(__ldg(x + ((n * H + yi) * W + xi) * C + c), __ldg(wc + r * k + s), acc);
+            }
+        }
+        z[idx] = bias != nullptr ? acc + __ldg(bias + c) : acc;
+    }
+}
+
+// dx[n,yi,xi,c] = sum_{r,s} w[c][r][s] * dz[n, (yi+pad-r)/st, (xi+pad-s)/st, c]
+__global__ void __launch_bounds__(256)
+dwconv_f32_bwd_data_kernel(const float* __restrict__ dz, const float* __restrict__ w, float* __restrict__ dx, int H,
+                           int W, int C, int k, int stride, int pad, int Ho, int Wo, long long total) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % C);
+        const long long pix = idx / C;
+        const int xi = (int)(pix % W), yi = (int)((pix / W) % H);
+        const long long n = pix / ((long long)W * H);
+        const float* wc = w + (long long)c * k * k;
+        float acc = 0.f;
+        for (int r = 0; r < k; ++r) {
+            const int ty = yi + pad - r;
+            if (ty < 0 || ty % stride != 0 || ty / stride >= Ho) continue;
+            for (int s = 0; s < k; ++s) {
+                const int tx = xi + pad - s;
+                if (tx < 0 || tx % stride != 0 || tx / stride >= Wo) continue;
+                acc = fmaf(__ldg(dz + ((n * Ho + ty / stride) * Wo + tx / stride) * C + c), __ldg(wc + r * k + s), acc);
+            }
+        }
+        dx[idx] = acc;
+    }
+}
+
+// weight gradient, group = tap (r, s): rows are output pixels, value dz * x at the tap's input pixel
+struct DwWgradOp {
+    const float* x;
+    const float* dz;
+    int H, W, C, k, stride, pad, Ho, Wo;
+    __device__ void operator()(int tap, long long pix, int c, float (&v)[1]) const {
+        const int xo = (int)(pix % Wo), yo = (int)((pix / Wo) % Ho);
+        const long long n = pix / ((long long)Wo * Ho);
+        const int yi = yo * stride - pad + tap / k, xi = xo * stride - pad + tap % k;
+        v[0] = (yi < 0 || yi >= H || xi < 0 || xi >= W) ? 0.f
+                                                         : __ldg(dz + pix * C + c) * __ldg(x + ((n * H + yi) * W + xi) * C + c);
+    }
+};
+__global__ void __launch_bounds__(256) dwconv_f32_wgrad_reduce_kernel(DwWgradOp op, long long rows, double* part) {
+    chunk_reduce<1>(op, rows, op.C, part);
+}
+// part [tap][chunk][C] -> dw [C][k*k]
+__global__ void dwconv_f32_wgrad_finish_kernel(const double* __restrict__ part, float* __restrict__ dw, int C, int k2) {
+    for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < C * k2; idx += gridDim.x * blockDim.x) {
+        const int c = idx / k2, tap = idx % k2;
+        double s = 0.0;
+        for (int ch = 0; ch < F32_CHUNKS; ++ch) s += part[((long long)tap * F32_CHUNKS + ch) * C + c];
+        dw[idx] = (float)s;
+    }
+}
+
+// squeeze-excite, group = image: pool sums x, the backward sums dy * x
+struct SePoolOp {
+    const float* x;
+    const float* dy;
+    int C;
+    long long HW;
+    __device__ void operator()(int n, long long p, int c, float (&v)[1]) const {
+        const long long i = ((long long)n * HW + p) * C + c;
+        v[0] = dy != nullptr ? __ldg(x + i) * __ldg(dy + i) : __ldg(x + i);
+    }
+};
+__global__ void __launch_bounds__(256) se_f32_reduce_kernel(SePoolOp op, double* part) {
+    chunk_reduce<1>(op, op.HW, op.C, part);
+}
+
+// forward y = x * s[n][c];  backward dx = dy * s[n][c] + dmean[n][c] / HW
+__global__ void __launch_bounds__(256)
+se_f32_apply_kernel(const float* __restrict__ x, const float* __restrict__ s, const float* __restrict__ dmean,
+                    float* __restrict__ y, long long HW, int C, float inv_hw, long long total) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % C);
+        const long long nc = idx / C / HW * C + c;
+        const float t = __ldg(x + idx) * __ldg(s + nc);
+        y[idx] = dmean != nullptr ? fmaf(__ldg(dmean + nc), inv_hw, t) : t;
+    }
+}
+
+inline bool dw_f32_ok(const b2y_conv_desc* d) {
+    return d->in_c == d->out_c && d->in_c > 0 && d->in_pitch == d->in_c && d->out_pitch == d->out_c && d->ksize >= 1 &&
+           d->ksize <= 7 && d->stride >= 1 && d->batch > 0;
+}
+
 }  // namespace
 
 extern "C" int b2y_dwconv_fwd(const b2y_conv_desc* d, const void* x, const float* w, const float* scale,
@@ -567,6 +683,87 @@ extern "C" int b2y_se_bwd(const void* x, long long x_pitch, const void* dy, long
         se_bwd_apply_kernel<__half><<<(int)gs, 256, 0, st>>>(
             reinterpret_cast<const __half*>(dy), dy_pitch, s, dmean, reinterpret_cast<__half*>(dx), dx_pitch, hw, c,
             1.f / (float)hw, accumulate, total);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_dwconv_fwd_f32(const b2y_conv_desc* d, const float* x, const float* w, const float* bias, float* z,
+                                  void* stream) {
+    if (!d || !x || !w || !z) return B2Y_ERR_INVALID;
+    if (!dw_f32_ok(d)) return B2Y_ERR_UNSUPPORTED;
+    const long long total = (long long)d->batch * d->out_h * d->out_w * d->out_c;
+    dwconv_f32_fwd_kernel<<<grid_1d(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        x, w, bias, z, d->in_h, d->in_w, d->in_c, d->ksize, d->stride, d->pad, d->out_h, d->out_w, total);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_dwconv_bwd_f32(const b2y_conv_desc* d, const float* x, const float* dz, const float* w, float* dx,
+                                  float* dw, void* stream) {
+    if (!d || !dz || !w || (!dx && !dw) || (dw && !x)) return B2Y_ERR_INVALID;
+    if (!dw_f32_ok(d)) return B2Y_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (dx != nullptr) {
+        const long long total = (long long)d->batch * d->in_h * d->in_w * d->in_c;
+        dwconv_f32_bwd_data_kernel<<<grid_1d(total), 256, 0, st>>>(dz, w, dx, d->in_h, d->in_w, d->in_c, d->ksize,
+                                                                  d->stride, d->pad, d->out_h, d->out_w, total);
+    }
+    if (dw != nullptr) {
+        const int k2 = d->ksize * d->ksize;
+        double* part = chunk_ws(st, k2, 1, d->in_c);
+        if (part == nullptr) return B2Y_ERR_CUDA;
+        const DwWgradOp op{x, dz, d->in_h, d->in_w, d->in_c, d->ksize, d->stride, d->pad, d->out_h, d->out_w};
+        dwconv_f32_wgrad_reduce_kernel<<<chunk_grid(d->in_c, k2), dim3(32, 8), 0, st>>>(
+            op, (long long)d->batch * d->out_h * d->out_w, part);
+        dwconv_f32_wgrad_finish_kernel<<<grid_1d((long long)d->in_c * k2), 256, 0, st>>>(part, dw, d->in_c, k2);
+    }
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_se_fwd_f32(const float* x, const float* w1, const float* w2, float* y, int batch, int hw, int c,
+                              int cr, float* ws /* fp32 [batch][3c+cr] */, void* stream) {
+    if (!x || !w1 || !w2 || !y || !ws || batch <= 0 || hw <= 0 || c <= 0 || cr <= 0) return B2Y_ERR_INVALID;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* pooled = ws;                  // layout of b2y_se_fwd: mean [N][C] | v [N][C] | s [N][C] | h [N][Cr]
+    float* v = pooled + (long long)batch * c;
+    float* s = v + (long long)batch * c;
+    float* h = s + (long long)batch * c;
+    double* part = chunk_ws(st, batch, 1, c);
+    if (part == nullptr) return B2Y_ERR_CUDA;
+    se_f32_reduce_kernel<<<chunk_grid(c, batch), dim3(32, 8), 0, st>>>(SePoolOp{x, nullptr, c, hw}, part);
+    chunk_sum_kernel<0><<<grid_1d((long long)batch * c), 256, 0, st>>>(part, pooled, c, batch, 1.f);
+    se_fc_kernel<<<batch, 256, sizeof(float) * (c + cr), st>>>(pooled, w1, w2, pooled, h, v, s, c, cr, 1.f / (float)hw);
+    const long long total = (long long)batch * hw * c;
+    se_f32_apply_kernel<<<grid_1d(total), 256, 0, st>>>(x, s, nullptr, y, hw, c, 0.f, total);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_se_bwd_f32(const float* x, const float* dy, const float* w1, const float* w2,
+                              const float* ws /* from b2y_se_fwd_f32 */, float* ws_bwd /* fp32 [batch][3c+cr] */,
+                              float* dx, float* dw1, float* dw2, int batch, int hw, int c, int cr, void* stream) {
+    if (!x || !dy || !w1 || !w2 || !ws || !ws_bwd || !dx || !dw1 || !dw2 || batch <= 0 || hw <= 0 || c <= 0 || cr <= 0)
+        return B2Y_ERR_INVALID;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float* mean = ws;
+    const float* v = mean + (long long)batch * c;
+    const float* s = v + (long long)batch * c;
+    const float* h = s + (long long)batch * c;
+    float* ds = ws_bwd;                                   // [N][C]  sum dy*x
+    float* dh = ds + (long long)batch * c;                // [N][Cr]
+    float* dmean = dh + (long long)batch * cr;            // [N][C]
+    float* dv = dmean + (long long)batch * c;             // [N][C]
+    double* part = chunk_ws(st, batch, 1, c);
+    if (part == nullptr) return B2Y_ERR_CUDA;
+    se_f32_reduce_kernel<<<chunk_grid(c, batch), dim3(32, 8), 0, st>>>(SePoolOp{x, dy, c, hw}, part);
+    chunk_sum_kernel<0><<<grid_1d((long long)batch * c), 256, 0, st>>>(part, ds, c, batch, 1.f);
+    se_fc_bwd_kernel<<<batch, 256, sizeof(float) * (c + cr), st>>>(ds, v, h, w1, w2, dv, dh, dmean, c, cr);
+    const int gw = grid_1d((long long)c * cr);
+    se_fc_wgrad_kernel<<<gw, 256, 0, st>>>(dv, h, dw2, batch, c, cr, 1.f);        // dW2 [C][Cr]
+    se_fc_wgrad_kernel<<<gw, 256, 0, st>>>(dh, mean, dw1, batch, cr, c, 1.f);     // dW1 [Cr][C]
+    const long long total = (long long)batch * hw * c;
+    se_f32_apply_kernel<<<grid_1d(total), 256, 0, st>>>(dy, s, dmean, dx, hw, c, 1.f / (float)hw, total);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
 }

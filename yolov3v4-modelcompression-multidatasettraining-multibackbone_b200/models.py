@@ -44,7 +44,9 @@ def _conv_block(mdef, in_ch, depthwise, quantized, qkw, maxabsscaler, index):
     groups = in_ch if depthwise else (mdef['groups'] if 'groups' in mdef else 1)
     child = 'DepthWise2d' if depthwise else 'Conv2d'
     seq = nn.Sequential()
-    if quantized in (1, 2, 3):
+    # google QAT keeps [depthwise] blocks in float: the reference's quantized == 1 branch is overwritten by its float
+    # `else` (reference models.py:120-184), so the block is Conv2d(groups=C) + BatchNorm2d + activation
+    if quantized in (1, 2, 3) and not (depthwise and quantized == 1):
         g, c, t = _quantized_layers()
         name = "{:04d}".format(index) + "_" + mdef['type'][:4]
         common = dict(in_channels=in_ch, out_channels=filters, kernel_size=k, stride=stride, padding=pad, groups=groups,
@@ -334,7 +336,7 @@ def get_yolo_layers(model):
 #   se      : fc1.weight, fc2.weight
 def _bn_slots(block, quant):
     head = block[0]
-    if quant:  # quantised convs keep the BN parameters on the conv module itself
+    if quant and hasattr(head, 'gamma'):  # quantised convs keep the BN parameters on the conv module itself
         return [head.beta, head.gamma, head.running_mean, head.running_var]
     bn = block[1]
     return [bn.bias, bn.weight, bn.running_mean, bn.running_var]
@@ -383,7 +385,7 @@ def save_weights(self, path='model.weights', cutoff=-1):
         self.version.tofile(f)
         self.seen.tofile(f)
         for mdef, block in zip(self.module_defs[:cutoff], self.module_list[:cutoff]):
-            for slot in _weight_slots(mdef, block):
+            for slot in _weight_slots(mdef, block, quant=True):
                 slot.data.cpu().numpy().tofile(f)
 
 
