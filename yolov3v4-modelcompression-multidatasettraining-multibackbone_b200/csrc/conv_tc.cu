@@ -285,13 +285,17 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
         // the TMA store needs the identity row mapping; the strided dgrad scatters rows through the register stores
         const bool tma_ok = g.out_identity;
         const bool full = g.Nout % block_n == 0;
+        // a clipped TMA store still writes whole 16-byte pieces of a row (measured on H100: a 255-wide fp32 output also
+        // wrote column 255), so it may clip the last N tile only where the valid width ends on such a piece
+        const int out_esize = out32 ? 4 : (e.out_dtype == OUT_I8 ? 1 : 2);
+        const bool clip_ok = tma_ok && ((long long)g.Nout * out_esize) % 16 == 0;
         // batch statistics ride on the short path when it stores through TMA and nothing is added to the accumulators
         const bool stats_ok = e.stat_sum == nullptr ||
                               (out16 && tma_ok && e.bias == nullptr && e.res == nullptr);
         p.epi_fast = g.kind == CONV_KIND_F16 && (out16 || (out32 && tma_ok)) && !e.out_fakequant &&
                      stats_ok && act_ok && al16(e.out) && e.out_pitch % (out16 ? 8 : 4) == 0 &&
                      (e.bias == nullptr || al16(e.bias)) && (e.res == nullptr || (al16(e.res) && e.res_pitch % 8 == 0)) &&
-                     (full || (tma_ok && e.res == nullptr));
+                     (full || (clip_ok && e.res == nullptr));
         // int8 graph: int8 codes out, no residual, whole N tiles, and a power-of-two accumulator scale so that
         // fma(acc, s, bias) equals the general path's (acc * s) + bias bit for bit
         int ex = 0;
@@ -301,9 +305,9 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
             e.res == nullptr && al16(e.out) && e.out_pitch % 16 == 0 && (e.bias == nullptr || al16(e.bias)) &&
             e.q_lo >= -128.f && e.q_hi <= 127.f && e.q_lo == floorf(e.q_lo) && e.q_hi == floorf(e.q_hi))
             p.epi_fast = 1;
-        // fake-quantised / linear fp32 rows of the int8 graph (the YOLO heads): through the TMA store, which clips Cout = 255
-        if (g.kind == CONV_KIND_I8 && out32 && tma_ok && e.stat_sum == nullptr && e.act == B2Y_ACT_LINEAR &&
-            pow2 && e.res == nullptr && al16(e.out) && e.out_pitch % 4 == 0 && (e.bias == nullptr || al16(e.bias)) &&
+        // fake-quantised / linear fp32 rows of the int8 graph (the YOLO heads): through the TMA store where it can clip
+        if (g.kind == CONV_KIND_I8 && out32 && tma_ok && (full || clip_ok) && e.stat_sum == nullptr &&
+            e.act == B2Y_ACT_LINEAR && pow2 && e.res == nullptr && al16(e.out) && e.out_pitch % 4 == 0 && (e.bias == nullptr || al16(e.bias)) &&
             (!e.out_fakequant || (e.q_lo >= -4194304.f && e.q_hi <= 4194303.f && e.q_lo == floorf(e.q_lo) &&
                                   e.q_hi == floorf(e.q_hi))))
             p.epi_fast = 1;
