@@ -69,7 +69,7 @@ def _train_model(name):
     return model
 
 
-@pytest.mark.parametrize("name", ["yolov3", "yolov4"])
+@pytest.mark.parametrize("name", ["yolov3", "yolov4", "yolov3-mobilenet"])
 def test_multiscale_training_bit_identical(name):
     model = _train_model(name)
     B = 2
@@ -83,10 +83,10 @@ def test_multiscale_training_bit_identical(name):
     assert eng.train_store.generation > 0            # the sequence did grow the slots
 
 
-@pytest.mark.parametrize("name", ["yolov3-mobilenet", "yolov3-tiny"])
+@pytest.mark.parametrize("name", ["yolov3-tiny"])
 def test_multiscale_training_with_atomics(name):
-    """Depthwise and overlapping 2x2 max-pool backward passes add with fp32 atomics, and batch-statistics BatchNorm over
-    two small images amplifies the reordering: two private runs of the same step differ by up to ~10 % of a tensor's
+    """The overlapping 2x2 max-pool backward adds with 16-bit atomics, and batch-statistics BatchNorm over two small
+    images amplifies the reordering: two private runs of the same step differ by up to ~10 % of a tensor's
     max.  Deviations are therefore taken relative to each tensor's max and compared as the worst over all outputs,
     gradients and running statistics of a step (the worst of many tensors is a stable yardstick; one small tensor is
     not): the shared run, against the closer private run, stays within twice the private spread plus 1e-3.  A wrong pad
@@ -121,20 +121,15 @@ def _eval_inputs(shape, dtype, seed):
 
 @pytest.mark.parametrize("name", ["yolov3-tiny", "yolov4", "yolov3-mobilenet"])
 def test_rect_eval_bit_identical(name):
-    """Bit for bit, except that the squeeze-excite pooling of MobileNet sums its channel means with fp32 atomics: there
-    the shared run stays within twice the spread of two private runs, relative to each output's max, plus 1e-5."""
+    """Bit for bit."""
     model = build_model(name, device="cuda").eval()
     batches = [(s, dt) for dt in (torch.uint8, torch.float32) for s in EVAL_SHAPES]
-    exact = name != "yolov3-mobilenet"
 
     def private(x):
         priv = copy.deepcopy(model)
         out = priv(x)
         del priv
         return [out[0]] + list(out[1])
-
-    def worst(u, v):
-        return max((a - b).abs().max().item() / max(b.abs().max().item(), 1e-30) for a, b in zip(u, v))
 
     with torch.no_grad():
         for rnd in range(2):                        # the second round replays the cached plans' graphs
@@ -144,13 +139,8 @@ def test_rect_eval_bit_identical(name):
                 io, p, _ = model(x)
                 got = [io] + list(p)
                 what = "%s %s %s round %d" % (name, shape, dt, rnd)
-                if exact:
-                    for i, (a, b) in enumerate(zip(got, r1)):
-                        assert torch.equal(a, b), what + (": io differs" if i == 0 else ": p[%d] differs" % (i - 1))
-                else:
-                    r2 = private(x)
-                    dev, spread = min(worst(got, r1), worst(got, r2)), worst(r1, r2)
-                    assert dev <= 2 * spread + 1e-5, "%s: deviation %.3g, private spread %.3g" % (what, dev, spread)
+                for i, (a, b) in enumerate(zip(got, r1)):
+                    assert torch.equal(a, b), what + (": io differs" if i == 0 else ": p[%d] differs" % (i - 1))
 
         # static_outputs: each shape's returned buffers belong to its plan and survive forwards of the other shapes
         model.static_outputs = True

@@ -36,9 +36,10 @@ inline int grid_for_rows(long long rows, int ppb, int per_sm) {
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-// block-level reduction of per-thread 8-vectors over the PPB pixel rows of a CTA, then one atomic per channel
-__device__ __forceinline__ void block_reduce_atomic(float (&a)[8], float* red /*[256][9]*/, float* dst, int CV, int PPB,
-                                                    float mul) {
+// block-level reduction of per-thread 8-vectors over the PPB pixel rows of a CTA, then one atomic per channel into the
+// fp64 stream accumulator (common.cuh stream_acc; the host adds it into the fp32 destination with acc_finalize)
+__device__ __forceinline__ void block_reduce_atomic(float (&a)[8], float* red /*[256][9]*/, double* dst, int CV,
+                                                    int PPB, float mul) {
     const int tid = threadIdx.x;
 #pragma unroll
     for (int j = 0; j < 8; ++j) red[tid * 9 + j] = a[j];
@@ -47,18 +48,19 @@ __device__ __forceinline__ void block_reduce_atomic(float (&a)[8], float* red /*
         const int v = i / 8, comp = i % 8;
         float s = 0.f;
         for (int k = 0; k < PPB; ++k) s += red[(v + k * CV) * 9 + comp];
-        atomicAdd(dst + v * 8 + comp, s * mul);
+        atomicAdd(dst + v * 8 + comp, (double)(s * mul));
     }
     __syncthreads();
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// forward: y = act(dwconv(x, w) * scale + bias); optional channel sums of the raw output (training BatchNorm)
+// forward: y = act(dwconv(x, w) * scale + bias); optional channel sums of the raw output (training BatchNorm) into the
+// fp64 accumulator stat_acc: [0, C) sums, [C, 2C) squares.
 // weights arrive as fp32 [C][k][k] (the nn.Conv2d(groups=C) parameter) and are staged as fp16 [tap][C] in smem.
 __global__ void __launch_bounds__(256)
 dwconv_fwd_kernel(const __half* __restrict__ x, long long xp, const float* __restrict__ w,
                   const float* __restrict__ scale, const float* __restrict__ bias, __half* __restrict__ y,
-                  long long yp, float* __restrict__ s1, float* __restrict__ s2, int B, int H, int W, int C, int k,
+                  long long yp, double* __restrict__ stat_acc, int B, int H, int W, int C, int k,
                   int stride, int pad, int Ho, int Wo, int act, float slope, int CV, int PPB) {
     extern __shared__ uint8_t smem_dw[];
     __half* ws = reinterpret_cast<__half*>(smem_dw);                                  // [k*k][C]
@@ -115,7 +117,7 @@ dwconv_fwd_kernel(const __half* __restrict__ x, long long xp, const float* __res
                 o[j] = apply_act(raw, act, slope);
             }
             Half8<__half>::store(y + pix * yp + cv * 8, o);
-            if (s1 != nullptr) {
+            if (stat_acc != nullptr) {
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     const float q = __half2float(__float2half_rn(o[j]));
@@ -125,9 +127,9 @@ dwconv_fwd_kernel(const __half* __restrict__ x, long long xp, const float* __res
             }
         }
     }
-    if (s1 != nullptr) {
-        block_reduce_atomic(a1, red, s1, CV, PPB, 1.f);
-        block_reduce_atomic(a2, red, s2, CV, PPB, 1.f);
+    if (stat_acc != nullptr) {
+        block_reduce_atomic(a1, red, stat_acc, CV, PPB, 1.f);
+        block_reduce_atomic(a2, red, stat_acc + C, CV, PPB, 1.f);
     }
 }
 
@@ -194,11 +196,12 @@ dwconv_bwd_data_kernel(const __half* __restrict__ dz, long long dzp, const float
     }
 }
 
-// weight gradient: dw[c][r][s] += alpha * inv_s * sum_pixels dz[pix][c] * x[pix @ (r,s)][c];  grid.y = tap
+// weight gradient: dw_acc[c][r][s] += alpha * inv_s * sum_pixels dz[pix][c] * x[pix @ (r,s)][c];  grid.y = tap.  dw_acc
+// is the fp64 stream accumulator, added into dw by acc_finalize
 __global__ void __launch_bounds__(256)
 dwconv_bwd_weight_kernel(const __half* __restrict__ x, long long xp, const __half* __restrict__ dz, long long dzp,
-                         float* __restrict__ dw, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo,
-                         float alpha, const float* __restrict__ inv_scale_ptr, int CV, int PPB) {
+                         double* __restrict__ dw_acc, int B, int H, int W, int C, int k, int stride, int pad, int Ho,
+                         int Wo, float alpha, const float* __restrict__ inv_scale_ptr, int CV, int PPB) {
     __shared__ float red[256 * 9];
     const int tap = blockIdx.y;
     const int r = tap / k, s = tap % k;
@@ -233,15 +236,15 @@ dwconv_bwd_weight_kernel(const __half* __restrict__ x, long long xp, const __hal
         const int v = i / 8, comp = i % 8;
         float sum = 0.f;
         for (int q = 0; q < PPB; ++q) sum += red[(v + q * CV) * 9 + comp];
-        atomicAdd(dw + (long long)(v * 8 + comp) * k2 + tap, sum * mul);
+        atomicAdd(dw_acc + (long long)(v * 8 + comp) * k2 + tap, (double)(sum * mul));
     }
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // squeeze-excite
-// pooled[n][c] += sum over the image's pixels of x (caller zeroes; the mean is taken in the fc kernel)
+// pooled[n][c] += sum over the image's pixels of x, into the fp64 accumulator (the mean is taken in the fc kernel)
 __global__ void __launch_bounds__(256)
-se_pool_kernel(const __half* __restrict__ x, long long xp, float* __restrict__ pooled, int HW, int C, int CV, int PPB) {
+se_pool_kernel(const __half* __restrict__ x, long long xp, double* __restrict__ pooled, int HW, int C, int CV, int PPB) {
     __shared__ float red[256 * 9];
     const int n = blockIdx.y;
     const int tid = threadIdx.x;
@@ -319,11 +322,11 @@ se_scale_kernel(const __half* __restrict__ x, long long xp, const float* __restr
     }
 }
 
-// backward, pass 1: ds_raw[n][c] += sum_pixels dy * x
+// backward, pass 1: ds_raw[n][c] += sum_pixels dy * x, into the fp64 accumulator
 template <typename GT>
 __global__ void __launch_bounds__(256)
 se_bwd_reduce_kernel(const __half* __restrict__ x, long long xp, const GT* __restrict__ dy, long long dyp,
-                     float* __restrict__ ds, int HW, int C, int CV, int PPB) {
+                     double* __restrict__ ds, int HW, int C, int CV, int PPB) {
     __shared__ float red[256 * 9];
     const int n = blockIdx.y;
     const int tid = threadIdx.x;
@@ -545,6 +548,7 @@ inline bool dw_f32_ok(const b2y_conv_desc* d) {
 extern "C" int b2y_dwconv_fwd(const b2y_conv_desc* d, const void* x, const float* w, const float* scale,
                               const float* bias, void* y, float* stat_sum, float* stat_sqsum, void* stream) {
     if (!d || !x || !w || !y) return B2Y_ERR_INVALID;
+    if ((stat_sum == nullptr) != (stat_sqsum == nullptr)) return B2Y_ERR_INVALID;
     if (d->in_c != d->out_c || !vec_ok(d->in_c, d->in_pitch, d->out_pitch) || d->ksize < 1 || d->ksize > 7)
         return B2Y_ERR_UNSUPPORTED;
     const Geo g = geo_for(d->in_c);
@@ -553,12 +557,19 @@ extern "C" int b2y_dwconv_fwd(const b2y_conv_desc* d, const void* x, const float
     if (smem > 200 * 1024) return B2Y_ERR_UNSUPPORTED;
     static unsigned long long mask = 0;
     if (set_smem(dwconv_fwd_kernel, smem, mask) != 0) return B2Y_ERR_CUDA;
-    dwconv_fwd_kernel<<<grid_for_rows(pixels, g.PPB, 4), 256, smem, static_cast<cudaStream_t>(stream)>>>(
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int c = d->in_c;
+    double* acc = nullptr;
+    if (stat_sum != nullptr && (acc = stream_acc(st, 2LL * c)) == nullptr) return B2Y_ERR_CUDA;
+    dwconv_fwd_kernel<<<grid_for_rows(pixels, g.PPB, 4), 256, smem, st>>>(
         reinterpret_cast<const __half*>(x), d->in_pitch, w, scale, bias, reinterpret_cast<__half*>(y), d->out_pitch,
-        stat_sum, stat_sqsum, d->batch, d->in_h, d->in_w, d->in_c, d->ksize, d->stride, d->pad, d->out_h, d->out_w,
-        d->act, d->slope, g.CV, g.PPB);
+        acc, d->batch, d->in_h, d->in_w, c, d->ksize, d->stride, d->pad, d->out_h, d->out_w, d->act, d->slope, g.CV,
+        g.PPB);
     B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
+    if (acc == nullptr) return B2Y_OK;
+    const int rc = acc_finalize(acc, stat_sum, c, st);
+    if (rc != B2Y_OK) return rc;
+    return acc_finalize(acc + c, stat_sqsum, c, st);
 }
 
 extern "C" int b2y_dwconv_bwd_data(const b2y_conv_desc* d, const void* dz, const float* w, void* dx, int accumulate,
@@ -597,13 +608,17 @@ extern "C" int b2y_dwconv_bwd_weight(const b2y_conv_desc* d, const void* x, cons
         return B2Y_ERR_UNSUPPORTED;
     const Geo g = geo_for(d->in_c);
     const long long pixels = (long long)d->batch * d->out_h * d->out_w;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const long long n = (long long)d->in_c * d->ksize * d->ksize;
+    double* acc = stream_acc(st, n);
+    if (acc == nullptr) return B2Y_ERR_CUDA;
     dim3 grid(grid_for_rows(pixels, g.PPB, 1), d->ksize * d->ksize);
-    dwconv_bwd_weight_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const __half*>(x), d->in_pitch, reinterpret_cast<const __half*>(dz), d->out_pitch, dw,
+    dwconv_bwd_weight_kernel<<<grid, 256, 0, st>>>(
+        reinterpret_cast<const __half*>(x), d->in_pitch, reinterpret_cast<const __half*>(dz), d->out_pitch, acc,
         d->batch, d->in_h, d->in_w, d->in_c, d->ksize, d->stride, d->pad, d->out_h, d->out_w, alpha, inv_scale_ptr,
         g.CV, g.PPB);
     B2Y_CUDA_CHECK(cudaGetLastError());
-    return B2Y_OK;
+    return acc_finalize(acc, dw, n, st);
 }
 
 extern "C" int b2y_se_fwd(const void* x, long long x_pitch, const float* w1, const float* w2, void* y,
@@ -619,13 +634,18 @@ extern "C" int b2y_se_fwd(const void* x, long long x_pitch, const float* w1, con
     float* s = v + (long long)batch * c;
     float* h = s + (long long)batch * c;
     B2Y_CUDA_CHECK(cudaMemsetAsync(pooled, 0, sizeof(float) * (size_t)batch * c, st));
+    double* acc = stream_acc(st, (long long)batch * c);
+    if (acc == nullptr) return B2Y_ERR_CUDA;
     const Geo g = geo_for(c);
     int gx = (hw + g.PPB - 1) / g.PPB;
     const int cap = (sm_count() * 4 + batch - 1) / batch;
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
-    se_pool_kernel<<<dim3(gx, batch), 256, 0, st>>>(reinterpret_cast<const __half*>(x), x_pitch, pooled, hw, c, g.CV,
+    se_pool_kernel<<<dim3(gx, batch), 256, 0, st>>>(reinterpret_cast<const __half*>(x), x_pitch, acc, hw, c, g.CV,
                                                     g.PPB);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    const int rc = acc_finalize(acc, pooled, (long long)batch * c, st);
+    if (rc != B2Y_OK) return rc;
     se_fc_kernel<<<batch, 256, sizeof(float) * (c + cr), st>>>(pooled, w1, w2, pooled, h, v, s, c, cr, 1.f / (float)hw);
     const long long total = (long long)batch * hw * (c / 8);
     long long gs = (total + 255) / 256;
@@ -652,6 +672,8 @@ extern "C" int b2y_se_bwd(const void* x, long long x_pitch, const void* dy, long
     float* dmean = dh + (long long)batch * cr;            // [N][C]
     float* dv = dmean + (long long)batch * c;             // [N][C]
     B2Y_CUDA_CHECK(cudaMemsetAsync(ds, 0, sizeof(float) * (size_t)batch * c, st));
+    double* acc = stream_acc(st, (long long)batch * c);
+    if (acc == nullptr) return B2Y_ERR_CUDA;
     const Geo g = geo_for(c);
     int gx = (hw + g.PPB - 1) / g.PPB;
     const int cap = (sm_count() * 4 + batch - 1) / batch;
@@ -662,12 +684,15 @@ extern "C" int b2y_se_bwd(const void* x, long long x_pitch, const void* dy, long
     if (gs > (long long)sm_count() * 8) gs = (long long)sm_count() * 8;
     if (grad_dtype == B2Y_DT_BF16)
         se_bwd_reduce_kernel<__nv_bfloat16><<<dim3(gx, batch), 256, 0, st>>>(
-            reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, ds, hw, c,
+            reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __nv_bfloat16*>(dy), dy_pitch, acc, hw, c,
             g.CV, g.PPB);
     else
         se_bwd_reduce_kernel<__half><<<dim3(gx, batch), 256, 0, st>>>(
-            reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, ds, hw, c, g.CV,
+            reinterpret_cast<const __half*>(x), x_pitch, reinterpret_cast<const __half*>(dy), dy_pitch, acc, hw, c, g.CV,
             g.PPB);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    const int rc = acc_finalize(acc, ds, (long long)batch * c, st);
+    if (rc != B2Y_OK) return rc;
     se_fc_bwd_kernel<<<batch, 256, sizeof(float) * (c + cr), st>>>(ds, v, h, w1, w2, dv, dh, dmean, c, cr);
     {
         const long long t2 = (long long)c * cr;
