@@ -42,6 +42,11 @@ def head_width(cout):
     return max(256, _round_up(cout, 16))
 
 
+def _meta(shape, dtype):
+    """Placeholder for a buffer that TrainPlan._carve places in an arena."""
+    return torch.empty(shape, dtype=dtype, device='meta')
+
+
 def _widen(view, channels):
     """The same NHWC view with `channels` channels (its buffer is at least that wide and zero beyond the view)."""
     B, H, W, C = view.shape
@@ -71,9 +76,9 @@ class _SeRec:
 class TrainShared:
     """Training state of one model that does not depend on the input shape, shared by its plans of every shape: the
     packed fp16 weights and data-gradient slabs (`w16`, `wT`) and the stem's packed weights, keyed by layer index, with
-    their pack tables; the forward-only plans' input-column maps (`col_maps`), which those tables point to and so must
-    live as long as they do; the OIHW fp32 gradient outputs of the plain-autograd path; and the side stream of the weight
-    gradients, so that one split-K workspace (`stream_ws`, keyed by stream) serves every plan."""
+    their pack tables; the input-column maps of the layers behind a gapped concat (`col_maps`), which those tables point
+    to and so must live as long as they do; the OIHW fp32 gradient outputs of the plain-autograd path; and the side
+    stream of the weight gradients, so that one split-K workspace (`stream_ws`, keyed by stream) serves every plan."""
 
     def __init__(self, device):
         self.device = device
@@ -98,17 +103,20 @@ class _Pin:
 
 
 class TrainPlan:
-    """forward_only: the plan of a train-mode forward that records no graph (batch statistics, running-statistics update,
-    no backward).  It runs every width the eval plan runs: activations bound at their physical widths (layout.phys_width),
-    weights packed with zero pad rows and input columns scattered through the source's channel map, the BatchNorm apply
-    told the logical width.  It holds no backward state, and its slots are its own (named ('fo', ...)), so a
-    gradient-free forward between a training forward and its backward leaves everything that step saved untouched."""
+    """The forward binds activations at their physical widths (layout.phys_width), packs weights with zero pad rows and
+    input columns scattered through the source's channel map, and tells the BatchNorm apply the logical width.
+
+    forward_only: the plan without its backward state, for a train-mode forward that records no graph (batch
+    statistics and the running-statistics update).  It runs every width the eval plan runs; the gradient plan refuses
+    BatchNorm widths its backward kernels cannot take.  Its slots and packed weights are its own (named ('fo', ...)), so
+    a gradient-free forward between a training forward and its backward leaves everything that step saved untouched."""
 
     def __init__(self, model, x_shape, device, keep_features=False, store=None, shared=None, *, forward_only=False):
         self.model = model
         self.device = device
         self.keep_features = bool(keep_features)
         self.forward_only = bool(forward_only)
+        self._tag = ('fo',) if self.forward_only else ()
         self.B, self.Cin, self.H, self.W = x_shape
         self.store = store if store is not None else SlotStore(device)
         self.shared = shared if shared is not None else TrainShared(device)
@@ -119,11 +127,43 @@ class TrainPlan:
         self._build()
 
     def _take(self, name, shape, dtype):
-        if self.forward_only:
-            name = ('fo',) + tuple(name)
+        name = self._tag + tuple(name)
         t = self.store.take(name, shape, dtype)
         self.held[name] = self.store.versions[name]
         return t
+
+    def _key(self, i):
+        """TrainShared key of layer i's packed weights (the forward-only plans pack their own)."""
+        return self._tag + (i,) if self._tag else i
+
+    def _new_buf(self, name, Cc, H, W, dtype=torch.float16):
+        # fp16: MobileNet widths (24, 40, 72 ...) get a pitch rounded up to the MMA K granule, pad channels stay zero
+        # forever (slots are zero-filled and the pitch depends on the width only)
+        pc = pitch(Cc, dtype)
+        return self._take((name, pc, dtype), (self.B, H, W, pc), dtype)
+
+    def _carve(self, name, fields, last=()):
+        """ONE slot `name` for every meta placeholder that the (holder, attribute) pairs `fields` hold, each at a 256-byte
+        aligned offset; every holder gets the real view.  Placeholders whose ids are in `last` go behind the others.
+        Returns (arena, bytes in front of the first of those)."""
+        held = {}
+        for holder, attr in fields:
+            t = getattr(holder, attr)
+            if t is not None and t.device.type == 'meta':
+                held.setdefault(id(t), (t, []))[1].append((holder, attr))
+        reqs = sorted(held.values(), key=lambda e: id(e[0]) in last)
+        offs, total, front = [], 0, None
+        for t, _ in reqs:
+            if front is None and id(t) in last:
+                front = total
+            offs.append(total)
+            total += _round_up(t.numel() * t.element_size(), 256)
+        arena = self._take(name, (max(total, 256),), torch.uint8)
+        for (t, holders), off in zip(reqs, offs):
+            real = arena[off:off + t.numel() * t.element_size()].view(t.dtype).view(t.shape)
+            for holder, attr in holders:
+                setattr(holder, attr, real)
+        return arena, total if front is None else front
 
     # ---------------------------------------------------------------------------------------------------------
     def _build(self):
@@ -137,58 +177,27 @@ class TrainPlan:
         tens, is_head, fused_into = lay.tens, lay.is_head, lay.fused_into
         self.layout = lay
         fo = self.forward_only
-        # the width a buffer is bound at: the physical one in the forward-only plan (the same as the logical one for every
-        # width the training plan accepts)
-        width = (lambda t: t.Cp) if fo else (lambda t: t.C)
+        # Activations are bound at their physical widths (layout.phys_width), which are the logical ones on every width
+        # the gradient plan accepts.  The rows of a non-head conv's packed forward weights: with a backward, Cout is the
+        # K of the data-gradient GEMM and is rounded up to its granule; without one, the output's physical width.
+        out_rows = (lambda i: tens[i].Cp) if fo else (lambda i: _round_up(shapes[i][0], 16))
         cidx = lambda i: torch.as_tensor(lay.chmap[i], dtype=torch.long, device=dev)
-        z_later = []        # forward-only: BatchNorm convs whose z lives in the one shared scratch slot
 
-        def new_buf(name, Cc, H, W, dtype=torch.float16):
-            # fp16: MobileNet widths (24, 40, 72 ...) get a pitch rounded up to the MMA K granule, pad channels stay
-            # zero forever (slots are zero-filled and the pitch depends on the width only)
-            pc = pitch(Cc, dtype)
-            return self._take((name, pc, dtype), (B, H, W, pc), dtype)
-
-        def zeros_later(shape, dtype):
-            """placeholder (meta tensor) for a buffer that is carved out of the zero-at-start-of-backward arena"""
-            return torch.empty(shape, dtype=dtype, device='meta')
-
-        self.grad_of = {}  # id(_Tensor) -> gradient _Tensor (fp16, same placement)
-
-        def make_grad(t, gbuf=None, c0=0):
-            g = _Tensor(t.C, t.H, t.W, GDT)
-            g.buf, g.c0 = gbuf, c0
-            self.grad_of[id(t)] = g
-            return g
-
-        # multi-source routes are buffers their producers write into; the gradients mirror the placement
+        # multi-source routes are buffers their producers write into
         for i, parts in lay.concats.items():
             dst = tens[i]
             # a conv reads a placed source through view_k, up to its next 16-channel boundary, which may lie past the
             # concat's own width when a physical width is 8 mod 16 (as in the eval plan)
-            wcat = max([width(dst)] + [off + _round_up(width(st), 16) for st, off, placed in parts if placed]) if fo \
-                else dst.C
-            dst.buf = new_buf(('cat', i), wcat, dst.H, dst.W)
-            gdst = None if fo else make_grad(dst, zeros_later(dst.buf.shape, GDT))
+            wcat = max([dst.Cp] + [off + _round_up(st.Cp, 16) for st, off, placed in parts if placed])
+            dst.buf = self._new_buf(('cat', i), wcat, dst.H, dst.W)
             for st, off, placed in parts:
                 if placed:
                     st.buf = dst.buf
-                    if not fo:
-                        make_grad(st, gdst.buf, off)
 
         def alloc(t, i):
-            hw = head_width(t.C)
             if t.buf is None:
-                t.buf = new_buf(('act', i), width(t) if t.dtype == torch.float16 else hw, t.H, t.W, t.dtype)
-            if fo:
-                return t
-            if id(t) not in self.grad_of:
-                if t.dtype == torch.float16:
-                    make_grad(t, zeros_later(t.buf.shape, GDT))
-                else:  # head output: its gradient is directly the GEMM operand dZ -> fp16 (times a device-side scale)
-                    g = _Tensor(hw, t.H, t.W, torch.float16)
-                    g.buf = zeros_later((B, t.H, t.W, hw), torch.float16)
-                    self.grad_of[id(t)] = g
+                t.buf = self._new_buf(('act', i), t.Cp if t.dtype == torch.float16 else head_width(t.C), t.H, t.W,
+                                      t.dtype)
             return t
 
         self.yolo = []
@@ -200,17 +209,13 @@ class TrainPlan:
                 src = tens[i - 1]
                 out = alloc(tens[i], i)
                 cr = fc[0].out_features
+                e = _SeRec(i, src, out, fc[0], fc[2], self._take(('se_ws', i), (B, 3 * src.Cp + cr), torch.float32))
                 if fo:
                     # fc1 columns / fc2 rows scattered to the input's physical channels (zero for pads and gaps)
-                    e = _SeRec(i, src, out, fc[0], fc[2], self._take(('se_ws', i), (B, 3 * src.Cp + cr), torch.float32))
                     e.w1 = torch.zeros((cr, src.Cp), dtype=torch.float32, device=dev)
                     e.w2 = torch.zeros((src.Cp, cr), dtype=torch.float32, device=dev)
                     e.cidx = cidx(i - 1)
-                    self.order.append(('se', e))
-                else:
-                    self.order.append(('se', _SeRec(i, src, out, fc[0], fc[2],
-                                                    self._take(('se_ws', i), (B, 3 * src.C + cr), torch.float32),
-                                                    self._take(('se_ws_bwd', i), (B, 3 * src.C + cr), torch.float32))))
+                self.order.append(('se', e))
                 feat_idx[i] = out
             elif t in ('convolutional', 'depthwise'):
                 conv, bn, act, slope = _block_parts(m)
@@ -227,45 +232,37 @@ class TrainPlan:
                 if r.stem and conv.in_channels > 4:
                     raise NotImplementedError("first layer with more than 4 input channels")
                 r.Cout = conv.out_channels
-                # GEMM K granule: Cout is the K of the data-gradient GEMM, Cin the K of the forward / weight-gradient one
-                r.Cpad = head_width(r.Cout) if r.head else _round_up(r.Cout, 16)
-                r.Ipad = _round_up(conv.in_channels, 16)
-                if fo and not r.head:
-                    r.Cpad = tens[i].Cp           # no data-gradient GEMM: the output's physical width
-                if fo and i > 0:
-                    # the forward GEMM's K: the source's physical width up to the MMA K granule (_Tensor.view_k)
-                    r.Ipad = _round_up(tens[i - 1].Cp, 16)
-                    if not r.depthwise and lay.chmap[i - 1] != tuple(range(conv.in_channels)):
-                        # shared, not plan-owned: the cached pack table (keyed by the weight pointers) holds its pointer
-                        key = ('fo', i, lay.chmap[i - 1])
-                        if key not in self.shared.col_maps:
-                            self.shared.col_maps[key] = torch.as_tensor(lay.chmap[i - 1], dtype=torch.int32, device=dev)
-                        r.col_map = self.shared.col_maps[key]
+                # GEMM K granules: the output rows of the packed weights, and the forward GEMM's K: the source's physical
+                # width up to the MMA K granule (_Tensor.view_k)
+                r.Cpad = head_width(r.Cout) if r.head else out_rows(i)
+                r.Ipad = _round_up(conv.in_channels if i == 0 else tens[i - 1].Cp, 16)
+                if i > 0 and not r.depthwise and lay.chmap[i - 1] != tuple(range(conv.in_channels)):
+                    # input columns scattered through the source's channel map.  Shared, not plan-owned: the cached pack
+                    # table (keyed by the weight pointers) holds its pointer
+                    key = self._tag + (i, lay.chmap[i - 1])
+                    if key not in self.shared.col_maps:
+                        self.shared.col_maps[key] = torch.as_tensor(lay.chmap[i - 1], dtype=torch.int32, device=dev)
+                    r.col_map = self.shared.col_maps[key]
                 if r.head and (bn is not None or act != 'linear'):
                     raise NotImplementedError("unsupported YOLO head conv: BatchNorm or a non-linear activation")
                 r.src = None if i == 0 else tens[i - 1]
                 r.y = alloc(tens[i], i)
                 if i + 1 < n and fused_into[i + 1] == i:
                     r.res = tens[sources(i + 1, defs[i + 1]['from'])[0]]
-                if bn is not None and fo:
+                if bn is not None:
+                    if not fo:
+                        # csrc/bn_train.cu: a thread owns 8 channels, a CTA of 256 threads at least one pixel row
+                        if r.Cout % 8 != 0 or r.Cout > 2048:
+                            raise NotImplementedError("layer %d: BatchNorm training needs a multiple of 8 channels, at "
+                                                      "most 2048 (got %d)" % (i, r.Cout))
                     # the BatchNorm apply works on the first Cout of Cp channels: a depthwise layer behind a gapped
                     # concat would have its channels elsewhere
-                    if lay.chmap[i] != tuple(range(r.Cout)):
+                    elif lay.chmap[i] != tuple(range(r.Cout)):
                         raise NotImplementedError("layer %d: BatchNorm over channels a concat placed with gaps" % i)
-                    if r.y.Cp > 2048:
+                    elif r.y.Cp > 2048:
                         raise NotImplementedError("layer %d: BatchNorm of more than 2048 channels (got %d)" % (i, r.Cout))
                     r.z = _Tensor(r.Cout, r.y.H, r.y.W, Cp=r.y.Cp)
-                    z_later.append(r)
-                    r.stats = zeros_later((2, r.y.Cp), torch.float32)
-                elif bn is not None:
-                    # csrc/bn_train.cu: a thread owns 8 channels, a CTA of 256 threads at least one pixel row
-                    if r.Cout % 8 != 0 or r.Cout > 2048:
-                        raise NotImplementedError("layer %d: BatchNorm training needs a multiple of 8 channels, at most "
-                                                  "2048 (got %d)" % (i, r.Cout))
-                    r.z = _Tensor(r.Cout, r.y.H, r.y.W)
-                    r.z.buf = new_buf(('z', i), r.Cout, r.y.H, r.y.W)
-                    r.stats = zeros_later((2, r.Cout), torch.float32)
-                    r.sums = zeros_later((2, r.Cout), torch.float32)
+                    r.stats = _meta((2, r.y.Cp), torch.float32)
                 else:
                     r.z = r.y   # no BN: the conv epilogue applies bias + activation directly
                     r.ones = torch.ones(r.Cpad, dtype=torch.float32, device=dev)
@@ -279,158 +276,14 @@ class TrainPlan:
                     # fp32 weights scattered to the input's physical channels, re-made by every pack
                     r.wdw = torch.zeros((r.y.Cp,) + tuple(conv.weight.shape[1:]), dtype=torch.float32, device=dev)
                     r.cidx = cidx(i - 1)
-                elif r.depthwise:
-                    r.dwg = zeros_later(tuple(conv.weight.shape), torch.float32)
             elif t == 'yolo':
                 self.yolo.append((m, tens[i - 1]))
             else:
                 self.order += pointwise_steps(lay, i, d, m, alloc)
-                if i in lay.grouped and not fo:
-                    gs = self.grad_of[id(lay.grouped[i])]
-                    make_grad(tens[i], gs.buf, gs.c0 + lay.grouped[i].C // 2)
                 if t == 'maxpool' and m.__class__.__name__ == 'Sequential':
                     feat_idx[i] = tens[i]
         self.feature_views = [feat_idx.get(i) for i in feature_slots(model)]
         self.feature_maps = [lay.chmap[i] for i in feature_slots(model)]
-        self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _) in self.yolo]
-        self.bn_counters = [r.bn.num_batches_tracked for r in self.convs if r.bn is not None]
-        if fo:
-            self._build_forward_only(z_later)
-            return
-        self._plan_grad_writes()
-        # ---- arenas ------------------------------------------------------------------------------------------------
-        # Everything that has to be zero when a pass starts is carved out of ONE allocation per pass, cleared by ONE
-        # memset (round 1: one fill launch per buffer, ~450 launches per step):
-        #   forward arena : the BatchNorm channel sums (sum z, sum z^2) the conv epilogues accumulate into
-        #   backward arena: activation gradients (bf16; consumers accumulate into them), BN backward sums, the per-layer
-        #                   [max|du|, s, 1/s] scale rows, and the packed fp32 weight gradients (split-K red.add targets)
-        self.dz_aux = torch.empty((len(self.convs) + 1, 4), dtype=torch.float32, device='meta')
-        for r in self.convs:
-            if not r.stem and not r.depthwise:
-                r.dw = torch.empty((r.Cpad, r.k, r.k, r.Ipad), dtype=torch.float32, device='meta')
-        fwd_req, bwd_req, seen = [], [], {}
-
-        def want(lst, holder, attr):
-            t = getattr(holder, attr)
-            if t is None or t.device.type != 'meta':
-                return
-            key = id(t)
-            if key not in seen:
-                seen[key] = []
-                lst.append(t)
-            seen[key].append((holder, attr))
-
-        for r in self.convs:
-            want(fwd_req, r, 'stats')
-        for g in self.grad_of.values():
-            want(bwd_req, g, 'buf')
-        for r in self.convs:
-            want(bwd_req, r, 'sums')
-            want(bwd_req, r, 'dw')
-            want(bwd_req, r, 'dwg')
-        want(bwd_req, self, 'dz_aux')
-
-        # gradient buffers whose first writer overwrites (see _plan_grad_writes) go behind the part that is memset.  The
-        # arena is a slot that plans of other shapes lay out differently, so bytes behind the memset hold whatever the
-        # last plan wrote there: a buffer with pad channels (MobileNet widths) stays in the memset part to keep its
-        # pad zero.
-        width = {}
-        for g in self.grad_of.values():
-            width[id(g.buf)] = max(width.get(id(g.buf), 0), g.c0 + g.C)
-        for g in self.grad_of.values():
-            if g.buf.shape[-1] > width[id(g.buf)]:
-                self.dirty_grad_bufs.add(id(g.buf))
-        grad_ids = {id(g.buf) for g in self.grad_of.values()}
-        is_clean = lambda t: id(t) in grad_ids and id(t) not in self.dirty_grad_bufs
-        bwd_req = [t for t in bwd_req if not is_clean(t)] + [t for t in bwd_req if is_clean(t)]
-        self.bwd_zero_bytes = sum(_round_up(t.numel() * t.element_size(), 256) for t in bwd_req if not is_clean(t))
-
-        def carve(name, reqs):
-            offs, total = [], 0
-            for t in reqs:
-                offs.append(total)
-                total += _round_up(t.numel() * t.element_size(), 256)
-            arena = self._take(name, (max(total, 256),), torch.uint8)
-            for t, off in zip(reqs, offs):
-                nbytes = t.numel() * t.element_size()
-                real = arena[off:off + nbytes].view(t.dtype).view(t.shape)
-                for holder, attr in seen[id(t)]:
-                    setattr(holder, attr, real)
-            return arena
-
-        self.fwd_arena = carve(('fwd_arena',), fwd_req)
-        self.bwd_arena = carve(('bwd_arena',), bwd_req)
-        # BatchNorm statistics saved by the forward for the backward: [mean, invstd, scale, shift] per layer
-        for r in self.convs:
-            if r.bn is not None:
-                r.save = torch.empty((4, r.Cout), dtype=torch.float32, device=dev)
-        # The weight gradients hang off the critical path (dz_i -> dW_i has no consumer until the optimiser), so they run
-        # on a second stream concurrently with the data-gradient / BatchNorm chain.  dz is therefore kept per layer
-        # (no buffer shared between a running wgrad and the next layer's BN backward).  The pitch is Cout rounded up to
-        # the K granule of the data-gradient GEMM; the pad channels stay zero.
-        self.dz_bufs = {}
-        for r in self.convs:
-            if r.bn is not None:
-                full = self._take(('dz', r.i, r.Cpad), (B, r.y.H, r.y.W, r.Cpad), torch.float16)
-                self.dz_bufs[r.i] = full[..., :r.Cout]
-        maxc = max(r.Cpad for r in self.convs)
-        self.db_scratch = torch.empty(maxc, dtype=torch.float32, device=dev)
-        self.stem_dw = torch.empty(maxc * 32, dtype=torch.float32, device=dev)
-        self.params = [p for p in model.parameters()]
-        for r in self.convs:
-            if not r.stem and not r.depthwise:
-                # zero-filled once: the K-pad columns (>= I) and pad rows (>= O) are never written again
-                O, I, k = r.conv.weight.shape[0], r.conv.weight.shape[1], r.k
-                if r.i not in self.shared.w16:
-                    self.shared.w16[r.i] = torch.zeros((r.Cpad, k, k, r.Ipad), dtype=torch.float16, device=dev)
-                    self.shared.wT[r.i] = torch.zeros(r.Cpad * I * k * k, dtype=torch.float16, device=dev)
-                r.w16, r.wT = self.shared.w16[r.i], self.shared.wT[r.i]
-        # the graph input and the tensor-core stem's im2col workspace (kept for the weight gradient) are taken here, not
-        # on first use, so that a larger shape grows every slot while its plan is built
-        self.static_x = self._take(('x',), (B, self.Cin, self.H, self.W), torch.float32)
-        st = self.convs[0]
-        if st.stem and st.bn is not None and not st.head and st.conv.in_channels * st.k * st.k <= 32:
-            d = ops.make_conv_desc((B, self.H, self.W, st.conv.in_channels), st.conv.in_channels, st.Cout, st.k, st.s,
-                                   st.p, st.Cout)
-            self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,), torch.float16)
-        self.unpack_table = self.unpack_key = None
-        self.runs = 0
-        self.fwd_graph = self.bwd_graph = None
-        self.bwd_key = None
-
-    def _build_forward_only(self, z_later):
-        """The buffers of the forward-only plan: its forward arena (the BatchNorm channel sums), ONE z slot for every
-        layer (the BatchNorm apply consumes z right after its conv), one `save` scratch, the packed forward weights."""
-        B, dev = self.B, self.device
-        fwd_req = [r for r in self.convs if r.stats is not None]
-        offs, total = [], 0
-        for r in fwd_req:
-            offs.append(total)
-            total += _round_up(r.stats.numel() * 4, 256)
-        self.fwd_arena = self._take(('fwd_arena',), (max(total, 256),), torch.uint8)
-        for r, off in zip(fwd_req, offs):
-            r.stats = self.fwd_arena[off:off + r.stats.numel() * 4].view(torch.float32).view(r.stats.shape)
-        if z_later:
-            zpix = lambda r: B * r.z.H * r.z.W * pitch(r.z.Cp, torch.float16)
-            zbuf = self._take(('z',), (max(zpix(r) for r in z_later),), torch.float16)
-            save = torch.empty(4 * max(r.z.Cp for r in z_later), dtype=torch.float32, device=dev)
-            for r in z_later:
-                r.z.buf = zbuf[:zpix(r)].view(B, r.z.H, r.z.W, pitch(r.z.Cp, torch.float16))
-                r.save = save[:4 * r.z.Cp].view(4, r.z.Cp)
-        self.params = [p for p in self.model.parameters()]
-        for r in self.convs:
-            if not r.stem and not r.depthwise:
-                key = ('fo', r.i)
-                if key not in self.shared.w16:
-                    # zero-filled once: pad rows, pad / gap columns and the K pad are never written
-                    self.shared.w16[key] = torch.zeros((r.Cpad, r.k, r.k, r.Ipad), dtype=torch.float16, device=dev)
-                r.w16 = self.shared.w16[key]
-        self.static_x = self._take(('x',), (B, self.Cin, self.H, self.W), torch.float32)
-        st = self.convs[0]
-        if st.stem and st.bn is not None and not st.head and st.conv.in_channels * st.k * st.k <= 32:
-            d = ops.make_conv_desc((B, self.H, self.W, st.conv.in_channels), st.conv.in_channels, st.Cpad, st.k, st.s,
-                                   st.p, st.Cpad)
-            self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,), torch.float16)
         # feature_out entries at the logical widths: a slice when the logical channels are the first C physical ones,
         # else (physical view, device index of the logical channels), as the eval plan gives them
         self.fo_features = []
@@ -441,97 +294,187 @@ class TrainPlan:
                 self.fo_features.append(t.buf[..., t.c0:t.c0 + t.C])
             else:
                 self.fo_features.append((t.view(), torch.as_tensor(cmap, device=dev)))
+        self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _) in self.yolo]
+        self.bn_counters = [r.bn.num_batches_tracked for r in self.convs if r.bn is not None]
+        # Everything that has to be zero when a pass starts is carved out of ONE allocation per pass, cleared by ONE
+        # memset (round 1: one fill launch per buffer, ~450 launches per step).  The forward arena holds the BatchNorm
+        # channel sums (sum z, sum z^2) the conv epilogues accumulate into.
+        self.fwd_arena, _ = self._carve(('fwd_arena',), [(r, 'stats') for r in self.convs])
+        self.params = [p for p in model.parameters()]
+        for r in self.convs:
+            if not r.stem and not r.depthwise:
+                # zero-filled once: the pad rows, the pad / gap columns and the K pad are never written
+                key = self._key(r.i)
+                if key not in self.shared.w16:
+                    self.shared.w16[key] = torch.zeros((r.Cpad, r.k, r.k, r.Ipad), dtype=torch.float16, device=dev)
+                r.w16 = self.shared.w16[key]
+        # the graph input and the tensor-core stem's im2col workspace (kept for the weight gradient) are taken here, not
+        # on first use, so that a larger shape grows every slot while its plan is built
+        self.static_x = self._take(('x',), (B, self.Cin, self.H, self.W), torch.float32)
+        st = self.convs[0]
+        if st.stem and st.bn is not None and not st.head and st.conv.in_channels * st.k * st.k <= 32:
+            d = ops.make_conv_desc((B, self.H, self.W, st.conv.in_channels), st.conv.in_channels, st.y.Cp, st.k, st.s,
+                                   st.p, st.y.Cp)
+            self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,), torch.float16)
+        bns = [r for r in self.convs if r.bn is not None]
+        if not fo:
+            self._build_backward()
+        elif bns:
+            # without a backward, ONE z slot and one `save` scratch serve every layer: the BatchNorm apply consumes z
+            # right after its conv
+            zpix = lambda r: B * r.z.H * r.z.W * pitch(r.z.Cp, torch.float16)
+            zbuf = self._take(('z',), (max(zpix(r) for r in bns),), torch.float16)
+            save = torch.empty(4 * max(r.z.Cp for r in bns), dtype=torch.float32, device=dev)
+            for r in bns:
+                r.z.buf = zbuf[:zpix(r)].view(B, r.z.H, r.z.W, pitch(r.z.Cp, torch.float16))
+                r.save = save[:4 * r.z.Cp].view(4, r.z.Cp)
         self.runs = 0
         self.fwd_graph = self.bwd_graph = None
 
-    def _pack_forward_only(self):
-        """fp32 master weights -> the forward-only plan's operands: ONE table-driven launch for the fp16 forward layout
-        (no data-gradient slabs; input columns through the source's channel map), the stem, and the fp32 depthwise /
-        squeeze-excite weights scattered to their input's physical channels."""
-        from .lib import PackItem, raw
-        body = [r for r in self.convs if not r.stem and not r.depthwise]
-        key = ('fo',) + tuple(r.conv.weight.data_ptr() for r in body)
-        table = self.shared.pack_tables.get(key)
-        if table is None and body:
-            items, tiles = [], 0
-            for r in body:
-                O, I, k = r.conv.weight.shape[0], r.conv.weight.shape[1], r.k
-                w = r.conv.weight.detach()
-                assert w.is_contiguous() and w.dtype == torch.float32
-                ti = int(raw().b2y_layout_tile_i(k))
-                if ti <= 0:
-                    raise NotImplementedError("kernel size %d is not supported by the training engine" % k)
-                items.append(PackItem(w.data_ptr(), r.w16.data_ptr(), None, O, r.Cpad, I, k, r.s, r.p, tiles, r.Ipad,
-                                      r.col_map.data_ptr() if r.col_map is not None else None))
-                tiles += ((r.Cpad + 31) // 32) * ((I + ti - 1) // ti)
-            arr = (PackItem * len(items))(*items)
-            host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-            table = self.shared.pack_tables[key] = (host.to(self.device), len(items), tiles)
-        if body:
-            tab, n, tiles = table
-            call("b2y_pack_conv_weights_multi", ptr(tab), n, tiles, stream_ptr())
+    def _build_backward(self):
+        """The state only a plan with a backward holds: the gradient mirror of the activations, the backward arena, each
+        BatchNorm layer's own z and saved statistics, dz, and the data-gradient weight slabs."""
+        B, dev, lay = self.B, self.device, self.layout
+        self.grad_of = {}  # id(_Tensor) -> gradient _Tensor (bf16, same placement)
+
+        def make_grad(t, gbuf, c0=0):
+            g = _Tensor(t.C, t.H, t.W, GDT)
+            g.buf, g.c0 = gbuf, c0
+            self.grad_of[id(t)] = g
+            return g
+
+        # the gradients mirror the placement of the multi-source routes and of the grouped ones
+        for i, parts in lay.concats.items():
+            gdst = make_grad(lay.tens[i], _meta(lay.tens[i].buf.shape, GDT))
+            for st, off, placed in parts:
+                if placed:
+                    make_grad(st, gdst.buf, off)
+        for st in self.order:
+            t = st[1].y if st[0] in ('conv', 'se') else getattr(st, 'out', None)
+            if t is None or id(t) in self.grad_of:
+                continue
+            if t.dtype == torch.float16:
+                make_grad(t, _meta(t.buf.shape, GDT))
+            else:  # head output: its gradient is directly the GEMM operand dZ -> fp16 (times a device-side scale)
+                hw = head_width(t.C)
+                g = self.grad_of[id(t)] = _Tensor(hw, t.H, t.W, torch.float16)
+                g.buf = _meta((B, t.H, t.W, hw), torch.float16)
+        for i, src in lay.grouped.items():
+            gs = self.grad_of[id(src)]
+            make_grad(lay.tens[i], gs.buf, gs.c0 + src.C // 2)
+        self._plan_grad_writes()
+
+        # The backward arena: activation gradients (bf16; consumers accumulate into them), BN backward sums, the
+        # per-layer [max|du|, s, 1/s] scale rows, and the packed fp32 weight gradients (split-K red.add targets)
+        self.dz_aux = _meta((len(self.convs) + 1, 4), torch.float32)
         for r in self.convs:
-            if r.stem:
-                r.w32 = _pad_rows(r.conv.weight.detach().float(), r.Cpad).contiguous()
-                if r.conv.weight.shape[1] * r.k * r.k <= 32 and not r.head:
-                    key = ('fo', r.i)
-                    if key not in self.shared.wstem:
-                        self.shared.wstem[key] = torch.empty((r.Cpad, 32), dtype=torch.float16, device=self.device)
-                    r.wstem = ops.pack_stem_weights(r.w32, out=self.shared.wstem[key])
-                else:
-                    r.wstem = None
-            elif r.depthwise:
-                r.wdw.index_copy_(0, r.cidx, r.conv.weight.detach())
+            if r.bn is not None:
+                r.sums = _meta((2, r.Cout), torch.float32)
+            if r.depthwise:
+                r.dwg = _meta(tuple(r.conv.weight.shape), torch.float32)
+            elif not r.stem:
+                r.dw = _meta((r.Cpad, r.k, r.k, r.Ipad), torch.float32)
+        # gradient buffers whose first writer overwrites (see _plan_grad_writes) go behind the part that is memset.  The
+        # arena is a slot that plans of other shapes lay out differently, so bytes behind the memset hold whatever the
+        # last plan wrote there: a buffer with pad channels (MobileNet widths) stays in the memset part to keep its
+        # pad zero.
+        width = {}
+        for g in self.grad_of.values():
+            width[id(g.buf)] = max(width.get(id(g.buf), 0), g.c0 + g.C)
+        for g in self.grad_of.values():
+            if g.buf.shape[-1] > width[id(g.buf)]:
+                self.dirty_grad_bufs.add(id(g.buf))
+        clean = {id(g.buf) for g in self.grad_of.values()} - self.dirty_grad_bufs
+        self.bwd_arena, self.bwd_zero_bytes = self._carve(
+            ('bwd_arena',), [(g, 'buf') for g in self.grad_of.values()] +
+            [(r, a) for r in self.convs for a in ('sums', 'dw', 'dwg')] + [(self, 'dz_aux')], clean)
         for st in self.order:
             if st[0] == 'se':
                 e = st[1]
-                e.w1.index_copy_(1, e.cidx, e.fc1.weight.detach())
-                e.w2.index_copy_(0, e.cidx, e.fc2.weight.detach())
+                e.ws_bwd = self._take(('se_ws_bwd', e.i), tuple(e.ws.shape), torch.float32)
+        # The weight gradients hang off the critical path (dz_i -> dW_i has no consumer until the optimiser), so they run
+        # on a second stream concurrently with the data-gradient / BatchNorm chain.  dz is therefore kept per layer
+        # (no buffer shared between a running wgrad and the next layer's BN backward).  The pitch is Cout rounded up to
+        # the K granule of the data-gradient GEMM; the pad channels stay zero.
+        self.dz_bufs = {}
+        for r in self.convs:
+            if r.bn is not None:
+                r.z.buf = self._new_buf(('z', r.i), r.z.Cp, r.z.H, r.z.W)
+                # BatchNorm statistics saved by the forward for the backward: [mean, invstd, scale, shift]
+                r.save = torch.empty((4, r.Cout), dtype=torch.float32, device=dev)
+                full = self._take(('dz', r.i, r.Cpad), (B, r.y.H, r.y.W, r.Cpad), torch.float16)
+                self.dz_bufs[r.i] = full[..., :r.Cout]
+            if not r.stem and not r.depthwise:
+                if r.i not in self.shared.wT:
+                    # zero-filled once: the pad rows (>= O) are never written again
+                    self.shared.wT[r.i] = torch.zeros(r.Cpad * r.conv.in_channels * r.k * r.k, dtype=torch.float16,
+                                                      device=dev)
+                r.wT = self.shared.wT[r.i]
+        maxc = max(r.Cpad for r in self.convs)
+        self.db_scratch = torch.empty(maxc, dtype=torch.float32, device=dev)
+        self.stem_dw = torch.empty(maxc * 32, dtype=torch.float32, device=dev)
+        self.unpack_table = self.unpack_key = None
+        self.bwd_key = None
 
     # ---------------------------------------------------------------------------------------------------------
     def _params_version(self):
         return sum(p._version for p in self.params)
 
+    def _item_table(self, cls, rows, fields):
+        """(device table, items, tiles) of a table-driven launch over the wgmma convolutions (csrc/multi.cu): item j is
+        cls(**fields[j]) and starts at the tile after item j - 1's rows[j - 1] / 32 x I / tile_i(k) tiles."""
+        from .lib import raw
+        items, tiles = [], 0
+        for n, f in zip(rows, fields):
+            ti = int(raw().b2y_layout_tile_i(f['k']))
+            if ti <= 0:
+                raise NotImplementedError("kernel size %d is not supported by the training engine" % f['k'])
+            items.append(cls(tile_begin=tiles, **f))
+            tiles += ((n + 31) // 32) * ((f['I'] + ti - 1) // ti)
+        host = torch.frombuffer(bytearray(bytes((cls * len(items))(*items))), dtype=torch.uint8)
+        return host.to(self.device), len(items), tiles
+
     def _pack(self):
-        """fp32 master weights -> fp16 operand layouts (forward [O][k][k][I], per-phase data-gradient slabs): ONE
-        table-driven launch over all wgmma convolutions (csrc/multi.cu) + the stem's own tiny pack."""
-        from .lib import PackItem, raw
+        """fp32 master weights -> the operands: ONE table-driven launch over all wgmma convolutions for the fp16 forward
+        layout [O][k][k][I] (input columns through the source's channel map) and, with a backward, the per-phase
+        data-gradient slabs; the stem's own tiny pack; the forward-only plan's fp32 depthwise / squeeze-excite weights
+        scattered to their input's physical channels."""
+        from .lib import PackItem
         body = [r for r in self.convs if not r.stem and not r.depthwise]
-        key = tuple(r.conv.weight.data_ptr() for r in body)
+        key = self._tag + tuple(r.conv.weight.data_ptr() for r in body)
         # one table per set of weight pointers, kept for the life of the shared state: captured graphs of every plan
         # read the table they were captured with
         table = self.shared.pack_tables.get(key)
-        if table is None:
-            items, tiles = [], 0
+        if table is None and body:
             for r in body:
-                O, I, k = r.conv.weight.shape[0], r.conv.weight.shape[1], r.k
-                w = r.conv.weight.detach()
-                assert w.is_contiguous() and w.dtype == torch.float32
-                ti = int(raw().b2y_layout_tile_i(k))
-                if ti <= 0:
-                    raise NotImplementedError("kernel size %d is not supported by the training engine" % k)
-                items.append(PackItem(w.data_ptr(), r.w16.data_ptr(), r.wT.data_ptr(), O, r.Cpad, I, k, r.s, r.p,
-                                      tiles, r.Ipad))
-                tiles += ((r.Cpad + 31) // 32) * ((I + ti - 1) // ti)
-            arr = (PackItem * len(items))(*items)
-            host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-            table = self.shared.pack_tables[key] = (host.to(self.device), len(items), tiles)
-        tab, n, tiles = table
-        call("b2y_pack_conv_weights_multi", ptr(tab), n, tiles, stream_ptr())
+                assert r.conv.weight.is_contiguous() and r.conv.weight.dtype == torch.float32
+            table = self.shared.pack_tables[key] = self._item_table(PackItem, [r.Cpad for r in body], [dict(
+                w=r.conv.weight.data_ptr(), w_fwd=r.w16.data_ptr(), w_dgrad=None if r.wT is None else r.wT.data_ptr(),
+                O=r.Cout, Opad=r.Cpad, I=r.conv.in_channels, k=r.k, stride=r.s, pad=r.p, Ipad=r.Ipad,
+                col_map=None if r.col_map is None else r.col_map.data_ptr()) for r in body])
+        if body:
+            tab, n, tiles = table
+            call("b2y_pack_conv_weights_multi", ptr(tab), n, tiles, stream_ptr())
         for r in self.convs:
             if r.stem:
-                w = r.conv.weight.detach()
-                if r.head:
-                    pad = torch.zeros((r.Cpad - r.Cout,) + tuple(w.shape[1:]), dtype=w.dtype, device=w.device)
-                    w = torch.cat([w, pad], 0)
-                r.w32 = w.float().contiguous()
+                # one row per channel of the output it writes
+                r.w32 = _pad_rows(r.conv.weight.detach().float(), self._zview(r).shape[3]).contiguous()
                 # tensor-core stem: full-im2col weight layout when the receptive field fits one 64-byte GEMM row
-                if w.shape[1] * r.k * r.k <= 32 and not r.head:
-                    if r.i not in self.shared.wstem:
-                        self.shared.wstem[r.i] = torch.empty((r.Cout, 32), dtype=torch.float16, device=self.device)
-                    r.wstem = ops.pack_stem_weights(r.w32, out=self.shared.wstem[r.i])
+                if r.conv.in_channels * r.k * r.k <= 32 and not r.head:
+                    key = self._key(r.i)
+                    if key not in self.shared.wstem:
+                        self.shared.wstem[key] = torch.empty((r.w32.shape[0], 32), dtype=torch.float16,
+                                                             device=self.device)
+                    r.wstem = ops.pack_stem_weights(r.w32, out=self.shared.wstem[key])
                 else:
                     r.wstem = None
+            elif r.wdw is not None:
+                r.wdw.index_copy_(0, r.cidx, r.conv.weight.detach())
+        for st in self.order:
+            if st[0] == 'se' and st[1].w1 is not None:
+                e = st[1]
+                e.w1.index_copy_(1, e.cidx, e.fc1.weight.detach())
+                e.w2.index_copy_(0, e.cidx, e.fc2.weight.detach())
 
     def _plan_grad_writes(self):
         """Which backward write into an activation-gradient buffer is the FIRST one of its channel range.
@@ -615,20 +558,14 @@ class TrainPlan:
 
     def _unpack_all(self):
         """packed fp32 weight gradients [O][k][k][I] of all wgmma convolutions -> OIHW destinations, ONE launch."""
-        from .lib import UnpackItem, raw
+        from .lib import UnpackItem
         body = [r for r in self.convs if not r.stem and not r.depthwise]
         dsts = [self._grad_dst(r.conv.weight) for r in body]
         key = tuple(d.data_ptr() for d in dsts)
         if self.unpack_table is None or key != self.unpack_key:
-            items, tiles = [], 0
-            for r, d in zip(body, dsts):
-                O, I, k = r.Cout, r.conv.in_channels, r.k
-                ti = int(raw().b2y_layout_tile_i(k))
-                items.append(UnpackItem(r.dw.data_ptr(), d.data_ptr(), O, I, k, 0, tiles, r.Ipad))
-                tiles += ((O + 31) // 32) * ((I + ti - 1) // ti)
-            arr = (UnpackItem * len(items))(*items)
-            host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-            self.unpack_table = (host.to(self.device), len(items), tiles)
+            self.unpack_table = self._item_table(UnpackItem, [r.Cout for r in body], [dict(
+                src=r.dw.data_ptr(), dst=d.data_ptr(), O=r.Cout, I=r.conv.in_channels, k=r.k, accumulate=0, Ipad=r.Ipad)
+                for r, d in zip(body, dsts)])
             self.unpack_key = key
         tab, n, tiles = self.unpack_table
         call("b2y_unpack_wgrad_multi", ptr(tab), n, tiles, stream_ptr())
@@ -690,7 +627,7 @@ class TrainPlan:
         model = self.model
         ver = self._params_version()
         if force_pack or ver != self.param_version:
-            self._pack_forward_only() if self.forward_only else self._pack()
+            self._pack()
             self.param_version = None if force_pack else ver
         x = x.contiguous().float()
         self.x = x
@@ -702,7 +639,7 @@ class TrainPlan:
                 self._conv_forward(r, x)
             elif kind == 'se':
                 e = st[1]
-                w1, w2 = (e.w1, e.w2) if self.forward_only else (e.fc1.weight.detach(), e.fc2.weight.detach())
+                w1, w2 = (e.fc1.weight.detach(), e.fc2.weight.detach()) if e.w1 is None else (e.w1, e.w2)
                 ops.se_fwd(e.src.view(), w1, w2, out=e.y.view(), ws=e.ws)
             else:
                 launch_pointwise(st)
@@ -718,10 +655,8 @@ class TrainPlan:
 
     def _conv_forward(self, r, x):
         if r.bn is None:
-            bias = r.conv.bias.detach() if r.conv.bias is not None else None
-            if (r.head or self.forward_only) and bias is not None:
-                bias = _pad_rows(bias, r.Cpad)
             out = self._zview(r)
+            bias = _pad_rows(r.conv.bias.detach() if r.conv.bias is not None else None, out.shape[3])
             if r.stem:
                 ops.stem_conv(x, r.w32, bias, r.k, r.s, r.p, act=r.act, slope=r.slope, out=out)
             else:
@@ -744,7 +679,7 @@ class TrainPlan:
                  ptr(r.zeros), ptr(r.ones), ptr(r.stats[1]), ptr(r.stats[0]), None, B_ * H_ * W_, C_, 0, 0.0, 0,
                  stream_ptr())
         elif r.depthwise:
-            w = r.wdw if self.forward_only else r.conv.weight.detach()
+            w = r.conv.weight.detach() if r.wdw is None else r.wdw
             ops.dwconv2d(r.src.view(), w, r.k, r.s, r.p, out=z, stats=(r.stats[0], r.stats[1]))
         else:
             ops.conv2d(r.src.view_k(), r.w16[:z.shape[3]], None, r.k, r.s, r.p, out=z, stats=(r.stats[0], r.stats[1]))
@@ -752,18 +687,11 @@ class TrainPlan:
         count = z.shape[0] * z.shape[1] * z.shape[2]
         res = r.res.view() if r.res is not None else None
         y = r.y.view()
-        if self.forward_only:
-            # z, y and the statistics are Cp wide; gamma, beta and the running statistics are the module's own Cout
-            call("b2y_bn_train_fwd_lw", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
-                 ptr(bn.weight.detach()), ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum),
-                 ptr(bn.running_mean), ptr(bn.running_var), ptr(r.save), ptr(res),
-                 ops._pitch(res) if res is not None else 0, ptr(y), ops._pitch(y), int(count), z.shape[3], r.Cout,
-                 ACT[r.act], float(r.slope), stream_ptr())
-            return
-        call("b2y_bn_train_fwd", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
+        # z, y and the statistics are Cp wide; gamma, beta and the running statistics are the module's own Cout
+        call("b2y_bn_train_fwd_lw", ptr(z), ops._pitch(z), ptr(r.stats[0]), ptr(r.stats[1]), int(count),
              ptr(bn.weight.detach()), ptr(bn.bias.detach()), float(bn.eps), float(bn.momentum),
              ptr(bn.running_mean), ptr(bn.running_var), ptr(r.save), ptr(res),
-             ops._pitch(res) if res is not None else 0, ptr(y), ops._pitch(y), int(count), r.Cout,
+             ops._pitch(res) if res is not None else 0, ptr(y), ops._pitch(y), int(count), z.shape[3], r.Cout,
              ACT[r.act], float(r.slope), stream_ptr())
 
     # ---------------------------------------------------------------------------------------------------------
@@ -916,23 +844,17 @@ class TrainPlan:
 
     # ---------------------------------------------------------------------------------------------------------
     def run(self, x):
-        """autograd entry: returns (yolo_out list, feature_out).  While the step's backward is pending (autograd
-        recorded it), the plan's slot store is pinned: the engine runs plans of other shapes on private storage."""
+        """autograd entry: returns (yolo_out list, feature_out at the logical widths).  While the step's backward is
+        pending (autograd recorded it), the plan's slot store is pinned: the engine runs plans of other shapes on private
+        storage."""
         if self.forward_only:
-            return self._run_forward_only(x)
-        outs = _DarknetTrain.apply(self, x, *self.params)
-        if outs[0].grad_fn is not None:
-            outs[0].grad_fn.b2y_pin = _Pin(self.store, self)   # released by backward or when the graph is freed
+            with torch.no_grad():
+                outs = self.forward_graphed(x)
+        else:
+            outs = _DarknetTrain.apply(self, x, *self.params)
+            if outs[0].grad_fn is not None:
+                outs[0].grad_fn.b2y_pin = _Pin(self.store, self)   # released by backward or when the graph is freed
         # the running statistics were just updated through raw pointers (also under graph replay): eval plans re-fold
-        object.__setattr__(self.model, '_b2y_epoch', getattr(self.model, '_b2y_epoch', 0) + 1)
-        feats = LazyFeatures([None if t is None else t.view() for t in self.feature_views])
-        return list(outs), feats
-
-
-    def _run_forward_only(self, x):
-        """(yolo_out list, feature_out) of a train-mode forward without autograd; feature_out at the logical widths."""
-        with torch.no_grad():
-            outs = self.forward_graphed(x)
         object.__setattr__(self.model, '_b2y_epoch', getattr(self.model, '_b2y_epoch', 0) + 1)
         return list(outs), LazyFeatures(self.fo_features)
 
