@@ -196,8 +196,12 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t cta_ra
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(cta_rank));
     return r;
 }
+// Arrive on an mbarrier of any CTA of the cluster (the stage-release of a multicast ring).  CTA-scope release, the
+// default: the consumer's reads of the stage were wgmma operand reads that wgmma.wait_group has already retired, so no
+// generic-proxy data is published through this arrive.  A .cluster-scope release compiles to a GPU-wide MEMBAR in
+// front of every arrive, once per k-step per peer, which stalls the MMA warps.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
 }
 // named barrier over `nthreads` threads (a multiple of 32); id 0 is __syncthreads()
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
