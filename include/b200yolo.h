@@ -356,12 +356,17 @@ int b2y_bn_train_fwd_lw(const void* z, long long z_pitch, const float* stat_sum,
                         float* running_mean, float* running_var, float* save, const void* residual, long long res_pitch,
                         void* y, long long y_pitch, long long pixels, int c, int c_logical, int act, float slope,
                         void* stream);
-/* sums = fp32 [2][c] (caller zeroes): S1 = sum du, S2 = sum du*xhat with du = dy*act'(z*scale+shift) */
+/* sums = fp32 [2][c] (caller zeroes): S1 = sum du, S2 = sum du*xhat with du = dy*act'(z*scale+shift).
+ * du_absmax (optional) = fp32 [4], caller zeroes: [0] = max|du| and [3] = max|xhat| over the layer (atomicMax);
+ * [1] and [2] are left to b2y_bn_train_bwd_apply's scale_out. */
 int b2y_bn_train_bwd_reduce(const void* z, long long z_pitch, const void* dy, long long dy_pitch, const float* save,
-                            float* sums, float* du_absmax /* optional atomicMax of |du|, caller zeroes */,
+                            float* sums, float* du_absmax /* optional fp32 [4], see above */,
                             long long pixels, int c, int act, float slope, int grad_dtype, void* stream);
 /* dz = s * gamma*invstd*(du - S1/N - xhat*S2/N) as fp16 (s = power of two chosen on the device -> scale_out[0..1] =
- * [s, 1/s]); also emits the parameter gradients dgamma_out = S2*grad_out_scale, dbeta_out = S1*grad_out_scale */
+ * [s, 1/s]); also emits the parameter gradients dgamma_out = S2*grad_out_scale, dbeta_out = S1*grad_out_scale.
+ * s maps the bound max_c |gamma*invstd| * (max|du| + |S1|/N + max|xhat|*|S2|/N) >= max|dz| to at most 2^12, with
+ * max|du| and max|xhat| read from the reduce's du_absmax[0] and [3]; without du_absmax they are taken as 1 and
+ * sqrt(pixels). */
 int b2y_bn_train_bwd_apply(const void* z, long long z_pitch, const void* dy, long long dy_pitch, const float* gamma,
                            const float* save, const float* sums, void* dz, long long dz_pitch, long long pixels, int c,
                            int act, float slope, int grad_dtype, const float* du_absmax, float* scale_out,

@@ -182,7 +182,7 @@ def test_bn_train_fused_passes(act, C, gdt):
     torch.cuda.synchronize()
     s_dev, inv_dev = float(aux[1]), float(aux[2])
     assert s_dev > 0 and abs(s_dev * inv_dev - 1.0) < 1e-6 and float(torch.log2(aux[1])) % 1.0 == 0.0
-    assert float(dz.float().abs().max()) <= 8192.0
+    assert float(dz.float().abs().max()) <= 4096.0 * (1 + 2.0 ** -10)     # the 2^12 target, within one fp16 ulp
     dz = dz.float() * inv_dev
     assert (_nchw(out) - y.detach().float()).abs().max() < 6e-3
     np.testing.assert_allclose(rmc.cpu().numpy(), rm_r.float().numpy(), rtol=1e-4, atol=1e-5)

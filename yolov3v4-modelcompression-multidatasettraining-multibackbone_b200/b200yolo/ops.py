@@ -369,7 +369,10 @@ def bn_train_fwd(z, s1, s2, gamma, beta, eps, momentum, running_mean, running_va
 
 
 def bn_train_bwd(z, dy, gamma, save, act, slope=0.1, grad_out_scale=1.0):
-    """Backward of bn_train_fwd. Returns (dz fp16 = s * gradient, dgamma, dbeta, aux=[max|du|, s, 1/s, -])."""
+    """Backward of bn_train_fwd. Returns (dz fp16 = s * gradient, dgamma, dbeta, aux=[max|du|, s, 1/s, max|xhat|]).
+
+    aux is the 4-float row the reduce and apply kernels share: the reduce writes max|du| and max|xhat| with atomicMax
+    into the zeroed row, and the apply derives the power of two s from them so that max|dz * s| <= 2^12."""
     B, H, W, Cc = z.shape
     dev = z.device
     n = B * H * W

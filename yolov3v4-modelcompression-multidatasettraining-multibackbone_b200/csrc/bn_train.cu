@@ -154,7 +154,7 @@ bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT*
     const int C = CV * 8;
     const bool active = tid < CV * PPB;
     const int cv = active ? tid % CV : 0, prow = tid / CV;
-    float sc[8], sh[8], mu[8], a1[8], a2[8];
+    float sc[8], sh[8], mu[8], a1[8], a2[8], dmax[8];   // dmax: max |z - mean| per channel
     float amax = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -162,7 +162,7 @@ bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT*
         mu[j] = __ldg(save + c);
         sc[j] = __ldg(save + 2 * C + c);
         sh[j] = __ldg(save + 3 * C + c);
-        a1[j] = a2[j] = 0.f;
+        a1[j] = a2[j] = dmax[j] = 0.f;
     }
     const long long stride = (long long)gridDim.x * PPB;
     if (active) {
@@ -191,18 +191,28 @@ bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT*
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         const float du = gf[j] * actg<ACT>(fmaf(xf[j], sc[j], sh[j]), act_rt, slope);
+                        const float d = xf[j] - mu[j];
                         a1[j] += du;
-                        a2[j] = fmaf(du, xf[j] - mu[j], a2[j]);
+                        a2[j] = fmaf(du, d, a2[j]);
                         amax = fmaxf(amax, fabsf(du));
+                        dmax[j] = fmaxf(dmax[j], fabsf(d));
                     }
                 }
             }
         }
     }
-    if (du_absmax != nullptr) {   // non-negative floats order like their bit patterns
+    if (du_absmax != nullptr) {   // [0] max|du|, [3] max|xhat|: non-negative floats order like their bit patterns
+        float xmax = 0.f;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+        for (int j = 0; j < 8; ++j) xmax = fmaxf(xmax, dmax[j] * __ldg(save + C + cv * 8 + j));
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+            xmax = fmaxf(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
+        }
         if ((tid & 31) == 0 && amax > 0.f) atomicMax(reinterpret_cast<unsigned int*>(du_absmax), __float_as_uint(amax));
+        if ((tid & 31) == 0 && xmax > 0.f)
+            atomicMax(reinterpret_cast<unsigned int*>(du_absmax + 3), __float_as_uint(xmax));
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -226,7 +236,8 @@ bn_train_bwd_reduce_kernel(const __half* __restrict__ z, long long zp, const GT*
 // dz = A*du + Bx*z + Cc   with  A = s*gamma*invstd, Bx = -A*invstd*S2/N, Cc = A*(-S1/N + mean*invstd*S2/N)
 // The data gradient dz feeds two tensor-core GEMMs whose operands share one 16-bit format with the fp16 activations /
 // weights, so it is written in fp16 times a per-layer power of two s derived on the device from a bound on max|dz|
-// (no host sync); the GEMM epilogues multiply by 1/s (scale_out[1]) read from device memory.
+// (no host sync); the GEMM epilogues multiply by 1/s (scale_out[1]) read from device memory.  du_absmax holds the
+// reduce's [max|du|, -, -, max|xhat|] (scale_out is its slots 1 and 2 in the training plan).
 template <typename GT, int ACT, int U>
 __global__ void __launch_bounds__(256, 2)
 bn_train_bwd_apply_kernel(const __half* __restrict__ z, long long zp, const GT* __restrict__ dy, long long dp,
@@ -242,12 +253,15 @@ bn_train_bwd_apply_kernel(const __half* __restrict__ z, long long zp, const GT* 
     const float inv_n = 1.f / (float)pixels;
     __shared__ float s_red[8];
     __shared__ float s_scale;
-    {   // every CTA derives the same scale: bound = max_c |gamma_c*invstd_c| * (max|du| + |S1_c|/N + 16*|S2_c|/N)
+    {   // every CTA derives the same scale from a bound on max|dz|, since |xhat| <= max|xhat|:
+        //   bound = max_c |gamma_c*invstd_c| * (max|du| + |S1_c|/N + max|xhat| * |S2_c|/N)
+        // Without the reduce's maxima, max|du| is taken as 1 and max|xhat| as sqrt(N) (sum xhat^2 <= N).
         float bound = 0.f;
-        const float dumax = du_absmax != nullptr ? *du_absmax : 1.f;
+        const float dumax = du_absmax != nullptr ? du_absmax[0] : 1.f;
+        const float xhmax = du_absmax != nullptr ? du_absmax[3] : sqrtf((float)pixels);
         for (int c = tid; c < C; c += 256) {
             const float g = gamma != nullptr ? gamma[c] : 1.f;
-            const float b = fabsf(g * save[C + c]) * (dumax + fabsf(sums[c]) * inv_n + 16.f * fabsf(sums[C + c]) * inv_n);
+            const float b = fabsf(g * save[C + c]) * (dumax + fabsf(sums[c]) * inv_n + xhmax * fabsf(sums[C + c]) * inv_n);
             bound = fmaxf(bound, b);
             if (blockIdx.x == 0) {
                 if (dbeta_out != nullptr) dbeta_out[c] = sums[c] * grad_out_scale;
