@@ -108,20 +108,26 @@ int b2y_conv2d_fwd_stats(const b2y_conv_desc* d, const void* x, const void* w_pa
 int b2y_stem_conv_fwd(const b2y_conv_desc* d, const float* x_nchw, const float* w, const float* bias, void* y,
                       void* stream);
 
-/* Tensor-core stem (in_c*ksize <= 16): the image is re-laid as NHWC fp16 with the kw taps unrolled into 16 channels
- * (workspace, b2y_stem_workspace_bytes), then the conv runs as a k x 1 implicit GEMM on the wgmma kernel.
- *   w_stem fp16 [out_c][k][16] from b2y_pack_stem_weights (w already BN-folded, OIHW fp32)
+/* The first layer's tensor-core paths take the (in_c, ksize) pairs with odd ksize and in_c*ksize*ksize <= 32, so
+ * that one output pixel's receptive field is one 32-column fp16 GEMM row (B2Y_STEM_IM2COL_SHAPES in csrc/common.cuh;
+ * other pairs return B2Y_ERR_UNSUPPORTED and run on b2y_stem_conv_fwd).  The plans choose (b200yolo/layout.py,
+ * stem_path): inference takes b2y_stem_conv_fwd_fused when out_c <= 64, else b2y_stem_conv_fwd_tc; training takes
+ * b2y_stem_conv_fwd_tc for a stem with BatchNorm, whose weight gradient then runs as a GEMM over the same workspace.
+ *
+ * im2col stem: the image is written as the im2col matrix [batch*out_h*out_w][32] fp16 (workspace,
+ * b2y_stem_workspace_bytes, 0 for a pair off the list), then the conv runs as one k-step GEMM on the wgmma kernel.
+ *   w_stem fp16 [out_c][32] from b2y_pack_stem_weights (w already BN-folded, OIHW fp32), column (kh*k + kw)*in_c + c
  *   stat_sum/stat_sqsum optional (training BN statistics, see b2y_conv2d_fwd_stats) */
 size_t b2y_stem_workspace_bytes(const b2y_conv_desc* d);
 int b2y_pack_stem_weights(const float* w_oihw_folded, int out_c, int in_c, int ksize, void* w_stem, void* stream);
 int b2y_stem_conv_fwd_tc(const b2y_conv_desc* d, const float* x_nchw, const void* w_stem, const float* bias,
                          void* workspace, void* y, float* stat_sum, float* stat_sqsum, void* stream);
 
-/* Fused tensor-core stem (in_c*ksize*ksize <= 32, out_c <= 64): the CTA builds the im2col tile in shared memory
+/* Fused tensor-core stem (the pairs above, out_c <= 64): the CTA builds the im2col tile in shared memory
  * straight from the image and feeds wgmma, so only the image is read and only y is written (no workspace).
  *   x_nchw   NCHW image, x_dtype = B2Y_STEM_X_F32 / _F16 / _U8; value = raw / x_div
  *            (x_div = 256 for uint8 images: reference test.py:95, train.py:348, detect.py:101 "/ 256.0")
- *   w_stem   fp16 [out_c][32] from b2y_pack_stem_weights (the layout it produces when in_c*k*k <= 32)
+ *   w_stem   fp16 [out_c][32] from b2y_pack_stem_weights
  *   y        NHWC fp16 */
 #define B2Y_STEM_X_F32 0
 #define B2Y_STEM_X_F16 1
@@ -300,7 +306,7 @@ int b2y_upsample_nearest_bwd(const void* dy, long long dy_pitch, void* dx, long 
 int b2y_maxpool_bwd(const void* x, long long x_pitch, const void* dy, long long dy_pitch, void* dx,
                     long long dx_pitch, int batch, int in_h, int in_w, int c, int ksize, int stride, int pad_mode,
                     int grad_dtype, void* stream);
-/* weight gradient of the stem (in_c <= 4): x fp32 NCHW, dz fp16 NHWC -> dw OIHW fp32 (+= scale * ...) */
+/* weight gradient of the stem (in_c <= 4, in_c*ksize*ksize <= 40): x fp32 NCHW, dz fp16 NHWC -> dw OIHW fp32 (+= scale * ...) */
 int b2y_stem_conv_bwd_weight(const b2y_conv_desc* d, const float* x_nchw, const void* dz, float* dw_oihw,
                              float scale, int grad_dtype, void* stream);
 

@@ -61,3 +61,43 @@ def anchor_vecs(name):
     ys = [d for d in defs if d['type'] == 'yolo']
     strides = orc.yolo_strides(name, len(ys))
     return [torch.as_tensor(np.asarray(d['anchors'])[d['mask']], dtype=torch.float32) / s for d, s in zip(ys, strides)]
+
+
+STEM_CFG = """[net]
+width=64
+height=64
+channels=3
+
+[convolutional]
+batch_normalize=1
+filters=%d
+size=%d
+stride=%d
+pad=1
+activation=leaky
+
+[convolutional]
+size=1
+stride=1
+pad=1
+filters=18
+activation=linear
+
+[yolo]
+mask=0,1,2
+anchors=10,14,23,27,37,58
+classes=1
+num=3
+"""
+
+
+def stem_model(in_c, k, stride, filters=32, seed=0, device=None):
+    """A first-layer conv (k x k, stride, BatchNorm, leaky) on in_c input channels and a one-class YOLO head behind a
+    1x1 conv, with the synthetic parameters of oracle.synth_state_dict.  The cfg format fixes 3 input channels, so the
+    first conv is replaced by one on in_c."""
+    import models
+    from utils.parse_config import parse_model_cfg_text
+    m = models.Darknet(parse_model_cfg_text(STEM_CFG % (filters, k, stride)))
+    m.module_list[0].Conv2d = torch.nn.Conv2d(in_c, filters, k, stride, (k - 1) // 2, bias=False)
+    m.load_state_dict(orc.synth_state_dict(m.state_dict(), seed))
+    return m if device is None else m.to(device)

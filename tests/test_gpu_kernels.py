@@ -176,11 +176,24 @@ def test_stem_conv():
     ref = F.leaky_relu(F.conv2d(x, w16, None, stride=1, padding=1), 0.1)
     y = ops.stem_conv(x.cuda(), w16.cuda(), None, 3, 1, 1, act="leaky")
     assert (y.float().permute(0, 3, 1, 2).cpu() - ref).abs().max() <= 2e-3 * max(1.0, ref.abs().max().item())
+    # the first layers that no im2col kernel is compiled for (layout.stem_path): 5x5 and 7x7, 4 channels at 3x3, and
+    # 1, 2 and 4 input channels
+    for cin, k, stride, cout in ((3, 5, 1, 32), (1, 7, 1, 32), (2, 5, 2, 64), (4, 3, 1, 32), (4, 7, 2, 16),
+                                 (2, 7, 1, 24), (1, 5, 2, 32)):
+        xk = torch.rand(2, cin, 40, 56, generator=g)
+        wk = torch.randn(cout, cin, k, k, generator=g) / (cin * k)
+        bk = torch.randn(cout, generator=g)
+        ref = F.leaky_relu(F.conv2d(xk, wk, bk, stride=stride, padding=k // 2), 0.1)
+        y = ops.stem_conv(xk.cuda(), wk.cuda(), bk.cuda(), k, stride, k // 2, act="leaky")
+        got = y.float().permute(0, 3, 1, 2).cpu()
+        assert got.shape == ref.shape
+        assert (got - ref).abs().max() <= 2e-3 * max(1.0, ref.abs().max().item()), (cin, k, stride, cout)
 
 
-@pytest.mark.parametrize("cin,k,stride,cout", [(3, 3, 1, 32), (3, 3, 2, 32), (3, 3, 1, 16), (1, 5, 1, 32), (3, 5, 1, 32)])
+@pytest.mark.parametrize("cin,k,stride,cout", [(3, 3, 1, 32), (3, 3, 2, 32), (3, 3, 1, 16), (1, 5, 1, 32), (2, 3, 1, 32),
+                                             (4, 1, 2, 72)])
 def test_stem_conv_tensor_core(cin, k, stride, cout):
-    """Both tensor-core stem layouts: full im2col row (cin*k*k <= 32) and one row per kernel row (cin*k <= 16)."""
+    """im2col workspace + GEMM stem: one 32-column im2col row per output pixel (B2Y_STEM_IM2COL_SHAPES)."""
     ops = _ops()
     g = torch.Generator().manual_seed(11)
     x = torch.rand(2, cin, 40, 56, generator=g)
@@ -197,7 +210,7 @@ def test_stem_conv_tensor_core(cin, k, stride, cout):
 
 @pytest.mark.parametrize("cin,k,stride,cout,dtype", [
     (3, 3, 1, 32, "f32"), (3, 3, 2, 32, "f16"), (3, 3, 1, 16, "u8"), (1, 5, 1, 32, "f32"), (3, 3, 1, 64, "u8256"),
-    (3, 3, 1, 48, "f32")])
+    (3, 3, 1, 48, "f32"), (2, 3, 1, 32, "f32"), (4, 1, 2, 64, "f16")])
 def test_stem_conv_fused(cin, k, stride, cout, dtype):
     """Fused stem: the CTA builds the im2col tile in smem from the NCHW image (fp32 / fp16 / uint8 with /255)."""
     ops = _ops()

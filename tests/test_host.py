@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GOLD, PKG, ROOT, cfg_path, module_defs, orc
+from helpers import GOLD, PKG, ROOT, cfg_path, module_defs, orc, stem_model
 
 def _snapshot():
     with open(os.path.join(GOLD, "cfg_snapshot.json")) as f:
@@ -244,6 +244,42 @@ def test_layout_is_decided_once_for_inference_and_training():
     with pytest.raises(NotImplementedError, match="int8 graph"):
         layout.infer_shapes(models.Darknet(cfg_path("yolov3-tiny")), (3, 96, 96), ('convolutional', 'yolo'),
                             "layer type '%s' in the int8 graph")
+
+
+def test_stem_path_follows_the_compiled_shape_list():
+    """layout.stem_path picks an im2col kernel only for an (in_c, k) pair that csrc/common.cuh compiles them for, and
+    the training plans record its choice; the gradient plan refuses, naming the layer, every first layer whose direct
+    weight gradient b2y_stem_conv_bwd_weight cannot take (more than 40 taps)."""
+    from b200yolo import layout
+    from b200yolo.engine import SlotStore
+    from b200yolo.train_engine import TrainPlan, TrainShared
+    with open(os.path.join(PKG, "csrc", "common.cuh")) as f:
+        line = re.search(r"#define B2Y_STEM_IM2COL_SHAPES\(X\)(.*)", f.read()).group(1)
+    listed = {(int(c), int(k)) for c, k in re.findall(r"X\((\d+), (\d+)\)", line)}
+    assert (3, 3) in listed and (1, 3) in listed
+    dev = torch.device("cpu")
+    for in_c in range(1, 5):
+        for k in range(1, 8):
+            on_list = (in_c, k) in listed
+            for out_c in (16, 32, 64, 72, 256):
+                want = ('fused' if out_c <= 64 else 'im2col') if on_list else 'direct'
+                assert layout.stem_path(in_c, k, out_c) == want, (in_c, k, out_c)
+                assert layout.stem_path(in_c, k, out_c, training=True) == ('im2col' if on_list else 'direct')
+                assert layout.stem_path(in_c, k, out_c, training=True, batch_norm=False) == 'direct'
+            for stride in (1, 2):
+                model = stem_model(in_c, k, stride).train()
+                shape = (2, in_c, 40, 48)
+                fo = TrainPlan(model, shape, dev, False, SlotStore(dev), TrainShared(dev), forward_only=True)
+                assert fo.convs[0].stem == ('im2col' if on_list else 'direct')
+                if fo.convs[0].stem == 'direct' and in_c * k * k > layout.STEM_WGRAD_MAX_TAPS:
+                    with pytest.raises(NotImplementedError, match="layer 0: the weight gradient of a %dx%d first "
+                                                                  "layer on %d channels" % (k, k, in_c)):
+                        TrainPlan(model, shape, dev, False, SlotStore(dev), TrainShared(dev))
+                else:
+                    plan = TrainPlan(model, shape, dev, False, SlotStore(dev), TrainShared(dev))
+                    assert plan.convs[0].stem == fo.convs[0].stem
+    with pytest.raises(NotImplementedError, match="more than 4 input channels"):
+        layout.stem_path(5, 3, 32)
 
 
 @pytest.mark.parametrize("name", ["yolov3", "yolov3-tiny", "yolov4", "yolov3-mobilenet"])

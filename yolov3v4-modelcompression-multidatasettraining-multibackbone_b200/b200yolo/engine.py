@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .layout import _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources
+from .layout import _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources, stem_path
 from .lib import WLAYOUT_S2_PAIRS
 
 
@@ -220,11 +220,6 @@ class Plan:
     def _w(self, i):
         return self.shared_weights.packs[self.wkey[i]]
 
-    def _stem_workspace(self, conv):
-        d = ops.make_conv_desc((self.B, self.H, self.W, conv.in_channels), conv.in_channels, conv.out_channels,
-                               conv.kernel_size[0], conv.stride[0], conv.padding[0], conv.out_channels)
-        return self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,))
-
     # ---------------------------------------------------------------------------------------------------------
     def _build(self):
         model, B = self.model, self.B
@@ -280,6 +275,13 @@ class Plan:
                 if i + 1 < n and fused_into[i + 1] == i:
                     res = tens[sources(i + 1, defs[i + 1]['from'])[0]]
                 src = None if i == 0 else tens[i - 1]
+                if src is None:
+                    k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+                    self.stem = stem_path(conv.in_channels, k, out.Cp)
+                    if self.stem == 'im2col':
+                        d = ops.make_conv_desc((B, self.H, self.W, conv.in_channels), conv.in_channels, out.Cp, k, s,
+                                               p, out.Cp)
+                        self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,))
                 self.steps.append(ConvStep('conv', i, src, out, res, conv, bn, act, slope))
             elif t == 'yolo':
                 raw = tens[i - 1]
@@ -359,10 +361,7 @@ class Plan:
                 bnp_p = None if bnp is None else tuple(_pad_rows(t, cp, f) for t, f in zip(bnp, (0.0, 0.0, 0.0, 1.0)))
                 wp, bias, w32 = ops.pack_conv_weights(wsrc, _pad_rows(conv.bias.detach(), cp) if conv.bias is not None
                                                       else None, bnp_p, eps, want_fp32=stem)
-                wstem = None
-                if stem and (conv.in_channels * conv.kernel_size[0] <= 16 or
-                             conv.in_channels * conv.kernel_size[0] ** 2 <= 32):
-                    wstem = ops.pack_stem_weights(w32)
+                wstem = ops.pack_stem_weights(w32) if stem and self.stem != 'direct' else None
                 base = packs[(i, 'base')] = (wp, bias, w32, wstem)
             if layout == 'pair':
                 packs[key] = base + (self._pair_pack(conv, bnp, eps),)
@@ -414,18 +413,14 @@ class Plan:
         layout = self.wkey[st.i][1]
         k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         if src is None:
-            if conv.in_channels > 4:
-                raise NotImplementedError("first layer with more than 4 input channels")
-            if wstem is not None and wstem.dim() == 2 and out.Cp <= 64:
-                # full-im2col weight layout: the fused kernel builds the A tile in smem (no workspace)
+            if self.stem == 'fused':
+                # the fused kernel builds the im2col tile in smem (no workspace)
                 ops.stem_conv_fused(x, wstem, bias, k, s, p, act=act, slope=slope, out=out.view(),
                                     x_div=256.0 if x.dtype == torch.uint8 else 1.0)
                 return
             if x.dtype != torch.float32:
                 x = x.float() / 256.0 if x.dtype == torch.uint8 else x.float()
-            if wstem is not None:
-                if getattr(self, 'stem_ws', None) is None:
-                    self.stem_ws = self._stem_workspace(conv)
+            if self.stem == 'im2col':
                 ops.stem_conv_tc(x, wstem, bias, conv.in_channels, k, s, p, act=act, slope=slope,
                                  out=out.view(), workspace=self.stem_ws)
             else:

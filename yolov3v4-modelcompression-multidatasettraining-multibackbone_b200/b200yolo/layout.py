@@ -70,6 +70,30 @@ def pitch(C, dtype):
     return (C + g - 1) // g * g
 
 
+STEM_WGRAD_MAX_TAPS = 40    # b2y_stem_conv_bwd_weight: 8 tap groups of 5 taps per output channel
+
+
+def stem_path(in_c, k, out_c, training=False, batch_norm=True):
+    """Kernel path of the first convolution, which reads the NCHW image (include/b200yolo.h, b2y_pack_stem_weights).
+
+    'fused'   b2y_stem_conv_fwd_fused: the im2col tile built in shared memory, inference with out_c <= 64
+    'im2col'  b2y_stem_conv_fwd_tc: the im2col matrix written to a workspace, then one GEMM, for wider inference
+              outputs; in training its epilogue gives the BatchNorm batch sums and the workspace feeds the weight
+              gradient, so a stem without BatchNorm (bias and activation in the direct kernel) stays direct
+    'direct'  b2y_stem_conv_fwd (and b2y_stem_conv_bwd_weight) on CUDA cores, any k
+
+    The two im2col kernels are compiled for the (in_c, k) pairs with odd k and in_c * k * k <= 32 (one output pixel's
+    receptive field fits one 32-column fp16 GEMM row), the list B2Y_STEM_IM2COL_SHAPES of csrc/common.cuh.  out_c is
+    the width the stem writes (its physical width in the plans)."""
+    if in_c > 4:
+        raise NotImplementedError("first layer with more than 4 input channels")
+    if k % 2 == 0 or in_c * k * k > 32:
+        return 'direct'
+    if training:
+        return 'im2col' if batch_norm else 'direct'
+    return 'fused' if out_c <= 64 else 'im2col'
+
+
 def sources(i, rel):
     """Absolute layer indices of the `layers=` / `from=` list of layer i (negative entries are relative to i)."""
     return [i + l if l < 0 else l for l in rel]

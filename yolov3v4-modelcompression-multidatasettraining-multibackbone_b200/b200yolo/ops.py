@@ -127,11 +127,11 @@ def stem_conv(x_nchw, w_oihw, bias, k, stride, pad, act="linear", slope=0.1, out
 
 
 def pack_stem_weights(w_oihw_folded, out=None):
+    """OIHW fp32 -> the [O][32] fp16 im2col rows of both tensor-core stems (layout.stem_path)."""
     O, I, k, _ = w_oihw_folded.shape
-    shape = (O, 32) if I * k * k <= 32 else (O, k, 16)     # full-im2col row vs one row per kernel row (conv_tc.cu)
     if out is None:
-        out = torch.empty(shape, dtype=torch.float16, device=w_oihw_folded.device)
-    assert out.shape == shape and out.dtype == torch.float16 and out.is_contiguous()
+        out = torch.empty((O, 32), dtype=torch.float16, device=w_oihw_folded.device)
+    assert out.shape == (O, 32) and out.dtype == torch.float16 and out.is_contiguous()
     call("b2y_pack_stem_weights", ptr(w_oihw_folded.contiguous().float()), O, I, k, ptr(out), stream_ptr())
     return out
 
@@ -147,7 +147,7 @@ def stem_workspace(desc, device):
 
 def stem_conv_tc(x_nchw, w_stem, bias, in_c, k, stride, pad, act="linear", slope=0.1, out=None, workspace=None,
                  stats=None):
-    """Tensor-core stem: NCHW fp32 image -> NHWC fp16 (in_c*k*k <= 32 or k*in_c <= 16). Returns (out, workspace)."""
+    """im2col workspace + GEMM stem: NCHW fp32 image -> NHWC fp16 (layout.stem_path). Returns (out, workspace)."""
     B, Cin, H, W = x_nchw.shape
     O = w_stem.shape[0]
     Ho, Wo = conv_out_hw(H, W, k, stride, pad)
@@ -165,7 +165,7 @@ STEM_X = {torch.float32: 0, torch.float16: 1, torch.uint8: 2}
 
 
 def stem_conv_fused(x_nchw, w_stem, bias, k, stride, pad, act="linear", slope=0.1, out=None, x_div=1.0):
-    """Fused tensor-core stem (in_c*k*k <= 32): NCHW fp32/fp16/uint8 image -> NHWC fp16, no workspace."""
+    """Fused tensor-core stem (layout.stem_path): NCHW fp32/fp16/uint8 image -> NHWC fp16, no workspace."""
     _require_cuda(x_nchw)
     B, Cin, H, W = x_nchw.shape
     O = w_stem.shape[0]

@@ -18,7 +18,7 @@ import os
 import torch
 
 from . import ops
-from .layout import _Tensor, infer_shapes, sources
+from .layout import _Tensor, infer_shapes, sources, stem_path
 from .lib import OUT_F32, OUT_I8, WLAYOUT_S2_PAIRS, B2YError, call, ptr, stream_ptr
 
 
@@ -73,6 +73,8 @@ class QPlan:
                 if not head and Cc % 16 != 0:
                     raise NotImplementedError("layer %d: int8 graph needs channel counts that are multiples of 16 "
                                               "(got %d)" % (i, Cc))
+                if i == 0:
+                    self.stem_fused = stem_path(self.Cin, conv.kernel_size[0], Cc) == 'fused'
                 self.steps.append(('conv', i, None if i == 0 else tens[i - 1], out, conv, head))
                 tens[i] = out
             elif t == 'shortcut':
@@ -238,7 +240,7 @@ class QPlan:
                     ws = self.stem_w.get(i)
                     if ws is None:
                         # fused tensor-core stem when the fake-quantised weights (int8 code x 2^-n) are exact in fp16
-                        fits = self.Cin * k * k <= 32 and conv.out_channels <= 64 and float(wq.abs().max()) < 6.0e4
+                        fits = self.stem_fused and float(wq.abs().max()) < 6.0e4
                         ws = self.stem_w[i] = ops.pack_stem_weights(wq) if fits else False
                     if ws is not False:
                         call("b2y_stem_conv_fwd_fused_q", C.byref(d), ptr(x), 0, 1.0, ptr(ws), ptr(bq), ptr(out.buf), s_a,

@@ -25,7 +25,8 @@ import torch.nn as nn
 
 from . import ops
 from .engine import LazyFeatures, SlotStore, _pad_rows, launch_pointwise, pointwise_steps
-from .layout import _Tensor, _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources
+from .layout import (STEM_WGRAD_MAX_TAPS, _Tensor, _block_parts, build_layout, feature_slots, infer_shapes, pitch,
+                     sources, stem_path)
 from .lib import ACT, ConvDesc, OUT_F16, call, ptr, stream_ptr
 
 GDT = torch.bfloat16   # gradient tensors: bf16 (range of fp32) -- fp16 over/underflows across ~100 BN layers
@@ -54,6 +55,8 @@ def _widen(view, channels):
 
 
 class _ConvRec:
+    """stem: None, or the first layer's path (layout.stem_path), which runs both its forward and its weight gradient:
+    'im2col' as GEMMs over one im2col workspace, 'direct' on CUDA cores."""
     __slots__ = ('i', 'conv', 'bn', 'act', 'slope', 'src', 'z', 'y', 'res', 'head', 'stem', 'k', 's', 'p', 'Cout',
                  'Cpad', 'w16', 'wT', 'stats', 'ones', 'zeros', 'w32', 'aux_row', 'wstem', 'save', 'sums', 'dw',
                  'depthwise', 'Ipad', 'dwg', 'col_map', 'wdw', 'cidx')
@@ -228,9 +231,9 @@ class TrainPlan:
                     raise NotImplementedError("grouped convolution is not supported by the sm_90a engine yet")
                 r.i, r.conv, r.bn, r.act, r.slope = i, conv, bn, act, slope
                 r.k, r.s, r.p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-                r.head, r.stem = is_head[i], (i == 0)
-                if r.stem and conv.in_channels > 4:
-                    raise NotImplementedError("first layer with more than 4 input channels")
+                r.head = is_head[i]
+                r.stem = stem_path(conv.in_channels, r.k, None, training=True, batch_norm=bn is not None) \
+                    if i == 0 else None
                 r.Cout = conv.out_channels
                 # GEMM K granules: the output rows of the packed weights, and the forward GEMM's K: the source's physical
                 # width up to the MMA K granule (_Tensor.view_k)
@@ -312,7 +315,7 @@ class TrainPlan:
         # on first use, so that a larger shape grows every slot while its plan is built
         self.static_x = self._take(('x',), (B, self.Cin, self.H, self.W), torch.float32)
         st = self.convs[0]
-        if st.stem and st.bn is not None and not st.head and st.conv.in_channels * st.k * st.k <= 32:
+        if st.stem == 'im2col':
             d = ops.make_conv_desc((B, self.H, self.W, st.conv.in_channels), st.conv.in_channels, st.y.Cp, st.k, st.s,
                                    st.p, st.y.Cp)
             self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,), torch.float16)
@@ -335,6 +338,12 @@ class TrainPlan:
         """The state only a plan with a backward holds: the gradient mirror of the activations, the backward arena, each
         BatchNorm layer's own z and saved statistics, dz, and the data-gradient weight slabs."""
         B, dev, lay = self.B, self.device, self.layout
+        for r in self.convs:
+            taps = r.conv.in_channels * r.k * r.k
+            if r.stem == 'direct' and taps > STEM_WGRAD_MAX_TAPS:
+                raise NotImplementedError("layer %d: the weight gradient of a %dx%d first layer on %d channels (%d taps; "
+                                          "the direct kernel takes at most %d)" % (r.i, r.k, r.k, r.conv.in_channels,
+                                                                                   taps, STEM_WGRAD_MAX_TAPS))
         self.grad_of = {}  # id(_Tensor) -> gradient _Tensor (bf16, same placement)
 
         def make_grad(t, gbuf, c0=0):
@@ -459,15 +468,12 @@ class TrainPlan:
             if r.stem:
                 # one row per channel of the output it writes
                 r.w32 = _pad_rows(r.conv.weight.detach().float(), self._zview(r).shape[3]).contiguous()
-                # tensor-core stem: full-im2col weight layout when the receptive field fits one 64-byte GEMM row
-                if r.conv.in_channels * r.k * r.k <= 32 and not r.head:
+                if r.stem == 'im2col':
                     key = self._key(r.i)
                     if key not in self.shared.wstem:
                         self.shared.wstem[key] = torch.empty((r.w32.shape[0], 32), dtype=torch.float16,
                                                              device=self.device)
                     r.wstem = ops.pack_stem_weights(r.w32, out=self.shared.wstem[key])
-                else:
-                    r.wstem = None
             elif r.wdw is not None:
                 r.wdw.index_copy_(0, r.cidx, r.conv.weight.detach())
         for st in self.order:
@@ -663,7 +669,7 @@ class TrainPlan:
                 ops.conv2d(r.src.view_k(), r.w16, bias, r.k, r.s, r.p, act=r.act, slope=r.slope, out=out)
             return
         z = r.z.view()
-        if r.stem and getattr(r, 'wstem', None) is not None:
+        if r.stem == 'im2col':
             # im2col workspace [B*Ho*Wo][32] fp16 (kept for the weight gradient) + one-k-step GEMM with the BN sums
             # coming out of its epilogue
             ops.stem_conv_tc(x, r.wstem, None, r.conv.in_channels, r.k, r.s, r.p, act='linear', out=z,
@@ -805,7 +811,7 @@ class TrainPlan:
                 ops.bias_act_bwd_reduce(dz, dz, r.ones, r.zeros, 'linear', dbeta=db)
                 self._emit(grads, conv.bias, db[:r.Cout] * inv_s, inv)
         I = conv.in_channels
-        if r.stem and getattr(r, 'wstem', None) is not None and getattr(self, 'stem_ws', None) is not None:
+        if r.stem == 'im2col':
             # dW = dz^T . im2col(x): the pixel-dimension GEMM on the tensor cores over the forward's workspace
             gw = self._grad_dst(conv.weight)
             kk = I * r.k * r.k

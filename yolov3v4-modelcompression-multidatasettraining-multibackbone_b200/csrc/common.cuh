@@ -10,6 +10,11 @@
 #include "b200yolo.h"  // status codes + activation ids (single source of truth)
 #include "wgmma.cuh"
 
+// (in_c, k) pairs of the first layer's two im2col kernels, stem_fused_kernel (stem_tc.cu) and stem_fullpack_kernel
+// (conv_tc.cu): odd k and in_c * k * k <= 32, so that one output pixel's receptive field fits one 32-column fp16 GEMM
+// row.  Each kernel's dispatch expands X(in_c, k) over this list; layout.stem_path states the same rule in Python.
+#define B2Y_STEM_IM2COL_SHAPES(X) X(1, 1) X(2, 1) X(3, 1) X(4, 1) X(1, 3) X(2, 3) X(3, 3) X(1, 5)
+
 namespace b2y {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

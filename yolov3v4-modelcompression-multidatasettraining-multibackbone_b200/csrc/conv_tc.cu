@@ -610,64 +610,10 @@ extern "C" int b2y_conv2d_bwd_data(const b2y_conv_desc* d, const void* dy, const
 
 
 // ---- tensor-core stem ------------------------------------------------------------------------------------------
-// The image (NCHW fp32, Cin <= 4) is first re-laid as NHWC fp16 with the kw taps unrolled into the channel dim:
-//   packed[n][y][x][kw*Cin + c] = x[n][c][y][x + kw - pad]   (16 "channels", zero padded)
-// so that the conv becomes a k x 1 implicit GEMM with K = 16 per tap row on the same wgmma kernel.
-template <int CIN, int K>
-__global__ void stem_pack_kernel(const float* __restrict__ x, __half* __restrict__ out, int B, int H, int W,
-                                 int pad) {
-    // one thread per pixel; all indices static so the 16-entry row lives in registers
-    const long long total = (long long)B * H * W;
-    const long long plane = (long long)H * W;
-    for (long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x; pix < total;
-         pix += (long long)gridDim.x * blockDim.x) {
-        const int xo = (int)(pix % W);
-        const long long n = pix / plane;
-        const long long in_plane = pix - n * plane;     // yo*W + xo
-        const float* xb = x + n * CIN * plane + in_plane;
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0.f;
-#pragma unroll
-        for (int kw = 0; kw < K; ++kw) {
-            const int xi = xo + kw - pad;
-            if (xi >= 0 && xi < W) {
-#pragma unroll
-                for (int c = 0; c < CIN; ++c) v[kw * CIN + c] = __ldg(xb + c * plane + (kw - pad));
-            }
-        }
-        uint4 o[2];
-        __half2* oh = reinterpret_cast<__half2*>(o);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) oh[j] = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-        uint4* op = reinterpret_cast<uint4*>(out + pix * 16);
-        op[0] = o[0];
-        op[1] = o[1];
-    }
-}
-
-// w (OIHW fp32, BN folded by the caller) -> [O][kh][16] fp16 with inner index kw*Cin + c
-__global__ void stem_pack_weights_kernel(const float* __restrict__ w, __half* __restrict__ out, int O, int Cin,
-                                         int k) {
-    const int total = O * k * 16;
-    for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-        const int j = idx % 16;
-        const int r = (idx / 16) % k;
-        const int o = idx / (16 * k);
-        float v = 0.f;
-        if (j < k * Cin) {
-            const int kw = j / Cin, c = j % Cin;
-            v = w[(((long long)o * Cin + c) * k + r) * k + kw];
-        }
-        out[idx] = __float2half_rn(v);
-    }
-}
-
-// Small stems (Cin*k*k <= 32, e.g. 3x3 on RGB = 27): the whole receptive field of one output pixel fits one 64-byte
-// GEMM row, so the pack writes the im2col matrix itself,
+// The first layer (NCHW fp32 image, B2Y_STEM_IM2COL_SHAPES, e.g. 3x3 on RGB = 27 taps): the whole receptive field of
+// one output pixel fits one 64-byte GEMM row, so the pack writes the im2col matrix itself,
 //   packed[n][yo][xo][(kh*K + kw)*Cin + c] = x[n][c][yo*s + kh - pad][xo*s + kw - pad]   (32 columns, zero padded)
-// and the conv is ONE k-step of a plain [M][32] x [32][Cout] GEMM (the 3-tap variant above costs three 32-byte-row
-// TMA gathers per tile and is bound by L2 request rate, not bytes).
+// and the conv is ONE k-step of a plain [M][32] x [32][Cout] GEMM on the wgmma kernel.
 template <int CIN, int K>
 __global__ void stem_fullpack_kernel(const float* __restrict__ x, __half* __restrict__ out, int B, int H, int W,
                                      int Ho, int Wo, int stride, int pad) {
@@ -723,25 +669,23 @@ __global__ void stem_fullpack_weights_kernel(const float* __restrict__ w, __half
     }
 }
 
-static inline bool stem_is_full(int in_c, int ksize) { return in_c * ksize * ksize <= 32; }
+static inline bool stem_im2col_shape(int in_c, int ksize) {
+#define B2Y_STEM_IS(CI, KK) if (in_c == CI && ksize == KK) return true;
+    B2Y_STEM_IM2COL_SHAPES(B2Y_STEM_IS)
+#undef B2Y_STEM_IS
+    return false;
+}
 
 extern "C" size_t b2y_stem_workspace_bytes(const b2y_conv_desc* d) {
-    if (!d) return 0;
-    if (stem_is_full(d->in_c, d->ksize)) return (size_t)d->batch * d->out_h * d->out_w * 32 * sizeof(__half);
-    return (size_t)d->batch * d->in_h * d->in_w * 16 * sizeof(__half);
+    if (!d || !stem_im2col_shape(d->in_c, d->ksize)) return 0;
+    return (size_t)d->batch * d->out_h * d->out_w * 32 * sizeof(__half);
 }
 
 extern "C" int b2y_pack_stem_weights(const float* w_oihw_folded, int out_c, int in_c, int ksize, void* w_stem,
                                      void* stream) {
     if (!w_oihw_folded || !w_stem) return B2Y_ERR_INVALID;
-    if (stem_is_full(in_c, ksize)) {
-        stem_fullpack_weights_kernel<<<(out_c * 32 + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-            w_oihw_folded, reinterpret_cast<__half*>(w_stem), out_c, in_c, ksize);
-        B2Y_CUDA_CHECK(cudaGetLastError());
-        return B2Y_OK;
-    }
-    if (in_c * ksize > 16) return B2Y_ERR_INVALID;
-    stem_pack_weights_kernel<<<(out_c * ksize * 16 + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    if (!stem_im2col_shape(in_c, ksize)) return B2Y_ERR_UNSUPPORTED;
+    stem_fullpack_weights_kernel<<<(out_c * 32 + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         w_oihw_folded, reinterpret_cast<__half*>(w_stem), out_c, in_c, ksize);
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;
@@ -754,78 +698,30 @@ extern "C" int b2y_stem_conv_fwd_tc(const b2y_conv_desc* d, const float* x_nchw,
     const int Wo = (d->in_w + 2 * d->pad - d->ksize) / d->stride + 1;
     if (Ho != d->out_h || Wo != d->out_w) return B2Y_ERR_INVALID;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (stem_is_full(d->in_c, d->ksize)) {
-        const long long opix = (long long)d->batch * Ho * Wo;
-        int fgrid = (int)((opix + 127) / 128);
-        if (fgrid > 132 * 64) fgrid = 132 * 64;
-        __half* fws = reinterpret_cast<__half*>(workspace);
+    const long long opix = (long long)d->batch * Ho * Wo;
+    int fgrid = (int)((opix + 127) / 128);
+    if (fgrid > 132 * 64) fgrid = 132 * 64;
+    __half* fws = reinterpret_cast<__half*>(workspace);
 #define B2Y_STEM_FULL(CI, KK)                                                                                       \
     if (d->in_c == CI && d->ksize == KK) {                                                                          \
         stem_fullpack_kernel<CI, KK><<<fgrid, 128, 0, st>>>(x_nchw, fws, d->batch, d->in_h, d->in_w, Ho, Wo,        \
                                                             d->stride, d->pad);                                     \
     } else
-        B2Y_STEM_FULL(3, 3) B2Y_STEM_FULL(1, 3) B2Y_STEM_FULL(2, 3) B2Y_STEM_FULL(1, 5) B2Y_STEM_FULL(3, 1)
-        B2Y_STEM_FULL(1, 1) B2Y_STEM_FULL(4, 1) B2Y_STEM_FULL(2, 1) { return B2Y_ERR_UNSUPPORTED; }
+    B2Y_STEM_IM2COL_SHAPES(B2Y_STEM_FULL) { return B2Y_ERR_UNSUPPORTED; }
 #undef B2Y_STEM_FULL
-        B2Y_CUDA_CHECK(cudaGetLastError());
-        GemmConvSpec g;
-        g.kind = CONV_KIND_F16;
-        g.a = workspace;
-        g.N = d->batch;
-        g.H = Ho;
-        g.W = Wo;
-        g.C = 32;
-        g.a_pitch = 32;
-        g.MH = Ho;
-        g.MW = Wo;
-        g.pointwise = true;
-        g.ntaps = 1;
-        g.w = w_stem;
-        g.Nout = d->out_c;
-        EpilogueArgs e;
-        e.bias = bias;
-        e.act = d->act;
-        e.slope = d->slope;
-        e.out = y;
-        e.out_pitch = d->out_pitch;
-        e.out_dtype = OUT_F16;
-        e.stat_sum = stat_sum;
-        e.stat_sqsum = stat_sqsum;
-        return gemm_conv_launch(g, e, st);
-    }
-    if (d->in_c * d->ksize > 16 || d->ksize > 16) return B2Y_ERR_UNSUPPORTED;
-    const long long pixels = (long long)d->batch * d->in_h * d->in_w;
-    int grid = (int)((pixels + 255) / 256);
-    if (grid > 132 * 32) grid = 132 * 32;
-    __half* ws = reinterpret_cast<__half*>(workspace);
-#define B2Y_STEM_PACK(CI, KK)                                                                             \
-    if (d->in_c == CI && d->ksize == KK) {                                                                \
-        stem_pack_kernel<CI, KK><<<grid, 256, 0, st>>>(x_nchw, ws, d->batch, d->in_h, d->in_w, d->pad);   \
-    } else
-    B2Y_STEM_PACK(3, 3) B2Y_STEM_PACK(1, 3) B2Y_STEM_PACK(3, 5) B2Y_STEM_PACK(1, 5) B2Y_STEM_PACK(4, 3)
-    B2Y_STEM_PACK(3, 1) B2Y_STEM_PACK(1, 1) B2Y_STEM_PACK(2, 3) { return B2Y_ERR_UNSUPPORTED; }
-#undef B2Y_STEM_PACK
     B2Y_CUDA_CHECK(cudaGetLastError());
     GemmConvSpec g;
     g.kind = CONV_KIND_F16;
     g.a = workspace;
     g.N = d->batch;
-    g.H = d->in_h;
-    g.W = d->in_w;
-    g.C = 16;
-    g.a_pitch = 16;
+    g.H = Ho;
+    g.W = Wo;
+    g.C = 32;
+    g.a_pitch = 32;
     g.MH = Ho;
     g.MW = Wo;
-    g.stride = d->stride;
-    g.lower_w = 0;            // the kw window is already centred by the pack
-    g.upper_w = 0;
-    g.lower_h = -d->pad;
-    g.upper_h = d->pad - (d->ksize - 1);
-    g.ntaps = d->ksize;
-    for (int r = 0; r < d->ksize; ++r) {
-        g.tap_oh[r] = (unsigned char)r;
-        g.tap_ow[r] = 0;
-    }
+    g.pointwise = true;
+    g.ntaps = 1;
     g.w = w_stem;
     g.Nout = d->out_c;
     EpilogueArgs e;

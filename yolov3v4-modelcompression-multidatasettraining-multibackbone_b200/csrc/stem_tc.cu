@@ -31,7 +31,7 @@ struct StemParams {
     float x_div;          // value = raw / x_div  (256 for uint8 images: reference test.py:95, train.py:348; 1 otherwise)
     float x_mul;          // host: 1/x_div when that multiplication gives the same fp16 as the division, else 0
     int B, H, W, Ho, Wo, stride, pad;
-    const __half* w;      // [BLOCK_N][32] fp16, column (kh*K + kw)*Cin + c  (b2y_pack_stem_weights, full layout)
+    const __half* w;      // [BLOCK_N][32] fp16, column (kh*K + kw)*Cin + c  (b2y_pack_stem_weights)
     const float* bias;    // [Cout] or null
     __half* out;          // NHWC fp16, or int8 codes when out_i8 (first layer of the INT8 graph)
     int out_i8;
@@ -331,7 +331,7 @@ static int stem_dispatch(const StemParams& p, int cin, int k, cudaStream_t st) {
         if (p.Cout <= 32) return stem_launch<XT, CI, KK, 32>(p, st);                           \
         return stem_launch<XT, CI, KK, 64>(p, st);                                             \
     }
-    B2Y_STEM_CASE(3, 3) B2Y_STEM_CASE(1, 3) B2Y_STEM_CASE(1, 5) B2Y_STEM_CASE(3, 1) B2Y_STEM_CASE(1, 1)
+    B2Y_STEM_IM2COL_SHAPES(B2Y_STEM_CASE)
 #undef B2Y_STEM_CASE
     return B2Y_ERR_UNSUPPORTED;
 }
@@ -340,8 +340,8 @@ static int stem_dispatch(const StemParams& p, int cin, int k, cudaStream_t st) {
 
 using namespace b2y;
 
-// x: NCHW image in x_dtype (B2Y_STEM_X_*), value = raw / x_div.  w_stem: the "full" [out_c][32] layout of
-// b2y_pack_stem_weights (in_c*k*k <= 32).  y: NHWC fp16.
+// x: NCHW image in x_dtype (B2Y_STEM_X_*), value = raw / x_div.  w_stem: the [out_c][32] rows of
+// b2y_pack_stem_weights ((in_c, k) in B2Y_STEM_IM2COL_SHAPES).  y: NHWC fp16.
 static int stem_fused_common(const b2y_conv_desc* d, const void* x_nchw, int x_dtype, float x_div, const void* w_stem,
                              const float* bias, void* y, int out_i8, float q_scale, float q_lo, float q_hi, void* stream) {
     if (!d || !x_nchw || !w_stem || !y) return B2Y_ERR_INVALID;
@@ -397,8 +397,8 @@ static int stem_fused_common(const b2y_conv_desc* d, const void* x_nchw, int x_d
     }
 }
 
-// x: NCHW image in x_dtype (B2Y_STEM_X_*), value = raw / x_div.  w_stem: the "full" [out_c][32] layout of
-// b2y_pack_stem_weights (in_c*k*k <= 32).  y: NHWC fp16.
+// x: NCHW image in x_dtype (B2Y_STEM_X_*), value = raw / x_div.  w_stem: the [out_c][32] rows of
+// b2y_pack_stem_weights ((in_c, k) in B2Y_STEM_IM2COL_SHAPES).  y: NHWC fp16.
 extern "C" int b2y_stem_conv_fwd_fused(const b2y_conv_desc* d, const void* x_nchw, int x_dtype, float x_div,
                                        const void* w_stem, const float* bias, void* y, void* stream) {
     return stem_fused_common(d, x_nchw, x_dtype, x_div, w_stem, bias, y, 0, 1.f, 0.f, 0.f, stream);
