@@ -441,6 +441,17 @@ int b2y_dwconv_fwd_f32(const b2y_conv_desc* d, const float* x, const float* w, c
 /* dx = dwconv^T(dz, w) and dw[c][k][k] = sum_pixels dz * x, both overwritten; either may be NULL */
 int b2y_dwconv_bwd_f32(const b2y_conv_desc* d, const float* x, const float* dz, const float* w, float* dx, float* dw,
                        void* stream);
+/* per-channel batch mean and unbiased variance (torch.var) of z = dwconv(x, w) + bias[c] (bias optional), z recomputed,
+ * not stored; sums in double (the statistics conv of a TPSQ depthwise layer, quantized_TPSQ.py:416-420) */
+int b2y_dwconv_stats_f32(const b2y_conv_desc* d, const float* x, const float* w, const float* bias, float* mean,
+                         float* var, void* stream);
+/* backward of those statistics: gs = g_mean[c] / n + 2 g_var[c] (z - mean[c]) / (n - 1) (z recomputed; g_mean / g_var
+ * optional, n = batch * out_h * out_w) into the workspace gs [batch][out_h][out_w][c]; then
+ * dx = dwconv^T(gs, w) + dwconv^T(dz2, w2) in one gather (dz2 / w2 optional: the layer's quantised conv on the same input)
+ * and dw[c][k][k] = sum_pixels gs * x.  dx and dw are overwritten; either may be NULL */
+int b2y_dwconv_stats_bwd_f32(const b2y_conv_desc* d, const float* x, const float* w, const float* bias, const float* mean,
+                             const float* g_mean, const float* g_var, const float* dz2, const float* w2, float* gs,
+                             float* dx, float* dw, void* stream);
 /* ws layout as b2y_se_fwd */
 int b2y_se_fwd_f32(const float* x, const float* w1, const float* w2, float* y, int batch, int hw, int c, int cr, float* ws,
                    void* stream);

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""One google-QAT (quantized=1) training step of yolov3-mobilenet: forward, compute_loss and backward at 416 x 416,
-batch 16, the size train.py --quantized 1 trains MobileNet at.  The QAT graph is data dependent (range trackers, freeze
-steps), so it runs eagerly, layer by layer; the step is timed with CUDA events after --warmup steps.  Weights are the
-synthetic ones of the tests (every tensor whose name the float model shares).
+"""One quantisation-aware training step of yolov3-mobilenet: forward, compute_loss and backward at 416 x 416, batch 16,
+the size train.py trains MobileNet at; --quantized 1 (google QAT, the default) or 2 (TPSQ).  The QAT graph is data
+dependent (range trackers, freeze steps), so it runs eagerly, layer by layer; the step is timed with CUDA events after
+--warmup steps.  Weights are the synthetic ones of the tests (every tensor whose name the float model shares).
 
 Printed (one JSON line): ms per step, images/s, and the card's name and power limit.
 
-    python tools/time_qat_mobilenet.py [--steps 5] [--warmup 2] [--batch 16] [--size 416]
+    python tools/time_qat_mobilenet.py [--quantized 1] [--steps 5] [--warmup 2] [--batch 16] [--size 416]
 """
 import argparse
 import json
@@ -25,6 +25,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--size", type=int, default=416)
+    ap.add_argument("--quantized", type=int, choices=(1, 2), default=1)
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -34,7 +35,8 @@ def main():
     from utils import utils as my_utils
     m = models.Darknet(cfg_path("yolov3-mobilenet"))
     sd = orc.synth_state_dict(m.state_dict(), 0)
-    qm = models.Darknet(cfg_path("yolov3-mobilenet"), quantized=1, a_bit=8, w_bit=8, shortcut_way=1, steps=100)
+    qm = models.Darknet(cfg_path("yolov3-mobilenet"), quantized=args.quantized, a_bit=8, w_bit=8, shortcut_way=1,
+                        steps=100)
     qm.load_state_dict({k: sd.get(k, v) for k, v in qm.state_dict().items()})
     qm = attach_hyp(qm.cuda()).train()
     x = orc.synth_images(args.batch, args.size, args.size, seed=0).cuda()
@@ -56,7 +58,7 @@ def main():
     end.record()
     torch.cuda.synchronize()
     ms = start.elapsed_time(end) / args.steps
-    out = {"model": "yolov3-mobilenet", "quantized": 1, "batch": args.batch, "size": args.size,
+    out = {"model": "yolov3-mobilenet", "quantized": args.quantized, "batch": args.batch, "size": args.size,
            "ms_per_step": round(ms, 2), "images_per_s": round(args.batch * 1000.0 / ms, 1),
            "device": torch.cuda.get_device_name(0)}
     try:

@@ -140,6 +140,8 @@ _PROTOS = {
     "b2y_se_bwd": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, vp, ll, i32, vp, vp, f32, i32, i32, i32, i32, i32, vp]),
     "b2y_dwconv_fwd_f32": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, vp]),
     "b2y_dwconv_bwd_f32": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp]),
+    "b2y_dwconv_stats_f32": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp]),
+    "b2y_dwconv_stats_bwd_f32": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b2y_se_fwd_f32": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp]),
     "b2y_se_bwd_f32": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "b2y_bn_f32_fwd": (i32, [vp, ll, i32, vp, vp, f32, f32, vp, vp, i32, vp, vp, i32, f32, vp]),

@@ -246,6 +246,99 @@ class DepthwiseBlockFn(torch.autograd.Function):
         return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None, None
 
 
+class DwGradLink:
+    """Couples the two depthwise convolutions of a TPSQ layer on one input (quantized_TPSQ.py:404-420, 530-538): the
+    statistics conv with the float weights and the quantised conv with W_q, whose weights are folded from those
+    statistics.  W_q's gradient feeds the variance's gradient through the fold, so the quantised conv's backward runs
+    first and must return dW_q; it leaves its output gradient here instead of computing its data gradient, and the
+    statistics conv's backward adds both data gradients in one gather."""
+
+    def __init__(self):
+        self.gy, self.w = None, None
+
+
+class DwConvFn(torch.autograd.Function):
+    """y = dwconv(x, w) over NHWC fp32 (groups = C).  backward: dw, and dx unless a DwGradLink hands gy to the statistics
+    conv on the same input (DwConvStatsFn)."""
+
+    @staticmethod
+    def forward(ctx, x, w, k, s, p, link):
+        C = x.shape[3]
+        x = x.contiguous()
+        wk = w.detach().contiguous()
+        d, shape = _dw_desc(x, C, k, s, p)
+        y = torch.empty(shape, dtype=torch.float32, device=x.device)
+        call("b2y_dwconv_fwd_f32", ctypes.byref(d), ptr(x), ptr(wk), None, ptr(y), stream_ptr())
+        ctx.save_for_backward(x, wk)
+        ctx.geom = (d, link)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, wk = ctx.saved_tensors
+        d, link = ctx.geom
+        gy = gy.contiguous().float()
+        # the statistics conv's backward only runs if W_q's gradient can reach the statistics through the fold
+        deferred = link is not None and ctx.needs_input_grad[1]
+        dx = torch.empty_like(x) if ctx.needs_input_grad[0] and not deferred else None
+        dw = torch.empty_like(wk) if ctx.needs_input_grad[1] else None
+        if dx is not None or dw is not None:
+            call("b2y_dwconv_bwd_f32", ctypes.byref(d), ptr(x), ptr(gy), ptr(wk), ptr(dx), ptr(dw), stream_ptr())
+        if deferred:
+            link.gy, link.w = gy, wk
+        return dx, dw, None, None, None, None
+
+
+class DwConvStatsFn(torch.autograd.Function):
+    """Per-channel batch mean and unbiased variance (torch.var) of z = dwconv(x, w) + b, the statistics conv of a TPSQ
+    depthwise layer; z is recomputed in the forward and the backward, never stored.  Both outputs are differentiable:
+    gz = g_mean / n + 2 g_var (z - mean) / (n - 1), and dx adds the linked quantised conv's data gradient."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, k, s, p, link):
+        C = x.shape[3]
+        x = x.contiguous()
+        wk = w.detach().contiguous()
+        bk = b.detach().contiguous() if b is not None else None
+        d, shape = _dw_desc(x, C, k, s, p)
+        mean = torch.empty(C, dtype=torch.float32, device=x.device)
+        var = torch.empty_like(mean)
+        call("b2y_dwconv_stats_f32", ctypes.byref(d), ptr(x), ptr(wk), ptr(bk), ptr(mean), ptr(var), stream_ptr())
+        ctx.save_for_backward(x, wk, bk, mean)
+        ctx.geom = (d, shape, link)
+        return mean, var
+
+    @staticmethod
+    def backward(ctx, g_mean, g_var):
+        x, wk, bk, mean = ctx.saved_tensors
+        d, shape, link = ctx.geom
+        gy, wq = (link.gy, link.w) if link is not None else (None, None)
+        if link is not None:
+            link.gy = link.w = None
+        gm = g_mean.contiguous().float() if g_mean is not None else None
+        gv = g_var.contiguous().float() if g_var is not None else None
+        dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        dw = torch.empty_like(wk) if ctx.needs_input_grad[1] else None
+        if dx is not None or dw is not None:
+            gs = torch.empty(shape, dtype=torch.float32, device=x.device)
+            call("b2y_dwconv_stats_bwd_f32", ctypes.byref(d), ptr(x), ptr(wk), ptr(bk), ptr(mean), ptr(gm), ptr(gv),
+                 ptr(gy), ptr(wq), ptr(gs), ptr(dx), ptr(dw), stream_ptr())
+        # sum_pixels gz = g_mean: the bias moves the mean and leaves the variance
+        db = (gm if gm is not None else torch.zeros_like(mean)) if ctx.needs_input_grad[2] else None
+        return dx, dw, db, None, None, None, None
+
+
+def dwconv2d(x, w, k, s, p, link=None):
+    """y = Conv2d(groups=C)(x, w) over NHWC fp32 on the kernels of depthwise.cu"""
+    return DwConvFn.apply(x, w, k, s, p, link)
+
+
+def dwconv_stats(x, w, b, k, s, p, link=None):
+    """(mean, var) of dwconv(x, w) + b over batch and pixels, differentiable; `link` couples the backward with the
+    quantised conv dwconv2d(x, W_q, ..., link) on the same input"""
+    return DwConvStatsFn.apply(x, w, b, k, s, p, link)
+
+
 def depthwise_block(block, d, x, training):
     """module tree Sequential(DepthWise2d, BatchNorm2d[, activation]) of models._conv_block -> NHWC fp32 output"""
     conv = block[0]
@@ -317,7 +410,10 @@ class QatRunner:
             if t == 'convolutional':
                 h = m[0](h)
             elif t == 'depthwise':
-                h = depthwise_block(m, d, h, model.training)
+                if hasattr(m[0], 'weight_quantizer'):     # TPSQ: one quantised BN-folded layer (models.py:140-155)
+                    h = m[0](h)
+                else:                                     # google QAT: the float block
+                    h = depthwise_block(m, d, h, model.training)
             elif t == 'se':
                 h = se_layer(m.se, h)
             elif t == 'shortcut':

@@ -452,10 +452,11 @@ float* stream_ws(cudaStream_t st, long long n);
 // channels x 8 pixel rows sums K values per (row, channel) over its chunk of the rows in double, the 8 rows are then added
 // in order, and the chunk's total goes to part[((group * chunks + chunk) * K + k) * C + c].  chunk_sum_kernel adds the
 // chunks in order.  No atomics, so two runs give the same bits.  grid = (ceil(C / 32), F32_CHUNKS, groups), block (32, 8).
+// V is the type op writes its per-row values in (double where a value must not be rounded to fp32 first).
 namespace b2y {
 constexpr int F32_CHUNKS = 128;
 
-template <int K, typename Op>
+template <int K, typename Op, typename V = float>
 __device__ __forceinline__ void chunk_reduce(const Op& op, long long rows, int C, double* __restrict__ part) {
     __shared__ double red[K][8][33];
     const int c = blockIdx.x * 32 + threadIdx.x;
@@ -467,7 +468,7 @@ __device__ __forceinline__ void chunk_reduce(const Op& op, long long rows, int C
     for (int k = 0; k < K; ++k) acc[k] = 0.0;
     if (c < C) {
         for (long long r = r0 + threadIdx.y; r < r1; r += 8) {
-            float v[K];
+            V v[K];
             op(blockIdx.z, r, c, v);
 #pragma unroll
             for (int k = 0; k < K; ++k) acc[k] += (double)v[k];

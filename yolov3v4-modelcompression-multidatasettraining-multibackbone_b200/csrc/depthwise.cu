@@ -429,8 +429,8 @@ inline int set_smem(K kern, size_t bytes, unsigned long long& mask) {
 
 // ------------------------------------------------------------------------------------------------------------
 // fp32 NHWC versions for the google-QAT graph (b200yolo/qat.py), whose depthwise blocks and SE layers stay in float
-// (reference models.py:115-197 under quantized=1).  Dense tensors (pitch = C), any C: MobileNet's widths 24, 40, 72, 120,
-// 184 and 200 are not multiples of 16.  One thread per (pixel, channel), consecutive threads on consecutive channels;
+// (reference models.py:115-197 under quantized=1), and for the quantised depthwise layers of the TPSQ graph.  Dense
+// tensors (pitch = C), any C: MobileNet's widths 24, 40, 72, 120, 184 and 200 are not multiples of 16.  One thread per (pixel, channel), consecutive threads on consecutive channels;
 // every reduction over pixels goes through chunk_reduce (common.cuh), so two runs give the same bits.
 
 // z[n,yo,xo,c] = bias[c] + sum_{r,s} x[n, yo*st-pad+r, xo*st-pad+s, c] * w[c][r][s]
@@ -459,10 +459,12 @@ dwconv_f32_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, 
     }
 }
 
-// dx[n,yi,xi,c] = sum_{r,s} w[c][r][s] * dz[n, (yi+pad-r)/st, (xi+pad-s)/st, c]
+// dx[n,yi,xi,c] = sum_{r,s} w[c][r][s] * dz[n, (yi+pad-r)/st, (xi+pad-s)/st, c]  (+ w2 * dz2 at the same taps when dz2
+// is given: the two convolutions of a TPSQ depthwise layer read the same input, so their data gradients share a gather)
 __global__ void __launch_bounds__(256)
-dwconv_f32_bwd_data_kernel(const float* __restrict__ dz, const float* __restrict__ w, float* __restrict__ dx, int H,
-                           int W, int C, int k, int stride, int pad, int Ho, int Wo, long long total) {
+dwconv_f32_bwd_data_kernel(const float* __restrict__ dz, const float* __restrict__ w, const float* __restrict__ dz2,
+                           const float* __restrict__ w2, float* __restrict__ dx, int H, int W, int C, int k, int stride,
+                           int pad, int Ho, int Wo, long long total) {
     for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
          idx += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(idx % C);
@@ -470,6 +472,7 @@ dwconv_f32_bwd_data_kernel(const float* __restrict__ dz, const float* __restrict
         const int xi = (int)(pix % W), yi = (int)((pix / W) % H);
         const long long n = pix / ((long long)W * H);
         const float* wc = w + (long long)c * k * k;
+        const float* wc2 = dz2 != nullptr ? w2 + (long long)c * k * k : nullptr;
         float acc = 0.f;
         for (int r = 0; r < k; ++r) {
             const int ty = yi + pad - r;
@@ -477,10 +480,92 @@ dwconv_f32_bwd_data_kernel(const float* __restrict__ dz, const float* __restrict
             for (int s = 0; s < k; ++s) {
                 const int tx = xi + pad - s;
                 if (tx < 0 || tx % stride != 0 || tx / stride >= Wo) continue;
-                acc = fmaf(__ldg(dz + ((n * Ho + ty / stride) * Wo + tx / stride) * C + c), __ldg(wc + r * k + s), acc);
+                const long long o = ((n * Ho + ty / stride) * Wo + tx / stride) * C + c;
+                acc = fmaf(__ldg(dz + o), __ldg(wc + r * k + s), acc);
+                if (wc2 != nullptr) acc = fmaf(__ldg(dz2 + o), __ldg(wc2 + r * k + s), acc);
             }
         }
         dx[idx] = acc;
+    }
+}
+
+// Batch statistics of z = dwconv(x, w) + bias, z recomputed here (never stored): the taps accumulate in double (the
+// fp32 x fp32 products are exact there) and z and z^2 go to chunk_reduce as doubles, so a channel whose |mean| is many
+// times its standard deviation keeps its variance.
+struct DwStatOp {
+    const float* x;
+    const float* w;
+    const float* bias;
+    int H, W, C, k, stride, pad, Ho, Wo;
+    __device__ void operator()(int, long long pix, int c, double (&v)[2]) const {
+        const int xo = (int)(pix % Wo), yo = (int)((pix / Wo) % Ho);
+        const long long n = pix / ((long long)Wo * Ho);
+        const float* wc = w + (long long)c * k * k;
+        double z = bias != nullptr ? (double)__ldg(bias + c) : 0.0;
+        for (int r = 0; r < k; ++r) {
+            const int yi = yo * stride - pad + r;
+            if (yi < 0 || yi >= H) continue;
+            for (int s = 0; s < k; ++s) {
+                const int xi = xo * stride - pad + s;
+                if (xi < 0 || xi >= W) continue;
+                z = fma((double)__ldg(x + ((n * H + yi) * W + xi) * C + c), (double)__ldg(wc + r * k + s), z);
+            }
+        }
+        v[0] = z;
+        v[1] = z * z;
+    }
+};
+__global__ void __launch_bounds__(256) dwconv_f32_stats_kernel(DwStatOp op, long long rows, double* part) {
+    chunk_reduce<2, DwStatOp, double>(op, rows, op.C, part);
+}
+// part [chunk][2][C] -> mean, unbiased variance (torch.var), formed in double
+__global__ void dwconv_f32_stats_finish_kernel(const double* __restrict__ part, long long count, float* __restrict__ mean,
+                                               float* __restrict__ var, int C) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double s1 = 0.0, s2 = 0.0;
+    for (int ch = 0; ch < F32_CHUNKS; ++ch) {
+        s1 += part[((long long)ch * 2) * C + c];
+        s2 += part[((long long)ch * 2 + 1) * C + c];
+    }
+    const double m = s1 / (double)count;
+    mean[c] = (float)m;
+    var[c] = count > 1 ? (float)(fmax(s2 - s1 * m, 0.0) / (double)(count - 1)) : 0.f;
+}
+
+// gradient into z = dwconv(x, w) + bias through its batch statistics:
+// gs = g_mean / n + 2 g_var (z - mean) / (n - 1), z recomputed (k^2 MACs per output, as in the forward)
+__global__ void __launch_bounds__(256)
+dwconv_f32_stats_grad_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                             const float* __restrict__ mean, const float* __restrict__ g_mean,
+                             const float* __restrict__ g_var, float* __restrict__ gs, int H, int W, int C, int k,
+                             int stride, int pad, int Ho, int Wo, long long total) {
+    const double n = (double)(total / C);
+    const float inv_n = (float)(1.0 / n), two_inv_n1 = n > 1.0 ? (float)(2.0 / (n - 1.0)) : 0.f;
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % C);
+        const long long pix = idx / C;
+        float g = g_mean != nullptr ? __ldg(g_mean + c) * inv_n : 0.f;
+        if (g_var != nullptr) {
+            const int xo = (int)(pix % Wo), yo = (int)((pix / Wo) % Ho);
+            const long long nn = pix / ((long long)Wo * Ho);
+            const float* wc = w + (long long)c * k * k;
+            float z = 0.f;
+            for (int r = 0; r < k; ++r) {
+                const int yi = yo * stride - pad + r;
+                if (yi < 0 || yi >= H) continue;
+                for (int s = 0; s < k; ++s) {
+                    const int xi = xo * stride - pad + s;
+                    if (xi < 0 || xi >= W) continue;
+                    z = fmaf(__ldg(x + ((nn * H + yi) * W + xi) * C + c), __ldg(wc + r * k + s), z);
+                }
+            }
+            // z - mean as (conv - (mean - bias)): the bias cancels before any rounding of the large terms
+            const float centred = z - (__ldg(mean + c) - (bias != nullptr ? __ldg(bias + c) : 0.f));
+            g = fmaf(__ldg(g_var + c) * two_inv_n1, centred, g);
+        }
+        gs[idx] = g;
     }
 }
 
@@ -730,8 +815,9 @@ extern "C" int b2y_dwconv_bwd_f32(const b2y_conv_desc* d, const float* x, const 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (dx != nullptr) {
         const long long total = (long long)d->batch * d->in_h * d->in_w * d->in_c;
-        dwconv_f32_bwd_data_kernel<<<grid_1d(total), 256, 0, st>>>(dz, w, dx, d->in_h, d->in_w, d->in_c, d->ksize,
-                                                                  d->stride, d->pad, d->out_h, d->out_w, total);
+        dwconv_f32_bwd_data_kernel<<<grid_1d(total), 256, 0, st>>>(dz, w, nullptr, nullptr, dx, d->in_h, d->in_w,
+                                                                  d->in_c, d->ksize, d->stride, d->pad, d->out_h,
+                                                                  d->out_w, total);
     }
     if (dw != nullptr) {
         const int k2 = d->ksize * d->ksize;
@@ -741,6 +827,51 @@ extern "C" int b2y_dwconv_bwd_f32(const b2y_conv_desc* d, const float* x, const 
         dwconv_f32_wgrad_reduce_kernel<<<chunk_grid(d->in_c, k2), dim3(32, 8), 0, st>>>(
             op, (long long)d->batch * d->out_h * d->out_w, part);
         dwconv_f32_wgrad_finish_kernel<<<grid_1d((long long)d->in_c * k2), 256, 0, st>>>(part, dw, d->in_c, k2);
+    }
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_dwconv_stats_f32(const b2y_conv_desc* d, const float* x, const float* w, const float* bias,
+                                    float* mean, float* var, void* stream) {
+    if (!d || !x || !w || !mean || !var) return B2Y_ERR_INVALID;
+    if (!dw_f32_ok(d)) return B2Y_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int c = d->in_c;
+    double* part = chunk_ws(st, 1, 2, c);
+    if (part == nullptr) return B2Y_ERR_CUDA;
+    const long long rows = (long long)d->batch * d->out_h * d->out_w;
+    const DwStatOp op{x, w, bias, d->in_h, d->in_w, c, d->ksize, d->stride, d->pad, d->out_h, d->out_w};
+    dwconv_f32_stats_kernel<<<chunk_grid(c, 1), dim3(32, 8), 0, st>>>(op, rows, part);
+    dwconv_f32_stats_finish_kernel<<<(c + 127) / 128, 128, 0, st>>>(part, rows, mean, var, c);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
+extern "C" int b2y_dwconv_stats_bwd_f32(const b2y_conv_desc* d, const float* x, const float* w, const float* bias,
+                                        const float* mean, const float* g_mean, const float* g_var, const float* dz2,
+                                        const float* w2, float* gs, float* dx, float* dw, void* stream) {
+    if (!d || !x || !w || !mean || !gs || (!dx && !dw) || (dz2 && !w2)) return B2Y_ERR_INVALID;
+    if (!dw_f32_ok(d)) return B2Y_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int c = d->in_c;
+    const long long total = (long long)d->batch * d->out_h * d->out_w * c;
+    dwconv_f32_stats_grad_kernel<<<grid_1d(total), 256, 0, st>>>(x, w, bias, mean, g_mean, g_var, gs, d->in_h, d->in_w,
+                                                                 c, d->ksize, d->stride, d->pad, d->out_h, d->out_w,
+                                                                 total);
+    if (dx != nullptr) {
+        const long long tin = (long long)d->batch * d->in_h * d->in_w * c;
+        dwconv_f32_bwd_data_kernel<<<grid_1d(tin), 256, 0, st>>>(gs, w, dz2, w2, dx, d->in_h, d->in_w, c, d->ksize,
+                                                                d->stride, d->pad, d->out_h, d->out_w, tin);
+    }
+    if (dw != nullptr) {
+        const int k2 = d->ksize * d->ksize;
+        double* part = chunk_ws(st, k2, 1, c);
+        if (part == nullptr) return B2Y_ERR_CUDA;
+        const DwWgradOp op{x, gs, d->in_h, d->in_w, c, d->ksize, d->stride, d->pad, d->out_h, d->out_w};
+        dwconv_f32_wgrad_reduce_kernel<<<chunk_grid(c, k2), dim3(32, 8), 0, st>>>(
+            op, (long long)d->batch * d->out_h * d->out_w, part);
+        dwconv_f32_wgrad_finish_kernel<<<grid_1d((long long)c * k2), 256, 0, st>>>(part, dw, c, k2);
     }
     B2Y_CUDA_CHECK(cudaGetLastError());
     return B2Y_OK;

@@ -6,7 +6,9 @@ The quantisation range is a LEARNED parameter `scale`, snapped to the nearest po
 (Search_Pow2, which also overwrites the parameter's data with P), with a soft clamp 0.5 (|x + P| - |x - P|), codes
 round(c (2^(b-1) - 1) / P) and values code * P / 2^(b-1).  Forward and backward of that quantiser are device kernels
 (b2y_tpsq_fwd_f32 / b2y_tpsq_bwd_f32: dx and the reduction sum(g * dy/dP) in one pass); the convolutions and the BN-fold
-chain are the same as in the google QAT layer (b200yolo/qat.py).  Module forwards take / return NHWC fp32 tensors.
+chain are the same as in the google QAT layer (b200yolo/qat.py).  Depthwise layers (groups = channels, MobileNet's
+[depthwise] blocks) run both convolutions on the fp32 depthwise kernels (qat.dwconv_stats / qat.dwconv2d) with the same
+fold; other grouped convolutions are not supported.  Module forwards take / return NHWC fp32 tensors.
 
 Reference quirks kept: Weight_Quantizer passes `warmup` in the out_channels slot of its base class, so weights are never
 warmed up (their scale parameter starts at 1.0); activations warm up on their first forward (99 candidates
@@ -196,19 +198,29 @@ class TPSQ_BNFold_QuantizedConv2d_For_FPGA(nn.Conv2d):
 
     def forward(self, input):
         from b200yolo import qat
+        depthwise = self.groups != 1
+        if depthwise and not self.groups == self.in_channels == self.out_channels:
+            raise NotImplementedError("grouped convolution (1 < groups < channels) in a TPSQ layer")
         if not input.is_cuda:
             raise RuntimeError("TPSQ layers run on the CUDA device only (no CPU fallback)")
-        if self.groups != 1:
-            raise NotImplementedError("depthwise TPSQ layers")
         k, st, pd = self.kernel_size[0], self.stride[0], self.padding[0]
         cb = self.bias if self.bias is not None else 0
+        link = None
         if self.training:
             self.step += 1
             if self.bn:
-                y1, s1, s2 = qat.conv2d(input, self.weight, k, st, pd, want_stats=True)
-                n = float(y1.shape[0] * y1.shape[1] * y1.shape[2])
-                mean = s1 / n + cb
-                var = (s2 - s1 * (s1 / n)) / (n - 1.0)                # torch.var: unbiased
+                if not depthwise:
+                    y1, s1, s2 = qat.conv2d(input, self.weight, k, st, pd, want_stats=True)
+                    n = float(y1.shape[0] * y1.shape[1] * y1.shape[2])
+                    mean = s1 / n + cb
+                    var = (s2 - s1 * (s1 / n)) / (n - 1.0)                # torch.var: unbiased
+                elif float(self.step) < self.freeze_step:
+                    # the fold takes the batch statistics: both convolutions of the layer share one backward
+                    link = qat.DwGradLink()
+                    mean, var = qat.dwconv_stats(input, self.weight, self.bias, k, st, pd, link)
+                else:
+                    with torch.no_grad():                                  # only the running statistics read them
+                        mean, var = qat.dwconv_stats(input, self.weight, self.bias, k, st, pd)
                 self.batch_mean, self.batch_var = mean, var
                 with torch.no_grad():
                     if float(self.first_bn) == 0 and not bool(self.running_mean.any()) and not bool(self.running_var.any()):
@@ -231,6 +243,9 @@ class TPSQ_BNFold_QuantizedConv2d_For_FPGA(nn.Conv2d):
             weight, bias = self.BN_fuse()
         q_weight = self.weight_quantizer(weight)
         q_bias = self.bias_quantizer(bias)
-        out = qat.conv2d(input, q_weight, k, st, pd) + q_bias
+        if depthwise:
+            out = qat.dwconv2d(input, q_weight, k, st, pd, link) + q_bias
+        else:
+            out = qat.conv2d(input, q_weight, k, st, pd) + q_bias
         out = qat.activation(out, self.activate, self.maxabsscaler)
         return self.activation_quantizer(out)
