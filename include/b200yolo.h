@@ -518,6 +518,28 @@ int b2y_kd_box(const float* student, const float* teacher, const long long* idx,
 int b2y_letterbox_u8(const unsigned char* src, int src_h, int src_w, int channels, long long src_pitch, int resized_h,
                      int resized_w, int top, int left, unsigned char* dst, int dst_h, int dst_w, int swap_rb, int color,
                      void* stream);
+/* One evaluation batch of LoadImagesAndLabels(rect=True) (utils/datasets.py:419-475, 511-531) in ONE launch: per item,
+ * load_image's cv2.resize INTER_AREA of the source to rs_w x rs_h (rs == source size: plain copy), placed at (top, left)
+ * of a dst_h x dst_w plane of `color` (letterbox with auto=False, scaleup=False only pads on this path), channel order
+ * reversed when swap_rb, into slot `slot` of dst uint8 planar [batch][channels][dst_h][dst_w].  Bit-identical to OpenCV's
+ * 8-bit INTER_AREA: integer factors (area_kx, area_ky > 0, used by cv::resize when both scales are integers within
+ * DBL_EPSILON) average the block, other sizes take the fractional path (area_kx = area_ky = 0).
+ * items: host table, checked (B2Y_ERR_INVALID, nothing launched, for a bad item: a size that does not fit, a scale that
+ * is not 1. / ((double)rs / src), integer factors where cv::resize would not use them or vice versa, a slot out of
+ * range); items_dev: the same n_items items in device memory, which the kernel reads. */
+typedef struct b2y_load_item {
+    const unsigned char* src;   /* device, HWC uint8 [src_h][src_w][channels] */
+    long long src_pitch;        /* bytes per source row */
+    int src_h, src_w;
+    int rs_h, rs_w;             /* size after INTER_AREA */
+    int area_kx, area_ky;       /* integer factors of the block-mean path, or 0 */
+    double scale_x, scale_y;    /* src_w / rs_w, src_h / rs_h as cv::resize computes them */
+    int top, left;              /* border */
+    int slot;                   /* batch index written */
+    int reserved;
+} b2y_load_item;
+int b2y_load_batch_u8(const b2y_load_item* items, const b2y_load_item* items_dev, int n_items, unsigned char* dst,
+                      int batch, int channels, int dst_h, int dst_w, int swap_rb, int color, void* stream);
 
 #ifdef __cplusplus
 }

@@ -58,6 +58,13 @@ class UnpackItem(C.Structure):
                 ("tile_begin", C.c_int), ("Ipad", C.c_int)]
 
 
+class LoadItem(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("src_pitch", C.c_longlong), ("src_h", C.c_int), ("src_w", C.c_int),
+                ("rs_h", C.c_int), ("rs_w", C.c_int), ("area_kx", C.c_int), ("area_ky", C.c_int),
+                ("scale_x", C.c_double), ("scale_y", C.c_double), ("top", C.c_int), ("left", C.c_int),
+                ("slot", C.c_int), ("reserved", C.c_int)]
+
+
 class QConvDesc(C.Structure):
     _fields_ = [
         ("conv", ConvDesc),
@@ -157,6 +164,7 @@ _PROTOS = {
     "b2y_kd_soft_rows": (i32, [vp, vp, ll, i32, i32, i32, f32, f32, vp, vp, vp]),
     "b2y_kd_box": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp, vp, vp, vp]),
     "b2y_letterbox_u8": (i32, [vp, i32, i32, i32, ll, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp]),
+    "b2y_load_batch_u8": (i32, [vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, vp]),
     "b2y_nms_count_workspace_bytes": (sz, [i32, i32]),
     "b2y_nms_count": (i32, [vp, i32, i32, i32, f32, i32, vp, vp, vp, vp, sz, vp]),
     "b2y_nms_run_workspace_bytes": (sz, [ll]),

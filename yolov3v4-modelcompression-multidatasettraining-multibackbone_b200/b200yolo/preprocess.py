@@ -9,8 +9,15 @@ reference's `/ 256`).  Bit-exact against cv2.resize(INTER_LINEAR) + cv2.copyMake
 
 Host images (numpy arrays / CPU tensors) are copied to the device as they are (raw BGR bytes, the smallest form of the
 image); resizing, padding, channel shuffle and the float conversion never touch the CPU.
+
+DeviceEvalLoader replaces test.py's DataLoader over LoadImagesAndLabels(rect=True): load_image's INTER_AREA downscale,
+the rect letterbox and the shuffle of a whole batch in one launch (b2y_load_batch_u8), bit-exact with the reference.
+
+    results, maps = test.test(cfg, data, model=model, dataloader=DeviceEvalLoader(dataset, batch_size))
 """
 import ctypes as C
+import os
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -41,6 +48,55 @@ def letterbox_params(shape, new_shape=(416, 416), auto=True, scaleFill=False, sc
     top, bottom = int(round(dh - 0.1)), int(round(dh + 0.1))
     left, right = int(round(dw - 0.1)), int(round(dw + 0.1))
     return new_unpad, ratio, (dw, dh), (top, bottom, left, right)
+
+
+DBL_EPSILON = 2.220446049250313e-16
+
+
+def load_image_size(h0, w0, img_size):
+    """The size load_image (datasets.py:511-531, augment=False) resizes a (h0, w0) source to: sources larger than
+    img_size shrink with INTER_AREA to (int(h0 * r), int(w0 * r)), r = img_size / max(h0, w0); others stay as they are."""
+    r = img_size / max(h0, w0)
+    if r < 1:
+        return int(h0 * r), int(w0 * r)
+    return h0, w0
+
+
+def inter_area_params(src_h, src_w, h, w):
+    """cv2.resize's INTER_AREA set-up for a downscale (h, w <= src_h, src_w): returns (scale_x, scale_y, kx, ky).
+    kx, ky > 0 are the integer factors of the block-mean path, which OpenCV takes when both scales are integers within
+    DBL_EPSILON (saturate_cast<int>(double) rounds half to even, as Python's round does); 0, 0 = the fractional path."""
+    scale_x = 1.0 / (w / src_w)
+    scale_y = 1.0 / (h / src_h)
+    kx, ky = round(scale_x), round(scale_y)
+    if abs(scale_x - kx) < DBL_EPSILON and abs(scale_y - ky) < DBL_EPSILON:
+        return scale_x, scale_y, kx, ky
+    return scale_x, scale_y, 0, 0
+
+
+def eval_labels(x, ratio, w, h, pad, out_h, out_w):
+    """LoadImagesAndLabels.__getitem__'s label mapping (datasets.py:441-467) for one image without augmentation:
+    normalised xywh (float32 [n, 5] with the class first) -> pixel xyxy through ratio and pad -> xywh normalised by the
+    letterboxed (out_h, out_w).  The same numpy operations in the same order, with the scalar types the reference has:
+    ratio and pad are numpy float64 (from its numpy batch shape), so under numpy 2's promotion each box coordinate is
+    computed in float64 and rounded once into the float32 array; the divisions by the integer sizes stay float32."""
+    if x.size == 0:
+        return np.zeros((0, 5), np.float32)
+    labels = x.copy()
+    labels[:, 1] = ratio[0] * w * (x[:, 1] - x[:, 3] / 2) + pad[0]
+    labels[:, 2] = ratio[1] * h * (x[:, 2] - x[:, 4] / 2) + pad[1]
+    labels[:, 3] = ratio[0] * w * (x[:, 1] + x[:, 3] / 2) + pad[0]
+    labels[:, 4] = ratio[1] * h * (x[:, 2] + x[:, 4] / 2) + pad[1]
+    b = labels[:, 1:5]
+    y = np.zeros_like(b)                             # utils.xyxy2xywh
+    y[:, 0] = (b[:, 0] + b[:, 2]) / 2
+    y[:, 1] = (b[:, 1] + b[:, 3]) / 2
+    y[:, 2] = b[:, 2] - b[:, 0]
+    y[:, 3] = b[:, 3] - b[:, 1]
+    labels[:, 1:5] = y
+    labels[:, [2, 4]] /= out_h
+    labels[:, [1, 3]] /= out_w
+    return labels
 
 
 def _device_image(img0, device):
@@ -82,8 +138,10 @@ def letterbox(img0, new_shape=(416, 416), color=(114, 114, 114), auto=True, scal
 
 
 def letterbox_batch(images, new_shape=640, scaleup=True, device=None):
-    """Fixed-size batch (auto=False, what LoadImagesAndLabels / LoadStreams(rect=False) use): list of HWC uint8 BGR
-    images -> (uint8 [B, 3, H, W] RGB batch on the device, [ratio], [(dw, dh)])."""
+    """Fixed-size batch (auto=False) of sources that are already `new_shape` or smaller, e.g. the output of load_image:
+    list of HWC uint8 BGR images -> (uint8 [B, 3, H, W] RGB batch on the device, [ratio], [(dw, dh)]).  Larger sources
+    are downscaled with letterbox's INTER_LINEAR, which is not what LoadImagesAndLabels does with raw cv2.imread images
+    (load_image shrinks them with INTER_AREA first): build evaluation batches with DeviceEvalLoader."""
     if isinstance(new_shape, int):
         new_shape = (new_shape, new_shape)
     first = _device_image(images[0], device)
@@ -94,3 +152,139 @@ def letterbox_batch(images, new_shape=640, scaleup=True, device=None):
         ratios.append(r)
         pads.append(p)
     return batch, ratios, pads
+
+
+class DeviceEvalLoader:
+    """test.py's `DataLoader(dataset, batch_size, collate_fn=dataset.collate_fn)` over a LoadImagesAndLabels built with
+    rect=True and no augmentation, with the images built on the device.  Iterating yields what that loader yields:
+    (uint8 [B, C, H, W] device batch, float32 [nT, 6] device targets (image index, class, xywh normalised), paths,
+    shapes = ((h0, w0), ((h / h0, w / w0), pad)) per image).
+
+    `dataset` is the reference's dataset or any object with its attributes: img_files, labels, batch, batch_shapes,
+    img_size, imgs (the --cache-images cache, with img_hw0 / img_hw), is_gray_scale, augment.  Sources are decoded with
+    cv2.imread on host threads and copied to the device once, as raw bytes; INTER_AREA, border, channel shuffle and
+    batching run in one launch per batch (b2y_load_batch_u8).  Labels are mapped on the host (a few floats per box, the
+    reference's own numpy arithmetic) and reach the device in one copy per batch."""
+
+    def __init__(self, dataset, batch_size, device=None, workers=None):
+        if getattr(dataset, "augment", False):
+            raise ValueError("DeviceEvalLoader builds evaluation batches only: the dataset has augment=True")
+        if not getattr(dataset, "rect", True) or getattr(dataset, "batch_shapes", None) is None:
+            raise ValueError("DeviceEvalLoader needs a rect=True dataset (rectangular batch shapes)")
+        self.dataset = dataset
+        self.batch_size = int(batch_size)
+        self.device = None if device is None else torch.device(device)
+        self.workers = workers or min(8, os.cpu_count() or 1)
+        self._pool = None
+
+    def __len__(self):
+        return (len(self.dataset.img_files) + self.batch_size - 1) // self.batch_size
+
+    def __iter__(self):
+        for b in range(len(self)):
+            yield self.batch(b)
+
+    def batch(self, b):
+        """Batch b: (imgs, targets, paths, shapes)."""
+        return self.device_batch(self.host_batch(b))
+
+    def _read(self, index):
+        ds = self.dataset
+        imgs = getattr(ds, "imgs", None)
+        if imgs is not None and imgs[index] is not None:        # --cache-images: load_image's output, kept in memory
+            img = imgs[index]
+            (h0, w0), hw = ds.img_hw0[index], ds.img_hw[index]
+        else:
+            import cv2
+            path = ds.img_files[index]
+            img = cv2.imread(path, flags=cv2.IMREAD_GRAYSCALE) if ds.is_gray_scale else cv2.imread(path)
+            if img is None:
+                raise FileNotFoundError("Image Not Found " + path)
+            h0, w0 = img.shape[:2]
+            hw = load_image_size(h0, w0, ds.img_size)
+        img = np.ascontiguousarray(img)
+        if img.ndim == 2:
+            img = img[:, :, None]
+        if img.dtype != np.uint8 or img.ndim != 3:
+            raise ValueError("%s: expected an HWC uint8 image" % ds.img_files[index])
+        return img, (h0, w0), tuple(hw)
+
+    def host_batch(self, b):
+        """Decode the sources of batch b (threads) and plan every item on the host: sizes, INTER_AREA path, border,
+        labels, shapes.  Returns a list of per-image dicts."""
+        ds = self.dataset
+        idx = list(range(b * self.batch_size, min(len(ds.img_files), (b + 1) * self.batch_size)))
+        if self._pool is None:
+            self._pool = ThreadPoolExecutor(self.workers)
+        reads = list(self._pool.map(self._read, idx)) if len(idx) > 1 else [self._read(i) for i in idx]
+        plans = []
+        for i, (img, (h0, w0), (h, w)) in zip(idx, reads):
+            # the batch shape stays the numpy row it is in the reference: ratio and pad come out as numpy float64
+            # scalars, which the label arithmetic below depends on
+            shape = ds.batch_shapes[ds.batch[i]]
+            (rw, rh), ratio, pad, (top, bottom, left, right) = letterbox_params((h, w), shape, auto=False, scaleup=False)
+            if (rw, rh) != (w, h):
+                raise NotImplementedError(
+                    "%s: resized to %dx%d, it does not fit its batch shape %s; letterbox would resize it a second time"
+                    % (ds.img_files[i], w, h, tuple(int(v) for v in shape)))
+            src_h, src_w, cn = img.shape
+            if cn != (1 if ds.is_gray_scale else 3):
+                raise ValueError("%s: %d channels in a %s dataset" % (ds.img_files[i], cn,
+                                                                     "gray-scale" if ds.is_gray_scale else "colour"))
+            if (src_h, src_w) == (h, w):
+                scales = (1.0, 1.0, 0, 0)
+            elif h > src_h or w > src_w:
+                raise NotImplementedError("%s: up-scaling (%dx%d -> %dx%d) is not part of evaluation loading"
+                                          % (ds.img_files[i], src_w, src_h, w, h))
+            else:
+                scales = inter_area_params(src_h, src_w, h, w)
+            out_h, out_w = h + top + bottom, w + left + right
+            plans.append(dict(img=img, rs=(h, w), top=top, left=left, out=(out_h, out_w), scales=scales,
+                              labels=eval_labels(ds.labels[i], ratio, w, h, pad, out_h, out_w),
+                              path=ds.img_files[i], shapes=((h0, w0), ((h / h0, w / w0), pad))))
+        if len({p["out"] for p in plans}) != 1:
+            raise ValueError("batch %d mixes letterboxed shapes %s: the loader's batch_size must be the dataset's"
+                             % (b, sorted({p["out"] for p in plans})))
+        return plans
+
+    def device_batch(self, plans):
+        """One host-to-device copy of the sources and the item table, one launch for the images, one copy of the
+        targets."""
+        from .lib import LoadItem
+        if not torch.cuda.is_available():
+            raise lib.B2YError("DeviceEvalLoader runs on the CUDA device only (no CPU fallback)")
+        if self.device is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        B, (H, W), cn = len(plans), plans[0]["out"], plans[0]["img"].shape[2]
+        isz = C.sizeof(LoadItem)
+        offs, total = [], isz * B
+        for p in plans:
+            total = (total + 15) // 16 * 16
+            offs.append(total)
+            total += p["img"].nbytes
+        dev = torch.empty(total, dtype=torch.uint8, device=self.device)
+        base = dev.data_ptr()
+        items = (LoadItem * B)()
+        host = np.empty(total, np.uint8)
+        for k, (p, o) in enumerate(zip(plans, offs)):
+            img = p["img"]
+            sx, sy, kx, ky = p["scales"]
+            items[k] = LoadItem(src=base + o, src_pitch=img.shape[1] * cn, src_h=img.shape[0], src_w=img.shape[1],
+                                rs_h=p["rs"][0], rs_w=p["rs"][1], area_kx=kx, area_ky=ky, scale_x=sx, scale_y=sy,
+                                top=p["top"], left=p["left"], slot=k)
+            host[o:o + img.nbytes] = img.reshape(-1)
+        host[:isz * B] = np.frombuffer(bytes(items), np.uint8)
+        dev.copy_(torch.from_numpy(host))
+        out = torch.empty((B, cn, H, W), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            call("b2y_load_batch_u8", C.cast(items, C.c_void_p), ptr(dev), B, ptr(out), B, cn, H, W,
+                 1 if cn == 3 else 0, 114, stream_ptr())
+        labels = []
+        for k, p in enumerate(plans):
+            lo = torch.zeros((len(p["labels"]), 6))
+            if len(p["labels"]):
+                lo[:, 1:] = torch.from_numpy(p["labels"])
+            lo[:, 0] = k
+            labels.append(lo)
+        targets = torch.cat(labels, 0).to(self.device)
+        return out, targets, tuple(p["path"] for p in plans), tuple(p["shapes"] for p in plans)

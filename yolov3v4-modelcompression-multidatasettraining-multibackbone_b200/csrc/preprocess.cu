@@ -4,6 +4,14 @@
 // consumes (it applies the "/ 256").  The arithmetic is OpenCV's (third-party dependency of the reference, not vendored;
 // this container: 4.13.0) -- restated in csrc/preprocess_core.h / oracle/preprocess_oracle.py and pinned against cv2's
 // own outputs; bit-exact.  HBM / gather bound: 4 source pixels read per output pixel, one byte written per channel.
+//
+// b2y_load_batch_u8 builds a whole evaluation batch of LoadImagesAndLabels(rect=True) (utils/datasets.py:419-475,
+// 511-531) in one table-driven launch: load_image's INTER_AREA downscale, the letterbox border (its own resize is not
+// reached: the rect batch shape always holds the resized image) and the channel shuffle.  Gather bound: an output byte
+// reads its source cell (about scale_x * scale_y bytes, each once from HBM and the rest from L1/L2) and does a few
+// float operations per source byte; the border bytes read nothing.
+#include <cmath>
+
 #include "b200yolo.h"
 #include "common.cuh"
 #include "preprocess_core.h"
@@ -17,7 +25,62 @@ __global__ void __launch_bounds__(256) letterbox_u8_kernel(const unsigned char* 
     b2y_lb_pixel(src, dst, p, x, (int)blockIdx.y);
 }
 
+// One launch for a whole evaluation batch: blockIdx.z = item, blockIdx.y = output row, threads along the row.  Each
+// output byte is the border colour or the INTER_AREA value computed straight from the source (copy when the source
+// already has the resized size), written to channel c of slot item.slot of the planar [B][C][H][W] batch.
+__global__ void __launch_bounds__(128) load_batch_u8_kernel(const b2y_load_item* __restrict__ items,
+                                                            unsigned char* __restrict__ dst, int C, int H, int W,
+                                                            int swap_rb, unsigned char color) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= W) return;
+    const b2y_load_item it = items[blockIdx.z];
+    const long long plane = (long long)H * W;
+    b2y_area_params p;
+    p.src_h = it.src_h; p.src_w = it.src_w; p.channels = C; p.src_pitch = it.src_pitch;
+    p.rs_h = it.rs_h; p.rs_w = it.rs_w; p.kx = it.area_kx; p.ky = it.area_ky;
+    p.scale_x = it.scale_x; p.scale_y = it.scale_y;
+    b2y_load_pixel(it.src, p, it.top, it.left, x, y, swap_rb, color,
+                   dst + (long long)it.slot * C * plane + (long long)y * W + x, plane);
+}
+
+bool exact_factor(double scale, int k) {            // cv::resize: |scale - saturate_cast<int>(scale)| < DBL_EPSILON
+    return k > 0 && std::fabs(scale - (double)k) < 2.220446049250313e-16;
+}
+
 }  // namespace
+
+extern "C" int b2y_load_batch_u8(const b2y_load_item* items, const b2y_load_item* items_dev, int n_items,
+                                 unsigned char* dst, int batch, int channels, int dst_h, int dst_w, int swap_rb,
+                                 int color, void* stream) {
+    if (!items || !items_dev || !dst || n_items <= 0 || batch <= 0 || channels < 1 || channels > 4 || dst_h <= 0 ||
+        dst_w <= 0 || color < 0 || color > 255)
+        return B2Y_ERR_INVALID;
+    if (n_items > 65535 || dst_h > 65535) return B2Y_ERR_UNSUPPORTED;
+    for (int i = 0; i < n_items; ++i) {
+        const b2y_load_item& it = items[i];
+        if (!it.src || it.src_h <= 0 || it.src_w <= 0 || it.src_pitch < (long long)it.src_w * channels ||
+            it.rs_h <= 0 || it.rs_w <= 0 || it.rs_h > it.src_h || it.rs_w > it.src_w || it.top < 0 || it.left < 0 ||
+            it.top + it.rs_h > dst_h || it.left + it.rs_w > dst_w || it.slot < 0 || it.slot >= batch)
+            return B2Y_ERR_INVALID;
+        if (it.rs_h == it.src_h && it.rs_w == it.src_w) continue;            // copy: no resize
+        // INTER_AREA downscale: the scales cv::resize derives from the two sizes, and the integer factors exactly when
+        // it takes the block-mean path (which reads kx * rs_w columns and ky * rs_h rows)
+        const double sx = 1.0 / ((double)it.rs_w / it.src_w), sy = 1.0 / ((double)it.rs_h / it.src_h);
+        if (it.scale_x != sx || it.scale_y != sy) return B2Y_ERR_INVALID;
+        const int kx = (int)std::nearbyint(sx), ky = (int)std::nearbyint(sy);
+        if (exact_factor(sx, kx) && exact_factor(sy, ky)) {
+            if (it.area_kx != kx || it.area_ky != ky || kx * it.rs_w != it.src_w || ky * it.rs_h != it.src_h)
+                return B2Y_ERR_INVALID;
+        } else if (it.area_kx != 0 || it.area_ky != 0) {
+            return B2Y_ERR_INVALID;
+        }
+    }
+    const dim3 grid((dst_w + 127) / 128, dst_h, n_items);
+    load_batch_u8_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(items_dev, dst, channels, dst_h, dst_w,
+                                                                              swap_rb ? 1 : 0, (unsigned char)color);
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
 
 extern "C" int b2y_letterbox_u8(const unsigned char* src, int src_h, int src_w, int channels, long long src_pitch,
                                 int resized_h, int resized_w, int top, int left, unsigned char* dst, int dst_h, int dst_w,

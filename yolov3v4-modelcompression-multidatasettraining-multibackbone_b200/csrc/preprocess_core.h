@@ -1,5 +1,6 @@
-// Per-pixel arithmetic of the device letterbox (csrc/preprocess.cu), shared with the host harness of the CPU tests
-// (tests/host/letterbox_host.cpp) so that the very same code is checked against cv2's outputs without a GPU.
+// Per-pixel arithmetic of the device letterbox and evaluation batch loader (csrc/preprocess.cu), shared with the host
+// harnesses of the CPU tests (tests/host/letterbox_host.cpp, tests/host/area_host.cpp) so that the very same code is
+// checked against cv2's outputs without a GPU.
 //
 // OpenCV 4.x modules/imgproc/src/resize.cpp, 8-bit INTER_LINEAR (fixed point, INTER_RESIZE_COEF_BITS = 11):
 //   fx = (float)((dx + 0.5) * scale_x - 0.5), sx = floor(fx), fx -= sx; columns clamp (sx < 0 -> fx = 0, sx = 0;
@@ -107,6 +108,150 @@ B2Y_HD void b2y_lb_pixel(const unsigned char* src, unsigned char* dst, const b2y
 B2Y_HD void b2y_lb_set_scales(b2y_lb_params& p) {
     p.scale_x = 1.0 / ((double)p.rs_w / (double)p.src_w);
     p.scale_y = 1.0 / ((double)p.rs_h / (double)p.src_h);
+}
+
+// ---- 8-bit INTER_AREA downscale (load_image of the reference's LoadImagesAndLabels, utils/datasets.py:511-531) ----
+// OpenCV 4.x resize.cpp, both scales >= 1 (scale = 1. / ((double)dsize / ssize)), restated and pinned against cv2:
+//   * integer factors (|scale - cvRound(scale)| < DBL_EPSILON on both axes): mean of the kx x ky block, integer sum;
+//     2 x 2 rounds (sum + 2) >> 2, every other block cvRound((float)sum * (1.f / (kx * ky)));
+//   * otherwise per axis and output index d (computeResizeAreaTab, in double): f1 = d * scale, f2 = f1 + scale,
+//     cell = min(scale, size - f1), s1 = ceil(f1), s2 = min(floor(f2), size - 1), s1 = min(s1, s2); the taps are
+//     s1 - 1 with (float)((s1 - f1) / cell) if s1 - f1 > 1e-3, s1 .. s2 - 1 with (float)(1. / cell), and s2 with
+//     (float)(min(min(f2 - s2, 1.), cell) / cell) if f2 - s2 > 1e-3 -- consecutive source indices.  Per source row of
+//     the y taps, a float row buf = buf + src * alpha over the x taps; then sum = beta0 * buf0, sum = sum + beta * buf
+//     (float, no FMA anywhere); the byte is saturate_cast<uchar>(sum) = cvRound, ties to even.
+struct b2y_area_params {
+    int src_h, src_w, channels;
+    long long src_pitch;              // bytes per source row
+    int rs_h, rs_w;                   // INTER_AREA output size
+    int kx, ky;                       // both > 0: integer factors (block mean); 0: the fractional path
+    double scale_x, scale_y;          // src / rs as cv::resize computes it
+};
+
+B2Y_HD double b2y_dmul(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    volatile double t = a * b;
+    return t;
+#endif
+}
+
+B2Y_HD float b2y_fmul(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    volatile float t = a * b;
+    return t;
+#endif
+}
+
+B2Y_HD float b2y_fadd(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    volatile float t = a + b;
+    return t;
+#endif
+}
+
+B2Y_HD int b2y_area_round(float v) {                     // saturate_cast<uchar>(float)
+    const int i = b2y_lb_round(v);
+    return i < 0 ? 0 : (i > 255 ? 255 : i);
+}
+
+// The taps of output index d along one axis: n consecutive source indices from first; weight k is w_lo for k == 0
+// when has_lo, w_hi for k == n - 1 when has_hi, w_mid otherwise.
+struct b2y_area_taps {
+    int first, n;
+    bool has_lo, has_hi;
+    float w_lo, w_mid, w_hi;
+    B2Y_HD float weight(int k) const { return (k == 0 && has_lo) ? w_lo : ((k == n - 1 && has_hi) ? w_hi : w_mid); }
+};
+
+B2Y_HD b2y_area_taps b2y_area_axis(int d, int size, double scale) {
+    const double f1 = b2y_dmul((double)d, scale);
+#if defined(__CUDA_ARCH__)
+    const double f2 = __dadd_rn(f1, scale);
+    const double rest = __dsub_rn((double)size, f1);
+#else
+    volatile double f2v = f1 + scale, restv = (double)size - f1;
+    const double f2 = f2v, rest = restv;
+#endif
+    const double cell = scale < rest ? scale : rest;
+    int s1 = (int)ceil(f1), s2 = (int)floor(f2);
+    s2 = s2 < size - 1 ? s2 : size - 1;
+    s1 = s1 < s2 ? s1 : s2;
+    b2y_area_taps t;
+#if defined(__CUDA_ARCH__)
+    const double lo = __dsub_rn((double)s1, f1), hi = __dsub_rn(f2, (double)s2);
+    t.w_lo = (float)__ddiv_rn(lo, cell);
+    t.w_mid = (float)__ddiv_rn(1.0, cell);
+    double h = hi < 1.0 ? hi : 1.0;
+    h = h < cell ? h : cell;
+    t.w_hi = (float)__ddiv_rn(h, cell);
+#else
+    volatile double lov = (double)s1 - f1, hiv = f2 - (double)s2;
+    const double lo = lov, hi = hiv;
+    t.w_lo = (float)(lo / cell);
+    t.w_mid = (float)(1.0 / cell);
+    double h = hi < 1.0 ? hi : 1.0;
+    h = h < cell ? h : cell;
+    t.w_hi = (float)(h / cell);
+#endif
+    t.has_lo = lo > 1e-3;
+    t.has_hi = hi > 1e-3;
+    t.first = t.has_lo ? s1 - 1 : s1;
+    t.n = (s2 - s1) + (t.has_lo ? 1 : 0) + (t.has_hi ? 1 : 0);
+    return t;
+}
+
+// Output pixel (x, y) of the resized image, channel sc of the source, as a byte.
+B2Y_HD int b2y_area_value(const unsigned char* src, const b2y_area_params& p, int x, int y, int sc) {
+    const int C = p.channels;
+    if (p.kx > 0 && p.ky > 0) {
+        const unsigned char* s = src + (long long)y * p.ky * p.src_pitch + (long long)x * p.kx * C + sc;
+        int sum = 0;
+        for (int j = 0; j < p.ky; ++j)
+            for (int i = 0; i < p.kx; ++i) sum += s[(long long)j * p.src_pitch + i * C];
+        if (p.kx == 2 && p.ky == 2) return (sum + 2) >> 2;
+#if defined(__CUDA_ARCH__)
+        const float inv = __fdiv_rn(1.f, (float)(p.kx * p.ky));
+#else
+        volatile float inv = 1.f / (float)(p.kx * p.ky);
+#endif
+        return b2y_area_round(b2y_fmul((float)sum, inv));
+    }
+    const b2y_area_taps tx = b2y_area_axis(x, p.src_w, p.scale_x);
+    const b2y_area_taps ty = b2y_area_axis(y, p.src_h, p.scale_y);
+    float sum = 0.f;
+    for (int j = 0; j < ty.n; ++j) {
+        const unsigned char* row = src + (long long)(ty.first + j) * p.src_pitch + (long long)tx.first * C + sc;
+        float buf = 0.f;
+        for (int i = 0; i < tx.n; ++i) buf = b2y_fadd(buf, b2y_fmul((float)row[i * C], tx.weight(i)));
+        const float v = b2y_fmul(ty.weight(j), buf);
+        sum = j == 0 ? v : b2y_fadd(sum, v);
+    }
+    return b2y_area_round(sum);
+}
+
+// One output pixel (all channels) of an evaluation batch slot: border `color` outside the resized image at (top, left),
+// else the INTER_AREA value (a plain copy when the source already has the resized size), channels reversed when swap_rb.
+// out points at channel 0 of the pixel in a planar [C][H][W] slot.
+B2Y_HD void b2y_load_pixel(const unsigned char* src, const b2y_area_params& p, int top, int left, int x, int y,
+                           int swap_rb, unsigned char color, unsigned char* out, long long plane) {
+    const int C = p.channels;
+    const int rx = x - left, ry = y - top;
+    if (rx < 0 || ry < 0 || rx >= p.rs_w || ry >= p.rs_h) {
+        for (int c = 0; c < C; ++c) out[c * plane] = color;
+        return;
+    }
+    if (p.rs_w == p.src_w && p.rs_h == p.src_h) {
+        const unsigned char* s = src + (long long)ry * p.src_pitch + (long long)rx * C;
+        for (int c = 0; c < C; ++c) out[c * plane] = s[swap_rb ? C - 1 - c : c];
+        return;
+    }
+    for (int c = 0; c < C; ++c) out[c * plane] = (unsigned char)b2y_area_value(src, p, rx, ry, swap_rb ? C - 1 - c : c);
 }
 
 #endif  // B2Y_PREPROCESS_CORE_H_
