@@ -541,6 +541,49 @@ typedef struct b2y_load_item {
 int b2y_load_batch_u8(const b2y_load_item* items, const b2y_load_item* items_dev, int n_items, unsigned char* dst,
                       int batch, int channels, int dst_h, int dst_w, int swap_rb, int color, void* stream);
 
+/* ---- input pipeline, training slice (csrc/preprocess.cu): LoadImagesAndLabels(augment=True).__getitem__
+ * (utils/datasets.py:419-501) as two table-driven launches per batch.  b2y_mosaic_u8 builds load_mosaic's canvases
+ * (:553-608): canvas slot `slot` of canvas uint8 HWC [batch][2s][2s][channels] is 114 outside the four tiles' rectangles
+ * [x1a, x2a) x [y1a, y2a), and inside tile k the pixel (x + dx, y + dy) of load_image's tile: the source itself when
+ * rs == source size, else cv2.resize(INTER_LINEAR) of the source to rs_w x rs_h (bit-identical to OpenCV's 8-bit fixed
+ * point; an exact 2x downscale, which cv::resize computes as INTER_AREA, gives the same bytes).  Later tiles win where
+ * rectangles overlap, as numpy's assignments in tile order do.
+ * b2y_affine_hsv_u8 builds the batch from the canvases: per item, cv2.warpAffine(canvas, M, (s, s), INTER_LINEAR,
+ * borderValue=114) (random_affine, :649-715) with im = invertAffineTransform(M); when hsv (colour only), augment_hsv's
+ * BGR2HSV -> lut[0..255] (hue), lut[256..511] (saturation), lut[512..767] (value) -> HSV2BGR (:534-545, OpenCV's
+ * default 8-bit dispatch); the left-right flip when flip; channels reversed (BGR -> RGB) into slot `slot` of dst uint8
+ * planar [batch][channels][s][s].
+ * items: host tables, checked (B2Y_ERR_INVALID, nothing launched, for a bad item: a null source, a pitch or a tile size
+ * that does not fit, a scale that is not 1. / ((double)rs / src), a rectangle outside the canvas or reading outside its
+ * tile, a map whose coordinates overflow OpenCV's fixed point, hsv on a gray-scale batch, a slot out of range);
+ * items_dev: the same n_items items in device memory, which the kernels read. */
+typedef struct b2y_mosaic_tile {
+    const unsigned char* src;   /* device, HWC uint8 [src_h][src_w][channels] */
+    long long src_pitch;        /* bytes per source row */
+    int src_h, src_w;
+    int rs_h, rs_w;             /* load_image's tile size */
+    double scale_x, scale_y;    /* src_w / rs_w, src_h / rs_h as cv::resize computes them */
+    int x1a, y1a, x2a, y2a;     /* rectangle on the canvas */
+    int dx, dy;                 /* tile pixel = canvas pixel + (dx, dy) */
+} b2y_mosaic_tile;
+typedef struct b2y_mosaic_item {
+    b2y_mosaic_tile tiles[4];
+    int slot;
+    int reserved;
+} b2y_mosaic_item;
+int b2y_mosaic_u8(const b2y_mosaic_item* items, const b2y_mosaic_item* items_dev, int n_items, unsigned char* canvas,
+                  int batch, int channels, int s, void* stream);
+typedef struct b2y_affine_item {
+    double im[6];               /* output pixel -> canvas: invertAffineTransform(M[:2]), row-major 2 x 3 */
+    unsigned char lut[768];     /* hue, saturation, value LUTs */
+    int hsv;                    /* 1: the HSV stage */
+    int flip;                   /* 1: left-right flip */
+    int slot;                   /* canvas slot read, batch slot written */
+    int reserved;
+} b2y_affine_item;
+int b2y_affine_hsv_u8(const b2y_affine_item* items, const b2y_affine_item* items_dev, int n_items,
+                      const unsigned char* canvas, unsigned char* dst, int batch, int channels, int s, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

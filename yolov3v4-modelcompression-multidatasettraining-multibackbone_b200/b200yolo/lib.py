@@ -65,6 +65,21 @@ class LoadItem(C.Structure):
                 ("slot", C.c_int), ("reserved", C.c_int)]
 
 
+class MosaicTile(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("src_pitch", C.c_longlong), ("src_h", C.c_int), ("src_w", C.c_int),
+                ("rs_h", C.c_int), ("rs_w", C.c_int), ("scale_x", C.c_double), ("scale_y", C.c_double),
+                ("x1a", C.c_int), ("y1a", C.c_int), ("x2a", C.c_int), ("y2a", C.c_int), ("dx", C.c_int), ("dy", C.c_int)]
+
+
+class MosaicItem(C.Structure):
+    _fields_ = [("tiles", MosaicTile * 4), ("slot", C.c_int), ("reserved", C.c_int)]
+
+
+class AffineItem(C.Structure):
+    _fields_ = [("im", C.c_double * 6), ("lut", C.c_ubyte * 768), ("hsv", C.c_int), ("flip", C.c_int),
+                ("slot", C.c_int), ("reserved", C.c_int)]
+
+
 class QConvDesc(C.Structure):
     _fields_ = [
         ("conv", ConvDesc),
@@ -165,6 +180,8 @@ _PROTOS = {
     "b2y_kd_box": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp, vp, vp, vp]),
     "b2y_letterbox_u8": (i32, [vp, i32, i32, i32, ll, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp]),
     "b2y_load_batch_u8": (i32, [vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, vp]),
+    "b2y_mosaic_u8": (i32, [vp, vp, i32, vp, i32, i32, i32, vp]),
+    "b2y_affine_hsv_u8": (i32, [vp, vp, i32, vp, vp, i32, i32, i32, vp]),
     "b2y_nms_count_workspace_bytes": (sz, [i32, i32]),
     "b2y_nms_count": (i32, [vp, i32, i32, i32, f32, i32, vp, vp, vp, vp, sz, vp]),
     "b2y_nms_run_workspace_bytes": (sz, [ll]),

@@ -14,6 +14,12 @@ DeviceEvalLoader replaces test.py's DataLoader over LoadImagesAndLabels(rect=Tru
 the rect letterbox and the shuffle of a whole batch in one launch (b2y_load_batch_u8), bit-exact with the reference.
 
     results, maps = test.test(cfg, data, model=model, dataloader=DeviceEvalLoader(dataset, batch_size))
+
+DeviceTrainLoader replaces train.py's DataLoader over LoadImagesAndLabels(augment=True): load_mosaic, random_affine,
+augment_hsv, the flip and the shuffle of a whole batch in two launches (b2y_mosaic_u8, b2y_affine_hsv_u8), with the
+reference's random draws, bit-exact with it.
+
+    dataloader = DeviceTrainLoader(dataset, batch_size, shuffle=not opt.rect, sampler=None)
 """
 import ctypes as C
 import os
@@ -288,3 +294,283 @@ class DeviceEvalLoader:
             labels.append(lo)
         targets = torch.cat(labels, 0).to(self.device)
         return out, targets, tuple(p["path"] for p in plans), tuple(p["shapes"] for p in plans)
+
+
+def train_tile_size(h0, w0, img_size):
+    """The size load_image (datasets.py:511-531) gives a (h0, w0) source with augment=True: any r = img_size /
+    max(h0, w0) != 1 resizes with INTER_LINEAR, up or down, to (int(h0 * r), int(w0 * r))."""
+    r = img_size / max(h0, w0)
+    if r != 1:
+        return int(h0 * r), int(w0 * r)
+    return h0, w0
+
+
+def mosaic_rects(k, xc, yc, w, h, s):
+    """load_mosaic's placement of tile k (datasets.py:565-579), its x2b = max(xc, w) of tile 2 included, with numpy's
+    slice clamping applied to the tile side: ((x1a, y1a, x2a, y2a), (x1b, y1b, x2b, y2b))."""
+    if k == 0:
+        x1a, y1a, x2a, y2a = max(xc - w, 0), max(yc - h, 0), xc, yc
+        x1b, y1b, x2b, y2b = w - (x2a - x1a), h - (y2a - y1a), w, h
+    elif k == 1:
+        x1a, y1a, x2a, y2a = xc, max(yc - h, 0), min(xc + w, s * 2), yc
+        x1b, y1b, x2b, y2b = 0, h - (y2a - y1a), min(w, x2a - x1a), h
+    elif k == 2:
+        x1a, y1a, x2a, y2a = max(xc - w, 0), yc, xc, min(s * 2, yc + h)
+        x1b, y1b, x2b, y2b = w - (x2a - x1a), 0, max(xc, w), min(y2a - y1a, h)
+    else:
+        x1a, y1a, x2a, y2a = xc, yc, min(xc + w, s * 2), min(s * 2, yc + h)
+        x1b, y1b, x2b, y2b = 0, 0, min(w, x2a - x1a), min(y2a - y1a, h)
+    x1b, x2b, _ = slice(x1b, x2b).indices(w)
+    y1b, y2b, _ = slice(y1b, y2b).indices(h)
+    return (x1a, y1a, x2a, y2a), (x1b, y1b, x2b, y2b)
+
+
+def _xyxy2xywh(b):
+    y = np.zeros_like(b)
+    y[:, 0] = (b[:, 0] + b[:, 2]) / 2
+    y[:, 1] = (b[:, 1] + b[:, 3]) / 2
+    y[:, 2] = b[:, 2] - b[:, 0]
+    y[:, 3] = b[:, 3] - b[:, 1]
+    return y
+
+
+def train_labels(tiles, s, M, scale, flip):
+    """Labels of one mosaic item, restating the reference's numpy arithmetic and dtypes: load_mosaic's pixel xyxy per
+    tile (float32 labels, Python-int sizes and pads) and clip to [0, 2s]; random_affine's float64 `xy @ M.T`, clip,
+    filter (w > 4, h > 4, area ratio > 0.2, aspect < 10) and cast back; xyxy2xywh, the normalisation by s and the
+    left-right flip.  tiles: [(labels float32 [n, 5], w, h, padw, padh)]."""
+    labels4 = []
+    for x, w, h, padw, padh in tiles:
+        labels = x.copy()
+        if x.size > 0:
+            labels[:, 1] = w * (x[:, 1] - x[:, 3] / 2) + padw
+            labels[:, 2] = h * (x[:, 2] - x[:, 4] / 2) + padh
+            labels[:, 3] = w * (x[:, 1] + x[:, 3] / 2) + padw
+            labels[:, 4] = h * (x[:, 2] + x[:, 4] / 2) + padh
+        labels4.append(labels)
+    targets = np.concatenate(labels4, 0)
+    np.clip(targets[:, 1:], 0, 2 * s, out=targets[:, 1:])
+    n = len(targets)
+    if n:
+        width = height = s
+        xy = np.ones((n * 4, 3))
+        xy[:, :2] = targets[:, [1, 2, 3, 4, 1, 4, 3, 2]].reshape(n * 4, 2)
+        xy = (xy @ M.T)[:, :2].reshape(n, 8)
+        x = xy[:, [0, 2, 4, 6]]
+        y = xy[:, [1, 3, 5, 7]]
+        xy = np.concatenate((x.min(1), y.min(1), x.max(1), y.max(1))).reshape(4, n).T
+        xy[:, [0, 2]] = xy[:, [0, 2]].clip(0, width)
+        xy[:, [1, 3]] = xy[:, [1, 3]].clip(0, height)
+        w = xy[:, 2] - xy[:, 0]
+        h = xy[:, 3] - xy[:, 1]
+        area = w * h
+        area0 = (targets[:, 3] - targets[:, 1]) * (targets[:, 4] - targets[:, 2])
+        ar = np.maximum(w / (h + 1e-16), h / (w + 1e-16))
+        i = (w > 4) & (h > 4) & (area / (area0 * scale + 1e-16) > 0.2) & (ar < 10)
+        targets = targets[i]
+        targets[:, 1:5] = xy[i]
+    if len(targets):
+        targets[:, 1:5] = _xyxy2xywh(targets[:, 1:5])
+        targets[:, [2, 4]] /= s
+        targets[:, [1, 3]] /= s
+        if flip:
+            targets[:, 1] = 1 - targets[:, 1]
+    return targets
+
+
+def hsv_luts(r):
+    """augment_hsv's three uint8 LUTs (datasets.py:534-545) for the gains r (float64 [3]), as one [768] array."""
+    x = np.arange(0, 256, dtype=np.int16)
+    lut_hue = ((x * r[0]) % 180).astype(np.uint8)
+    lut_sat = np.clip(x * r[1], 0, 255).astype(np.uint8)
+    lut_val = np.clip(x * r[2], 0, 255).astype(np.uint8)
+    return np.concatenate((lut_hue, lut_sat, lut_val))
+
+
+class DeviceTrainLoader:
+    """train.py's `DataLoader(dataset, batch_size, shuffle, sampler, collate_fn=dataset.collate_fn)` over a
+    LoadImagesAndLabels built with augment=True and rect=False (mosaic training), with the images built on the device.
+    Iterating yields what that loader yields: (uint8 [B, C, s, s] device batch, float32 [nT, 6] device targets (image
+    index, class, xywh normalised), paths, shapes = (None,) * B).
+
+    The index order is a DataLoader's over the same sampler (RandomSampler when shuffle, the given `sampler`, e.g. a
+    DistributedSampler, whose set_epoch works through `.sampler`), and the `random` / `np.random` draws of every item
+    are made in the order a num_workers=0 DataLoader makes them, before any pixel is touched: the mosaic centre and
+    the 3 extra indices, random_affine's six draws, augment_hsv's gains (colour only), the flip.  Each distinct image
+    of a batch is taken once, from the --cache-images arrays (imgs, img_hw0, img_hw) when the dataset has them, else
+    by cv2.imread on host threads; sources and both item tables reach the device in one copy.  b2y_mosaic_u8 builds the
+    2s x 2s canvases (load_image's INTER_LINEAR for uncached sources) in a workspace kept across batches;
+    b2y_affine_hsv_u8 warps, applies the HSV LUTs, flips and reverses the channels into the batch.  Labels are mapped
+    on the host with the reference's numpy arithmetic (train_labels) and copied once per batch.
+
+    `dataset` is the reference's dataset or any object with its attributes: img_files, labels, img_size, hyp, augment,
+    rect, image_weights (with indices), is_gray_scale, imgs (+ img_hw0, img_hw)."""
+
+    def __init__(self, dataset, batch_size, shuffle=True, sampler=None, drop_last=False, device=None, workers=None):
+        if not getattr(dataset, "augment", False):
+            raise ValueError("DeviceTrainLoader builds augmented training batches: the dataset has augment=False "
+                             "(build evaluation batches with DeviceEvalLoader)")
+        if getattr(dataset, "rect", False):
+            raise ValueError("DeviceTrainLoader builds mosaic batches: rect=True training (letterbox after load_image) "
+                             "is not supported")
+        self.dataset = dataset
+        self.batch_size = int(batch_size)
+        self._index = torch.utils.data.DataLoader(range(len(dataset.img_files)), batch_size=self.batch_size,
+                                                  shuffle=shuffle, sampler=sampler, drop_last=drop_last,
+                                                  collate_fn=list)
+        self.sampler = self._index.sampler
+        self.device = None if device is None else torch.device(device)
+        self.workers = workers or min(8, os.cpu_count() or 1)
+        self._pool = None
+        self._canvas = None
+
+    def __len__(self):
+        return len(self._index)
+
+    def __iter__(self):
+        for indices in self._index:
+            yield self.device_batch(self.host_batch(indices))
+
+    def _read(self, index):
+        ds = self.dataset
+        imgs = getattr(ds, "imgs", None)
+        if imgs is not None and imgs[index] is not None:         # --cache-images: load_image's output
+            img, hw = imgs[index], tuple(ds.img_hw[index])
+        else:
+            import cv2
+            path = ds.img_files[index]
+            img = cv2.imread(path, flags=cv2.IMREAD_GRAYSCALE) if ds.is_gray_scale else cv2.imread(path)
+            if img is None:
+                raise FileNotFoundError("Image Not Found " + path)
+            hw = train_tile_size(img.shape[0], img.shape[1], ds.img_size)
+        img = np.ascontiguousarray(img)
+        if img.ndim == 2:
+            img = img[:, :, None]
+        if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != (1 if ds.is_gray_scale else 3):
+            raise ValueError("%s: expected an HWC uint8 %s image" % (ds.img_files[index],
+                                                                    "gray-scale" if ds.is_gray_scale else "colour"))
+        return img, hw
+
+    def draws(self, indices):
+        """The random draws of the items of one batch, in __getitem__'s order: per item (index, xc, yc, the 4 tile
+        indices, (angle, scale, tx, ty, shear x, shear y), HSV gains or None, flip)."""
+        import random
+        ds = self.dataset
+        s, hyp = ds.img_size, ds.hyp
+        out = []
+        for index in indices:
+            if getattr(ds, "image_weights", False):
+                index = ds.indices[index]
+            xc, yc = [int(random.uniform(s * 0.5, s * 1.5)) for _ in range(2)]
+            tiles = [index] + [random.randint(0, len(ds.labels) - 1) for _ in range(3)]
+            a = random.uniform(-hyp["degrees"], hyp["degrees"])
+            sc = random.uniform(1 - hyp["scale"], 1 + hyp["scale"])
+            tx = random.uniform(-hyp["translate"], hyp["translate"])
+            ty = random.uniform(-hyp["translate"], hyp["translate"])
+            shx = random.uniform(-hyp["shear"], hyp["shear"])
+            shy = random.uniform(-hyp["shear"], hyp["shear"])
+            gains = None
+            if not ds.is_gray_scale:
+                gains = np.random.uniform(-1, 1, 3) * [hyp["hsv_h"], hyp["hsv_s"], hyp["hsv_v"]] + 1
+            flip = random.random() < 0.5
+            out.append((index, xc, yc, tiles, (a, sc, tx, ty, shx, shy), gains, flip))
+        return out
+
+    def host_batch(self, indices):
+        """Draw, decode (threads) and plan the items of one batch on the host: tiles and their rectangles, the affine
+        map and its inverse, LUTs, flips, labels.  Returns (sources {index: (img, (h, w))}, [per-item dict])."""
+        import math
+        import cv2
+        ds = self.dataset
+        s = ds.img_size
+        draws = self.draws(indices)
+        need = sorted({i for d in draws for i in d[3]})
+        if self._pool is None:
+            self._pool = ThreadPoolExecutor(self.workers)
+        reads = list(self._pool.map(self._read, need)) if len(need) > 1 else [self._read(i) for i in need]
+        sources = dict(zip(need, reads))
+        plans = []
+        for index, xc, yc, tiles, (a, sc, tx, ty, shx, shy), gains, flip in draws:
+            rects, tile_labels = [], []
+            for k, i in enumerate(tiles):
+                h, w = sources[i][1]
+                (x1a, y1a, x2a, y2a), (x1b, y1b, x2b, y2b) = mosaic_rects(k, xc, yc, w, h, s)
+                if (x2a - x1a, y2a - y1a) != (max(x2b - x1b, 0), max(y2b - y1b, 0)):
+                    raise ValueError("%s: mosaic tile %d does not fit its rectangle" % (ds.img_files[i], k))
+                rects.append(((x1a, y1a, x2a, y2a), (x1b - x1a, y1b - y1a)))
+                tile_labels.append((ds.labels[i], w, h, x1a - x1b, y1a - y1b))
+            # random_affine(border=-s // 2) on the 2s x 2s canvas: M = S @ T @ R, as the reference composes it
+            border = -s // 2
+            R = np.eye(3)
+            R[:2] = cv2.getRotationMatrix2D(angle=a, center=(2 * s / 2, 2 * s / 2), scale=sc)
+            T = np.eye(3)
+            T[0, 2] = tx * (2 * s) + border
+            T[1, 2] = ty * (2 * s) + border
+            S = np.eye(3)
+            S[0, 1] = math.tan(shx * math.pi / 180)
+            S[1, 0] = math.tan(shy * math.pi / 180)
+            M = S @ T @ R
+            im = cv2.invertAffineTransform(M[:2])
+            plans.append(dict(index=index, tiles=tiles, rects=rects, M=M, im=im, flip=flip,
+                              lut=None if gains is None else hsv_luts(gains),
+                              labels=train_labels(tile_labels, s, M, sc, flip), path=ds.img_files[index]))
+        return sources, plans
+
+    def device_batch(self, planned):
+        """One host-to-device copy of the sources and both item tables, b2y_mosaic_u8 then b2y_affine_hsv_u8, one
+        copy of the targets."""
+        from .lib import AffineItem, MosaicItem
+        if not torch.cuda.is_available():
+            raise lib.B2YError("DeviceTrainLoader runs on the CUDA device only (no CPU fallback)")
+        if self.device is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        sources, plans = planned
+        s, B = self.dataset.img_size, len(plans)
+        cn = next(iter(sources.values()))[0].shape[2]
+        off_aff = C.sizeof(MosaicItem) * B
+        total = off_aff + C.sizeof(AffineItem) * B
+        offs = {}
+        for i, (img, _) in sources.items():
+            total = (total + 15) // 16 * 16
+            offs[i] = total
+            total += img.nbytes
+        dev = torch.empty(total, dtype=torch.uint8, device=self.device)
+        base = dev.data_ptr()
+        host = np.empty(total, np.uint8)
+        for i, (img, _) in sources.items():
+            host[offs[i]:offs[i] + img.nbytes] = img.reshape(-1)
+        mos, aff = (MosaicItem * B)(), (AffineItem * B)()
+        for k, p in enumerate(plans):
+            mos[k].slot = aff[k].slot = k
+            for t, (i, ((x1a, y1a, x2a, y2a), (dx, dy))) in enumerate(zip(p["tiles"], p["rects"])):
+                img, (h, w) = sources[i]
+                sh, sw = img.shape[:2]
+                mos[k].tiles[t] = lib.MosaicTile(src=base + offs[i], src_pitch=sw * cn, src_h=sh, src_w=sw, rs_h=h,
+                                                 rs_w=w, scale_x=1.0 / (w / sw), scale_y=1.0 / (h / sh), x1a=x1a,
+                                                 y1a=y1a, x2a=x2a, y2a=y2a, dx=dx, dy=dy)
+            aff[k].im[:] = [float(v) for v in p["im"].reshape(-1)]
+            if p["lut"] is not None:
+                C.memmove(aff[k].lut, p["lut"].ctypes.data, 768)
+                aff[k].hsv = 1
+            aff[k].flip = 1 if p["flip"] else 0
+        host[:off_aff] = np.frombuffer(bytes(mos), np.uint8)
+        host[off_aff:off_aff + C.sizeof(AffineItem) * B] = np.frombuffer(bytes(aff), np.uint8)
+        dev.copy_(torch.from_numpy(host))
+        if self._canvas is None or self._canvas.shape[0] < B or tuple(self._canvas.shape[1:]) != (2 * s, 2 * s, cn):
+            self._canvas = torch.empty((max(B, self.batch_size), 2 * s, 2 * s, cn), dtype=torch.uint8,
+                                       device=self.device)
+        out = torch.empty((B, cn, s, s), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            call("b2y_mosaic_u8", C.cast(mos, C.c_void_p), ptr(dev), B, ptr(self._canvas), self._canvas.shape[0], cn,
+                 s, stream_ptr())
+            call("b2y_affine_hsv_u8", C.cast(aff, C.c_void_p), C.c_void_p(base + off_aff), B, ptr(self._canvas),
+                 ptr(out), B, cn, s, stream_ptr())
+        labels = []
+        for k, p in enumerate(plans):
+            lo = torch.zeros((len(p["labels"]), 6))
+            if len(p["labels"]):
+                lo[:, 1:] = torch.from_numpy(p["labels"])
+            lo[:, 0] = k
+            labels.append(lo)
+        targets = torch.cat(labels, 0).to(self.device)
+        return out, targets, tuple(p["path"] for p in plans), (None,) * B

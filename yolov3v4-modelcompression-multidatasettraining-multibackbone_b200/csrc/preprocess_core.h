@@ -1,6 +1,6 @@
-// Per-pixel arithmetic of the device letterbox and evaluation batch loader (csrc/preprocess.cu), shared with the host
-// harnesses of the CPU tests (tests/host/letterbox_host.cpp, tests/host/area_host.cpp) so that the very same code is
-// checked against cv2's outputs without a GPU.
+// Per-pixel arithmetic of the device letterbox, evaluation and training batch loaders (csrc/preprocess.cu), shared with
+// the host harnesses of the CPU tests (tests/host/letterbox_host.cpp, area_host.cpp, augment_host.cpp) so that the very
+// same code is checked against cv2's outputs without a GPU.
 //
 // OpenCV 4.x modules/imgproc/src/resize.cpp, 8-bit INTER_LINEAR (fixed point, INTER_RESIZE_COEF_BITS = 11):
 //   fx = (float)((dx + 0.5) * scale_x - 0.5), sx = floor(fx), fx -= sx; columns clamp (sx < 0 -> fx = 0, sx = 0;
@@ -71,6 +71,34 @@ B2Y_HD void b2y_lb_coeff(int d, double scale, int src, bool clamp, int& s, int& 
     s = si;
 }
 
+// The taps of resized pixel (rx, ry): source columns sx, x1 with weights a0, a1; rows y0, y1 with weights b0, b1.
+struct b2y_lb_taps {
+    int sx, x1, y0, y1, a0, a1, b0, b1;
+};
+
+B2Y_HD b2y_lb_taps b2y_lb_pixel_taps(const b2y_lb_params& p, int rx, int ry) {
+    b2y_lb_taps t;
+    int sy;
+    b2y_lb_coeff(rx, p.scale_x, p.src_w, true, t.sx, t.a0, t.a1);
+    b2y_lb_coeff(ry, p.scale_y, p.src_h, false, sy, t.b0, t.b1);
+    t.x1 = t.sx + 1 < p.src_w ? t.sx + 1 : p.src_w - 1;
+    int y0 = sy < 0 ? 0 : sy, y1 = sy + 1 < 0 ? 0 : sy + 1;
+    t.y0 = y0 < p.src_h ? y0 : p.src_h - 1;
+    t.y1 = y1 < p.src_h ? y1 : p.src_h - 1;
+    return t;
+}
+
+// Channel sc of the resized pixel whose taps are t.
+B2Y_HD int b2y_lb_value(const unsigned char* src, const b2y_lb_params& p, const b2y_lb_taps& t, int sc) {
+    const int C = p.channels;
+    const unsigned char* r0 = src + (long long)t.y0 * p.src_pitch;
+    const unsigned char* r1 = src + (long long)t.y1 * p.src_pitch;
+    const int h0 = (int)r0[t.sx * C + sc] * t.a0 + (int)r0[t.x1 * C + sc] * t.a1;
+    const int h1 = (int)r1[t.sx * C + sc] * t.a0 + (int)r1[t.x1 * C + sc] * t.a1;
+    const int v = (((t.b0 * (h0 >> 4)) >> 16) + ((t.b1 * (h1 >> 4)) >> 16) + 2) >> 2;
+    return v < 0 ? 0 : (v > 255 ? 255 : v);
+}
+
 // One output pixel (all channels): dst is planar [channels][dst_h][dst_w].
 B2Y_HD void b2y_lb_pixel(const unsigned char* src, unsigned char* dst, const b2y_lb_params& p, int x, int y) {
     const int C = p.channels;
@@ -86,23 +114,8 @@ B2Y_HD void b2y_lb_pixel(const unsigned char* src, unsigned char* dst, const b2y
         for (int c = 0; c < C; ++c) out[c * plane] = s[p.swap_rb ? C - 1 - c : c];
         return;
     }
-    int sx, a0, a1, sy, b0, b1;
-    b2y_lb_coeff(rx, p.scale_x, p.src_w, true, sx, a0, a1);
-    b2y_lb_coeff(ry, p.scale_y, p.src_h, false, sy, b0, b1);
-    const int x1 = sx + 1 < p.src_w ? sx + 1 : p.src_w - 1;
-    int y0 = sy < 0 ? 0 : sy, y1 = sy + 1 < 0 ? 0 : sy + 1;
-    y0 = y0 < p.src_h ? y0 : p.src_h - 1;
-    y1 = y1 < p.src_h ? y1 : p.src_h - 1;
-    const unsigned char* r0 = src + (long long)y0 * p.src_pitch;
-    const unsigned char* r1 = src + (long long)y1 * p.src_pitch;
-    for (int c = 0; c < C; ++c) {
-        const int sc = p.swap_rb ? C - 1 - c : c;
-        const int h0 = (int)r0[sx * C + sc] * a0 + (int)r0[x1 * C + sc] * a1;
-        const int h1 = (int)r1[sx * C + sc] * a0 + (int)r1[x1 * C + sc] * a1;
-        int v = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
-        v = v < 0 ? 0 : (v > 255 ? 255 : v);
-        out[c * plane] = (unsigned char)v;
-    }
+    const b2y_lb_taps t = b2y_lb_pixel_taps(p, rx, ry);
+    for (int c = 0; c < C; ++c) out[c * plane] = (unsigned char)b2y_lb_value(src, p, t, p.swap_rb ? C - 1 - c : c);
 }
 
 B2Y_HD void b2y_lb_set_scales(b2y_lb_params& p) {
@@ -252,6 +265,159 @@ B2Y_HD void b2y_load_pixel(const unsigned char* src, const b2y_area_params& p, i
         return;
     }
     for (int c = 0; c < C; ++c) out[c * plane] = (unsigned char)b2y_area_value(src, p, rx, ry, swap_rb ? C - 1 - c : c);
+}
+
+// ---- training-time augmentation (LoadImagesAndLabels(augment=True).__getitem__, utils/datasets.py:419-501) ----
+// Mosaic tiles (load_mosaic, :553-608): a canvas pixel inside a tile's rectangle is the tile pixel at (x + dx, y + dy);
+// an uncached tile is load_image's cv2.resize(INTER_LINEAR) of its source, i.e. b2y_lb_value.  cv::resize takes the
+// INTER_AREA 2 x 2 block mean for an exact 2x downscale; the bilinear weights there are 1024 / 1024 on both axes and
+// give the same (a + b + c + d + 2) >> 2, so this one path covers it.
+B2Y_HD int b2y_tile_value(const unsigned char* src, const b2y_lb_params& p, int tx, int ty, int sc) {
+    if (p.rs_w == p.src_w && p.rs_h == p.src_h) return src[(long long)ty * p.src_pitch + (long long)tx * p.channels + sc];
+    const b2y_lb_taps t = b2y_lb_pixel_taps(p, tx, ty);
+    return b2y_lb_value(src, p, t, sc);
+}
+
+// cv2.warpAffine(src, M, dsize, INTER_LINEAR, BORDER_CONSTANT) for 8-bit images, OpenCV 4.x imgwarp.cpp: im = the
+// inverse of M (invertAffineTransform, in double, computed by the caller).  Per output pixel, with AB_BITS = 10 and
+// INTER_BITS = 5: X = (cvRound((im1 * y + im2) * 1024) + 16 + cvRound(im0 * x * 1024)) >> 5 (and Y with im3..im5);
+// the top-left tap is (X >> 5, Y >> 5), the fraction (X & 31, Y & 31).  The 32 x 32 fixed-point table of
+// initInterTab2D holds (1 - fy)(1 - fx), (1 - fy) fx, fy (1 - fx), fy fx times 32768 for fx, fy = k / 32: exact
+// products that sum to 32768, so OpenCV's rounding correction never fires.  The byte is (sum w * S + (1 << 14)) >> 15;
+// a tap outside the source reads the border value.
+struct b2y_warp_taps {
+    int sx, sy, w[4];
+};
+
+B2Y_HD int b2y_dround(double v) {                        // cvRound(double): nearest, ties to even
+#if defined(__CUDA_ARCH__)
+    return __double2int_rn(v);
+#else
+    return (int)std::nearbyint(v);
+#endif
+}
+
+B2Y_HD double b2y_dadd(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dadd_rn(a, b);
+#else
+    volatile double t = a + b;
+    return t;
+#endif
+}
+
+B2Y_HD b2y_warp_taps b2y_warp_pixel_taps(const double* im, int x, int y) {
+    const int X0 = b2y_dround(b2y_dmul(b2y_dadd(b2y_dmul(im[1], (double)y), im[2]), 1024.0)) + 16;
+    const int Y0 = b2y_dround(b2y_dmul(b2y_dadd(b2y_dmul(im[4], (double)y), im[5]), 1024.0)) + 16;
+    const int X = (X0 + b2y_dround(b2y_dmul(b2y_dmul(im[0], (double)x), 1024.0))) >> 5;
+    const int Y = (Y0 + b2y_dround(b2y_dmul(b2y_dmul(im[3], (double)x), 1024.0))) >> 5;
+    b2y_warp_taps t;
+    t.sx = X >> 5;
+    t.sy = Y >> 5;
+    const int fx = X & 31, fy = Y & 31;
+    t.w[0] = (32 - fy) * (32 - fx) * 32;
+    t.w[1] = (32 - fy) * fx * 32;
+    t.w[2] = fy * (32 - fx) * 32;
+    t.w[3] = fy * fx * 32;
+    return t;
+}
+
+// Channel c of the warped pixel: src HWC [h][w][C] with row pitch `pitch` bytes.
+B2Y_HD int b2y_warp_value(const unsigned char* src, int h, int w, int C, long long pitch, const b2y_warp_taps& t, int c,
+                          int border) {
+    const bool x0 = t.sx >= 0 && t.sx < w, x1 = t.sx + 1 >= 0 && t.sx + 1 < w;
+    const bool y0 = t.sy >= 0 && t.sy < h, y1 = t.sy + 1 >= 0 && t.sy + 1 < h;
+    const unsigned char* p = src + (long long)t.sy * pitch + (long long)t.sx * C + c;
+    const int sum = t.w[0] * (y0 && x0 ? (int)p[0] : border) + t.w[1] * (y0 && x1 ? (int)p[C] : border) +
+                    t.w[2] * (y1 && x0 ? (int)p[pitch] : border) + t.w[3] * (y1 && x1 ? (int)p[pitch + C] : border);
+    const int v = (sum + (1 << 14)) >> 15;
+    return v < 0 ? 0 : (v > 255 ? 255 : v);
+}
+
+// cv2.cvtColor(COLOR_BGR2HSV) for 8-bit images (OpenCV 4.x color_hsv: integer tables, hsv_shift = 12, H in 0..179):
+// sdiv(v) = cvRound((255 << 12) / (double)v), hdiv(d) = cvRound((180 << 12) / (6. * d)), both 0 at 0.
+B2Y_HD void b2y_bgr2hsv(int b, int g, int r, int& h, int& s, int& v) {
+    v = b > g ? b : g;
+    v = v > r ? v : r;
+    int vmin = b < g ? b : g;
+    vmin = vmin < r ? vmin : r;
+    const int diff = v - vmin;
+    const int vr = v == r ? -1 : 0, vg = v == g ? -1 : 0;
+#if defined(__CUDA_ARCH__)
+    const int sdiv = v ? __double2int_rn(__ddiv_rn((double)(255 << 12), (double)v)) : 0;
+    const int hdiv = diff ? __double2int_rn(__ddiv_rn((double)(180 << 12), 6.0 * diff)) : 0;
+#else
+    const int sdiv = v ? (int)std::nearbyint((double)(255 << 12) / (double)v) : 0;
+    const int hdiv = diff ? (int)std::nearbyint((double)(180 << 12) / (6.0 * diff)) : 0;
+#endif
+    s = (diff * sdiv + (1 << 11)) >> 12;
+    int hh = (vr & (g - b)) + (~vr & ((vg & (b - r + 2 * diff)) + (~vg & (r - g + 4 * diff))));
+    hh = (hh * hdiv + (1 << 11)) >> 12;
+    hh += hh < 0 ? 180 : 0;
+    h = hh < 0 ? 0 : (hh > 255 ? 255 : hh);
+}
+
+B2Y_HD float b2y_ffma(float a, float b, float c) {
+#if defined(__CUDA_ARCH__)
+    return __fmaf_rn(a, b, c);
+#else
+    return std::fmaf(a, b, c);
+#endif
+}
+
+B2Y_HD float b2y_fsub(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fsub_rn(a, b);
+#else
+    volatile float t = a - b;
+    return t;
+#endif
+}
+
+// cv2.cvtColor(COLOR_HSV2BGR) for 8-bit images as OpenCV 4.x's default (vectorised, AVX2) dispatch computes it, in
+// float: h = H * (6.f / 180), s = S * (1.f / 255), v = V * (1.f / 255); sector = trunc(h) mod 6, f = h - trunc(h);
+// tab = {v, v * (1 - s), v * fma(-s, f, 1), v * fma(-s, 1 - f, 1)} -- the two inner products FUSED with the
+// subtraction, as the optimised build contracts them (the scalar path, cv2.setUseOptimized(False), rounds them
+// separately and differs in the last bit on about 1 in 7000 bytes); each output byte is trunc(tab[k] * 255.f).
+// The vector loop covers whole blocks of 32 pixels of a row; every row width the training loader uses (img_size is a
+// multiple of 32) runs it end to end.
+B2Y_HD void b2y_hsv2bgr(int H, int S, int V, int& b, int& g, int& r) {
+    const float hh = b2y_fmul((float)H, 6.0f / 180), s = b2y_fmul((float)S, 1.0f / 255), v = b2y_fmul((float)V, 1.0f / 255);
+    const float pre = truncf(hh), f = b2y_fsub(hh, pre);
+    const float t1 = b2y_fmul(v, b2y_fsub(1.f, s));
+    const float t2 = b2y_fmul(v, b2y_ffma(-s, f, 1.f));
+    const float t3 = b2y_fmul(v, b2y_ffma(-s, b2y_fsub(1.f, f), 1.f));
+    const int sh = 4 * ((int)pre % 6);
+    // sector_data of color_hsv ({1,3,0}, {1,0,2}, {3,0,1}, {0,2,1}, {0,1,3}, {2,1,0}): the tab index of b, g and r
+    // per sector, one nibble per sector
+    const int kb = (0x200311 >> sh) & 15, kg = (0x112003 >> sh) & 15, kr = (0x031120 >> sh) & 15;
+    b = (int)b2y_fmul(kb == 0 ? v : (kb == 1 ? t1 : (kb == 2 ? t2 : t3)), 255.f);
+    g = (int)b2y_fmul(kg == 0 ? v : (kg == 1 ? t1 : (kg == 2 ? t2 : t3)), 255.f);
+    r = (int)b2y_fmul(kr == 0 ? v : (kr == 1 ? t1 : (kr == 2 ? t2 : t3)), 255.f);
+}
+
+// One output pixel of a training batch after the mosaic canvas: warp (border 114), augment_hsv's BGR2HSV -> LUT ->
+// HSV2BGR when lut != nullptr (colour only), then written reversed (BGR -> RGB) into channel planes out[c * plane].
+// (x, y) is the position in the warped image; the caller applies the left-right flip by choosing where out points.
+B2Y_HD void b2y_augment_pixel(const unsigned char* canvas, int ch, int cw, int C, const double* im,
+                              const unsigned char* lut, int x, int y, unsigned char* out, long long plane) {
+    const b2y_warp_taps t = b2y_warp_pixel_taps(im, x, y);
+    const long long pitch = (long long)cw * C;
+    if (C == 3) {
+        int b = b2y_warp_value(canvas, ch, cw, 3, pitch, t, 0, 114);
+        int g = b2y_warp_value(canvas, ch, cw, 3, pitch, t, 1, 114);
+        int r = b2y_warp_value(canvas, ch, cw, 3, pitch, t, 2, 114);
+        if (lut) {
+            int h, s, v;
+            b2y_bgr2hsv(b, g, r, h, s, v);
+            b2y_hsv2bgr(lut[h], lut[256 + s], lut[512 + v], b, g, r);
+        }
+        out[0] = (unsigned char)r;
+        out[plane] = (unsigned char)g;
+        out[2 * plane] = (unsigned char)b;
+        return;
+    }
+    for (int c = 0; c < C; ++c) out[c * plane] = (unsigned char)b2y_warp_value(canvas, ch, cw, C, pitch, t, c, 114);
 }
 
 #endif  // B2Y_PREPROCESS_CORE_H_
