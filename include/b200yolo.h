@@ -235,6 +235,9 @@ typedef struct b2y_qconv_desc {
     float q_lo, q_hi;     /* clamp range, -2^(b-1) .. 2^(b-1)-1 */
     int out_kind;         /* B2Y_OUT_I8: requantised int8; B2Y_OUT_F32/F16: fake-quant value (heads: linear) */
     int requant;          /* 0: write act(acc*acc_scale+bias) without requantisation (linear head, ptq_cos.py:718) */
+    int clamp_addends;    /* b2y_qconv2d_shortcut_fwd only.  0: the addends are rounded onto scale_x / scale_a but not
+                             clamped (COSPTQuantizedShortcut, google QuantizedShortcut_min); 1: their codes are also clamped
+                             to [sum_lo, sum_hi] before the add (google QuantizedShortcut_max, quantized_google.py:294) */
 } b2y_qconv_desc;
 /* INT8 conv on int8 wgmma with int32 accumulation (exact whenever the fp32 reference is). */
 int b2y_qconv2d_fwd(const b2y_qconv_desc* d, const void* x_i8, const void* w_i8, const float* bias, void* y,
@@ -260,6 +263,12 @@ int b2y_requant_i8(const void* x, long long x_pitch, void* out, long long out_pi
                    float s_in, float s_out, float lo, float hi, void* stream);
 int b2y_upsample_nearest_i8(const void* x, long long x_pitch, void* y, long long y_pitch, int batch, int in_h,
                             int in_w, int c, int scale, void* stream);
+/* Max-pool of int8 NHWC codes: the plain nn.MaxPool2d (and ZeroPad2d((0,1,0,1)) + MaxPool2d(2, 1)) that the google-QAT
+ * graph keeps over fake-quantised values (models.py:207-214).  Same shapes and pad_mode as b2y_maxpool: 0 = symmetric
+ * (k-1)//2 padding with -inf, 1 = one zero row / column on the right and bottom (a zero value is code 0 on any grid).
+ * c a multiple of 16, pitches multiples of 16 and >= c, x and y 16-byte aligned; y_pitch may exceed c (a concat slot). */
+int b2y_maxpool_i8(const void* x, long long x_pitch, void* y, long long y_pitch, int batch, int in_h, int in_w, int c,
+                   int ksize, int stride, int pad_mode, void* stream);
 int b2y_stem_conv_fwd_q(const b2y_conv_desc* d, const float* x_nchw, const float* w_q, const float* bias_q, void* y_i8,
                         float out_scale, float lo, float hi, void* stream);
 

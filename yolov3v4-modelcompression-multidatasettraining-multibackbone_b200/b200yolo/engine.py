@@ -541,6 +541,17 @@ class Engine:
             from .qat import QatRunner
             if model.training:
                 return QatRunner(model).forward(x)
+            if model.quantized == 1:
+                # eval of a google-QAT model whose structure qengine.int8_graph_refusal accepts: the integer network,
+                # bit-identical to the module forwards; the plan re-packs itself when training has moved the QAT state
+                key = (tuple(x.shape), 'q1', x.device.index)
+                plan = self.plans.get(key)
+                if plan is None:
+                    from .qengine import QPlan, int8_graph_refusal
+                    if int8_graph_refusal(model) is None:
+                        plan = self.plans[key] = QPlan(model, tuple(x.shape), x.device)
+                if plan is not None:
+                    return plan.forward(x)
             with torch.no_grad():
                 return QatRunner(model).forward(x)
         if model.quantized != 3:

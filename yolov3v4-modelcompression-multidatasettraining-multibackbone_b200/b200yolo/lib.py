@@ -85,7 +85,7 @@ class QConvDesc(C.Structure):
         ("conv", ConvDesc),
         ("acc_scale", C.c_float), ("out_scale", C.c_float),
         ("q_lo", C.c_float), ("q_hi", C.c_float),
-        ("out_kind", C.c_int), ("requant", C.c_int),
+        ("out_kind", C.c_int), ("requant", C.c_int), ("clamp_addends", C.c_int),
     ]
 
 
@@ -138,6 +138,7 @@ _PROTOS = {
     "b2y_qshortcut_i8": (i32, [vp, ll, vp, ll, vp, ll, ll, i32, f32, f32, f32, f32, f32, f32, f32, vp]),
     "b2y_requant_i8": (i32, [vp, ll, vp, ll, ll, i32, f32, f32, f32, f32, vp]),
     "b2y_upsample_nearest_i8": (i32, [vp, ll, vp, ll, i32, i32, i32, i32, i32, vp]),
+    "b2y_maxpool_i8": (i32, [vp, ll, vp, ll, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b2y_stem_conv_fwd_q": (i32, [C.POINTER(ConvDesc), vp, vp, vp, vp, f32, f32, f32, vp]),
     "b2y_bn_act_bwd_reduce": (i32, [vp, ll, vp, ll, vp, vp, vp, vp, vp, vp, vp, ll, i32, i32, f32, i32, vp]),
     "b2y_conv2d_bwd_data": (i32, [C.POINTER(ConvDesc), vp, vp, vp, i32, i32, i32, vp, vp]),

@@ -184,6 +184,7 @@ struct EpilogueArgs {
     const void* qres = nullptr;
     long long qres_pitch = 0;
     float qs_a_in = 1.f, qs_x = 1.f, qs_a = 1.f, qs_sum = 1.f, qs_lo = -128.f, qs_hi = 127.f;
+    int qs_clamp = 0;
 };
 
 // Generic implicit-GEMM launch description: A = NHWC activation-like tensor gathered tap by tap, B = [Nout][ntaps*C].
@@ -326,9 +327,10 @@ int gemm_conv_launch(const GemmConvSpec& g, const EpilogueArgs& e, cudaStream_t 
             p.qs_rsum = 1.f / e.qs_sum;
             p.qs_lo = e.qs_lo;
             p.qs_hi = e.qs_hi;
+            p.qs_clamp = e.qs_clamp;
             p.qs_cx = e.out_scale / e.qs_sum;
             p.qs_ca = e.qs_a_in / e.qs_sum;
-            p.qs_simple = e.out_scale >= e.qs_x && e.qs_a_in >= e.qs_a && p.qs_cx <= 4096.f && p.qs_ca <= 4096.f &&
+            p.qs_simple = !e.qs_clamp && e.out_scale >= e.qs_x && e.qs_a_in >= e.qs_a && p.qs_cx <= 4096.f && p.qs_ca <= 4096.f &&
                           p.qs_cx >= 1.f / 4096.f && p.qs_ca >= 1.f / 4096.f && e.qs_lo >= -128.f && e.qs_hi <= 127.f;
         }
     }
@@ -810,5 +812,6 @@ extern "C" int b2y_qconv2d_shortcut_fwd(const b2y_qconv_desc* d, const void* x_i
     e.qs_sum = scale_sum;
     e.qs_lo = sum_lo;
     e.qs_hi = sum_hi;
+    e.qs_clamp = d->clamp_addends ? 1 : 0;
     return conv_tc_launch(CONV_KIND_I8, &d->conv, x_i8, w_i8, e, static_cast<cudaStream_t>(stream));
 }

@@ -73,6 +73,7 @@ struct ConvTcParams {
     const int8_t* qres;     // the other addend's int8 codes (NHWC) or null
     long long qres_pitch;
     float qs_rx, qs_x, qs_a_in, qs_ra, qs_a, qs_rsum, qs_lo, qs_hi;
+    int qs_clamp;           // the addend codes are clamped to [qs_lo, qs_hi] too (google QuantizedShortcut_max)
     int qs_simple;          // both addend roundings are identities: code = clamp(rha(q*qs_cx + a*qs_ca))
     float qs_cx, qs_ca;     // out_scale / scale_sum, a_in / scale_sum
 };
@@ -649,8 +650,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             const int8_t* ab = reinterpret_cast<const int8_t*>(qa);
 #pragma unroll
                             for (int j = 0; j < 32; ++j) {
-                                const float xf = round_half_away(v[j] * p.out_scale * p.qs_rx) * p.qs_x;   // rounded, NOT clamped
-                                const float af = round_half_away((float)ab[j] * p.qs_a_in * p.qs_ra) * p.qs_a;
+                                float xr = round_half_away(v[j] * p.out_scale * p.qs_rx);   // rounded, clamped in
+                                float ar = round_half_away((float)ab[j] * p.qs_a_in * p.qs_ra);  // qs_clamp mode only
+                                if (p.qs_clamp) {
+                                    xr = fminf(fmaxf(xr, p.qs_lo), p.qs_hi);
+                                    ar = fminf(fmaxf(ar, p.qs_lo), p.qs_hi);
+                                }
+                                const float xf = xr * p.qs_x, af = ar * p.qs_a;
                                 const float q = round_half_away((xf + af) * p.qs_rsum);
                                 v[j] = fminf(fmaxf(q, p.qs_lo), p.qs_hi);
                             }

@@ -478,6 +478,101 @@ extern "C" int b2y_upsample_nearest_i8(const void* x, long long x_pitch, void* y
     return B2Y_OK;
 }
 
+// Max-pool of int8 NHWC codes (the plain nn.MaxPool2d of the google-QAT graph, models.py:207-214).  Every input sits on
+// one power-of-two grid, so the max of the codes is the code of the max.  16 channels (one 16-byte vector) per thread,
+// four signed-byte maxima per __vmaxs4.
+__device__ __forceinline__ uint4 vmax_s8x16(uint4 a, uint4 b) {
+    return make_uint4(__vmaxs4(a.x, b.x), __vmaxs4(a.y, b.y), __vmaxs4(a.z, b.z), __vmaxs4(a.w, b.w));
+}
+
+// any window: out-of-range taps are skipped (-inf padding); zero_pad adds code 0 when the window touches the right or
+// bottom pad of ZeroPad2d((0,1,0,1))
+__global__ void maxpool_i8_kernel(const int8_t* __restrict__ x, long long xp, int8_t* __restrict__ y, long long yp,
+                                  int H, int W, int CV, int k, int stride, int pad, int Ho, int Wo, long long total,
+                                  int zero_pad) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int cv = (int)(idx % CV);
+        const long long pix = idx / CV;
+        const int xo = (int)(pix % Wo);
+        const int yo = (int)((pix / Wo) % Ho);
+        const long long n = pix / ((long long)Wo * Ho);
+        uint4 m = make_uint4(0x80808080u, 0x80808080u, 0x80808080u, 0x80808080u);
+        bool touched_pad = false;
+        for (int kh = 0; kh < k; ++kh) {
+            const int yi = yo * stride - pad + kh;
+            for (int kw = 0; kw < k; ++kw) {
+                const int xi = xo * stride - pad + kw;
+                if (yi < 0 || yi >= H || xi < 0 || xi >= W) {
+                    touched_pad = true;
+                    continue;
+                }
+                m = vmax_s8x16(m, __ldg(reinterpret_cast<const uint4*>(x + ((n * H + yi) * W + xi) * xp) + cv));
+            }
+        }
+        if (zero_pad && touched_pad) m = vmax_s8x16(m, make_uint4(0u, 0u, 0u, 0u));
+        reinterpret_cast<uint4*>(y + pix * yp)[cv] = m;
+    }
+}
+
+// Stride-1 "same" pooling (SPP: k = 5 / 9 / 13) over a map of up to POOL_PLANE_I8_MAX pixels: one CTA holds the plane of
+// one image x 16 channels in shared memory and takes the window as a row pass then a column pass (2k loads, not k*k),
+// as maxpool_plane_kernel does for fp16.  Clipping the window at the border is the -inf padding.
+constexpr int POOL_PLANE_I8_MAX = 1024;   // 32 x 32 pixels, 2 x 16 KB of shared memory
+__global__ void __launch_bounds__(256) maxpool_i8_plane_kernel(const int8_t* __restrict__ x, long long xp,
+                                                               int8_t* __restrict__ y, long long yp, int H, int W,
+                                                               int CV, int k) {
+    __shared__ uint4 sx[POOL_PLANE_I8_MAX];
+    __shared__ uint4 sr[POOL_PLANE_I8_MAX];
+    const long long n = blockIdx.x / CV;
+    const int cv = blockIdx.x - (int)(n * CV);
+    const int HW = H * W, pad = (k - 1) / 2;
+    for (int i = threadIdx.x; i < HW; i += blockDim.x)
+        sx[i] = __ldg(reinterpret_cast<const uint4*>(x + (n * HW + i) * xp) + cv);
+    __syncthreads();
+    for (int i = threadIdx.x; i < HW; i += blockDim.x) {
+        const int yi = i / W, xo = i - yi * W;
+        const int x0 = max(xo - pad, 0), x1 = min(xo - pad + k, W);
+        uint4 m = sx[yi * W + x0];
+        for (int xi = x0 + 1; xi < x1; ++xi) m = vmax_s8x16(m, sx[yi * W + xi]);
+        sr[i] = m;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < HW; i += blockDim.x) {
+        const int yo = i / W, xo = i - yo * W;
+        const int y0 = max(yo - pad, 0), y1 = min(yo - pad + k, H);
+        uint4 m = sr[y0 * W + xo];
+        for (int yi = y0 + 1; yi < y1; ++yi) m = vmax_s8x16(m, sr[yi * W + xo]);
+        reinterpret_cast<uint4*>(y + (n * HW + i) * yp)[cv] = m;
+    }
+}
+
+extern "C" int b2y_maxpool_i8(const void* x, long long x_pitch, void* y, long long y_pitch, int batch, int in_h,
+                              int in_w, int c, int ksize, int stride, int pad_mode, void* stream) {
+    if (!x || !y || batch < 1 || in_h < 1 || in_w < 1 || c < 16 || c % 16 != 0 || x_pitch < c || y_pitch < c ||
+        x_pitch % 16 != 0 || y_pitch % 16 != 0 || ksize < 1 || stride < 1 || (pad_mode != 0 && pad_mode != 1))
+        return B2Y_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15)) return B2Y_ERR_INVALID;
+    const int pad = pad_mode == 1 ? 0 : (ksize - 1) / 2;
+    const int extra = pad_mode == 1 ? 1 : 2 * pad;      // ZeroPad2d((0,1,0,1)) widens by one on one side only
+    if (in_h + extra < ksize || in_w + extra < ksize) return B2Y_ERR_INVALID;
+    const int Ho = (in_h + extra - ksize) / stride + 1, Wo = (in_w + extra - ksize) / stride + 1;
+    const int CV = c / 16;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (pad_mode == 0 && stride == 1 && (ksize & 1) && in_h * in_w <= POOL_PLANE_I8_MAX &&
+        (long long)batch * CV <= 0x7fffffffLL) {
+        maxpool_i8_plane_kernel<<<batch * CV, 256, 0, st>>>(reinterpret_cast<const int8_t*>(x), x_pitch,
+                                                            reinterpret_cast<int8_t*>(y), y_pitch, in_h, in_w, CV, ksize);
+    } else {
+        const long long total = (long long)batch * Ho * Wo * CV;
+        maxpool_i8_kernel<<<grid_for(total, 256), 256, 0, st>>>(reinterpret_cast<const int8_t*>(x), x_pitch,
+                                                               reinterpret_cast<int8_t*>(y), y_pitch, in_h, in_w, CV,
+                                                               ksize, stride, pad, Ho, Wo, total, pad_mode);
+    }
+    B2Y_CUDA_CHECK(cudaGetLastError());
+    return B2Y_OK;
+}
+
 // First quantised layer: the image is float (not on an int8 grid), so conv 0 runs in fp32 on the fake-quantised
 // weights (exactly what the reference does, ptq_cos.py:288-296) and only its output is requantised to int8.
 __global__ void __launch_bounds__(128)
