@@ -2,7 +2,8 @@
 
 The reference ships its cfg files under cfg/**; they are data, not code, and are not copied into this repo.
 This module re-creates the architectures (YOLOv3 / Darknet-53, YOLOv3-tiny, YOLOv4 / CSPDarknet-53 + SPP + PAN,
-YOLOv4-tiny, YOLOv2 / Darknet-19 and YOLOv2-tiny with one 5-anchor head) from their published structure so that tests and bench.py work on a box without /root/reference.
+YOLOv4-tiny, YOLOv2 / Darknet-19 and YOLOv2-tiny with one 5-anchor head, the MobileNetV3 and GhostNet backbones under a
+YOLOv3 head) from their published structure so that tests and bench.py work on a box without /root/reference.
 tests/test_cfg_parity.py checks (when the reference is present) that the generated text parses to the same
 module definitions as the reference's own cfg files.
 """
@@ -214,6 +215,61 @@ def yolov3_mobilenet(classes=80):
     return c.text()
 
 
+def yolov3_ghost(classes=80):
+    """YOLOv3 head on a GhostNet backbone (the reference's cfg/yolov3-ghostnet/yolov3-ghost-coco.cfg).  A ghost module is
+    a 1x1 primary conv, a 3x3 depthwise cheap operation ([convolutional] groups=C) and a concat of the two; a bottleneck
+    is an expanding ghost module, a k x k stride-2 depthwise conv when it downsamples, [se], and a linear ghost module,
+    with a shortcut from its input, through a depthwise conv and a 1x1 conv where the width or the size changes."""
+    c = _Cfg([("batch", 16), ("subdivisions", 1)] + _net()[2:])
+    nout = 3 * (classes + 5)
+
+    def conv(filters, size, stride=1, act="none", groups=1):
+        return c.block("convolutional", ("batch_normalize", 1), ("filters", filters), ("size", size), ("stride", stride),
+                       ("pad", size // 2), ("groups", groups), ("activation", act))
+
+    def ghost(half, act):
+        primary = conv(half, 1, act=act)
+        conv(half, 3, act=act, groups=half)
+        return c.route(-1, primary)
+
+    width = 16
+    start = conv(width, 3, 2, act="relu")
+    # (expanded half width, output half width, kernel, stride, se, shortcut block without its activation key)
+    blocks = ((8, 8, 3, 1, 0, 0), (24, 12, 3, 2, 0, 0), (36, 12, 3, 1, 0, 0), (36, 20, 5, 2, 1, 0), (60, 20, 3, 1, 1, 1),
+              (120, 40, 3, 2, 0, 0), (100, 40, 3, 1, 0, 0), (92, 40, 3, 1, 0, 0), (92, 40, 3, 1, 0, 0),
+              (240, 56, 3, 1, 1, 0), (336, 56, 3, 1, 1, 0), (336, 80, 5, 2, 1, 0), (480, 80, 3, 1, 0, 0),
+              (480, 80, 3, 1, 1, 0), (480, 80, 3, 1, 0, 0), (480, 80, 3, 1, 1, 1))
+    for exp, out, k, stride, se, bare in blocks:
+        ghost(exp, "relu")
+        if stride == 2:
+            conv(2 * exp, k, 2, groups=2 * exp)
+        if se:
+            c.block("se", ("reduction", 4))
+        end = ghost(out, "none")
+        frm = start
+        if stride == 2 or 2 * out != width:     # the projected input is added to the block's output
+            c.route(start)
+            conv(width, k, stride, groups=width)
+            conv(2 * out, 1)
+            frm = end
+        c.block("shortcut", ("from", frm - c.n), *(() if bare else (("activation", "none"),)))
+        start, width = c.n - 1, 2 * out
+    conv(960, 1, act="relu")
+    for scale, (mid, mask, skip) in enumerate(((512, (6, 7, 8), None), (256, (3, 4, 5), 96), (128, (0, 1, 2), 45))):
+        if skip is not None:
+            c.route(-4)
+            conv(mid, 1, act="leaky")
+            c.upsample(2)
+            c.route(-1, skip)
+        for _ in range(3):
+            conv(mid, 1, act="leaky")
+            conv(mid * 2, 3, act="leaky")
+        c.block("convolutional", ("size", 1), ("stride", 1), ("pad", 0), ("filters", nout), ("groups", 1),
+                ("activation", "linear"))
+        c.yolo(mask, COCO_ANCHORS_V3, classes, 9, (("random", 1),))
+    return c.text()
+
+
 def _v2_head(c, classes):
     """One stride-32 head over all five anchors: 5 * (classes + 5) filters (425 for 80 classes)."""
     c.conv(5 * (classes + 5), 1, act="linear", bn=0)
@@ -250,7 +306,7 @@ def yolov2_tiny(classes=80):
 
 
 ARCHS = {"yolov3": yolov3, "yolov3-tiny": yolov3_tiny, "yolov4": yolov4, "yolov3-mobilenet": yolov3_mobilenet,
-         "yolov2": yolov2, "yolov2-tiny": yolov2_tiny}
+         "yolov3-ghost": yolov3_ghost, "yolov2": yolov2, "yolov2-tiny": yolov2_tiny}
 
 
 def cfg_text(name, classes=80):

@@ -156,7 +156,8 @@ class ActFn(torch.autograd.Function):
 
 
 def activation(x, name, maxabsscaler=False):
-    if name == 'linear':
+    # 'none' (GhostNet's cfg): the reference layers print a warning and leave the output unchanged
+    if name in ('linear', 'none'):
         return x
     return ActFn.apply(x, name, 0.25 if maxabsscaler else 0.1)
 
@@ -337,6 +338,59 @@ def dwconv_stats(x, w, b, k, s, p, link=None):
     """(mean, var) of dwconv(x, w) + b over batch and pixels, differentiable; `link` couples the backward with the
     quantised conv dwconv2d(x, W_q, ..., link) on the same input"""
     return DwConvStatsFn.apply(x, w, b, k, s, p, link)
+
+
+def check_groups(layer):
+    """dense (groups = 1) and depthwise (groups = in = out channels) QAT layers run; other groupings are refused"""
+    if layer.groups != 1 and not layer.groups == layer.in_channels == layer.out_channels:
+        raise NotImplementedError("grouped convolution (1 < groups < channels) in a %s layer"
+                                  % layer.__class__.__name__)
+    return layer.groups != 1
+
+
+def fold_batch_norm(layer, x, k, s, p, freeze_step):
+    """Training-mode BatchNorm fold of a google / TPSQ QAT conv layer with bn=1 (quantized_google.py:320-374,
+    quantized_TPSQ.py:404-440): the batch statistics of the float-weight conv (the mean shifted by the conv bias, the
+    unbiased variance), the running-statistics update seeded on the first call, and before `freeze_step` the fold on the
+    batch statistics, with their gradient, after it the fold on the running statistics.  Returns the folded weight and
+    bias and the DwGradLink the quantised depthwise conv on `x` must take (None for dense layers)."""
+    cb = layer.bias if layer.bias is not None else 0
+    link = None
+    if layer.groups == 1:
+        y1, s1, s2 = conv2d(x, layer.weight, k, s, p, want_stats=True)   # channel sums from the conv epilogue
+        n = float(y1.shape[0] * y1.shape[1] * y1.shape[2])
+        mean = s1 / n + cb
+        var = (s2 - s1 * (s1 / n)) / (n - 1.0)                           # torch.var: unbiased
+    elif float(layer.step) < freeze_step:
+        # the fold takes the batch statistics: both convolutions of the layer share one backward
+        link = DwGradLink()
+        mean, var = dwconv_stats(x, layer.weight, layer.bias, k, s, p, link)
+    else:
+        with torch.no_grad():                                            # only the running statistics read them
+            mean, var = dwconv_stats(x, layer.weight, layer.bias, k, s, p)
+    layer.batch_mean, layer.batch_var = mean, var
+    with torch.no_grad():
+        if float(layer.first_bn) == 0 and not bool(layer.running_mean.any()) and not bool(layer.running_var.any()):
+            layer.first_bn.add_(1)
+            layer.running_mean.add_(mean)
+            layer.running_var.add_(var)
+        else:
+            layer.running_mean.mul_(1 - layer.momentum).add_(mean * layer.momentum)
+            layer.running_var.mul_(1 - layer.momentum).add_(var * layer.momentum)
+    if float(layer.step) < freeze_step:
+        sc = layer.gamma / torch.sqrt(var + layer.eps)
+        bias = layer.beta + (cb - mean) * sc
+    else:
+        sc = layer.gamma / torch.sqrt(layer.running_var + layer.eps)
+        bias = layer.beta + (cb - layer.running_mean) * sc
+    return layer.weight * sc.reshape(-1, 1, 1, 1), bias.reshape(-1), link
+
+
+def qconv(layer, x, w, k, s, p, link=None):
+    """the layer's convolution on its quantised weights: the wgmma conv, or for groups = C the fp32 depthwise conv"""
+    if layer.groups == 1:
+        return conv2d(x, w, k, s, p)
+    return dwconv2d(x, w, k, s, p, link)
 
 
 def depthwise_block(block, d, x, training):

@@ -198,54 +198,21 @@ class TPSQ_BNFold_QuantizedConv2d_For_FPGA(nn.Conv2d):
 
     def forward(self, input):
         from b200yolo import qat
-        depthwise = self.groups != 1
-        if depthwise and not self.groups == self.in_channels == self.out_channels:
-            raise NotImplementedError("grouped convolution (1 < groups < channels) in a TPSQ layer")
+        qat.check_groups(self)
         if not input.is_cuda:
             raise RuntimeError("TPSQ layers run on the CUDA device only (no CPU fallback)")
         k, st, pd = self.kernel_size[0], self.stride[0], self.padding[0]
-        cb = self.bias if self.bias is not None else 0
         link = None
         if self.training:
             self.step += 1
             if self.bn:
-                if not depthwise:
-                    y1, s1, s2 = qat.conv2d(input, self.weight, k, st, pd, want_stats=True)
-                    n = float(y1.shape[0] * y1.shape[1] * y1.shape[2])
-                    mean = s1 / n + cb
-                    var = (s2 - s1 * (s1 / n)) / (n - 1.0)                # torch.var: unbiased
-                elif float(self.step) < self.freeze_step:
-                    # the fold takes the batch statistics: both convolutions of the layer share one backward
-                    link = qat.DwGradLink()
-                    mean, var = qat.dwconv_stats(input, self.weight, self.bias, k, st, pd, link)
-                else:
-                    with torch.no_grad():                                  # only the running statistics read them
-                        mean, var = qat.dwconv_stats(input, self.weight, self.bias, k, st, pd)
-                self.batch_mean, self.batch_var = mean, var
-                with torch.no_grad():
-                    if float(self.first_bn) == 0 and not bool(self.running_mean.any()) and not bool(self.running_var.any()):
-                        self.first_bn.add_(1)
-                        self.running_mean.add_(mean)
-                        self.running_var.add_(var)
-                    else:
-                        self.running_mean.mul_(1 - self.momentum).add_(mean * self.momentum)
-                        self.running_var.mul_(1 - self.momentum).add_(var * self.momentum)
-                if float(self.step) < self.freeze_step:
-                    s = self.gamma / torch.sqrt(var + self.eps)
-                    bias = reshape_to_bias(self.beta + (cb - mean) * s)
-                else:
-                    s = self.gamma / torch.sqrt(self.running_var + self.eps)
-                    bias = reshape_to_bias(self.beta + (cb - self.running_mean) * s)
-                weight = self.weight * reshape_to_weight(s)
+                weight, bias, link = qat.fold_batch_norm(self, input, k, st, pd, self.freeze_step)
             else:
                 bias, weight = self.bias, self.weight
         else:
             weight, bias = self.BN_fuse()
         q_weight = self.weight_quantizer(weight)
         q_bias = self.bias_quantizer(bias)
-        if depthwise:
-            out = qat.dwconv2d(input, q_weight, k, st, pd, link) + q_bias
-        else:
-            out = qat.conv2d(input, q_weight, k, st, pd) + q_bias
+        out = qat.qconv(self, input, q_weight, k, st, pd, link) + q_bias
         out = qat.activation(out, self.activate, self.maxabsscaler)
         return self.activation_quantizer(out)

@@ -7,6 +7,9 @@ composed of the sm_90a kernels: wgmma convolutions (forward / data gradient / we
 BatchNorm channel sums from the conv epilogue), b2y_minmax_f32 (range trackers), b2y_fakequant_f32 with its
 straight-through backward, activation forward / backward.  torch.autograd chains them and differentiates the [C]-sized
 fold arithmetic (batch-statistics fold -> frozen running-statistics fold at 0.9 * steps, google.py:349-370).
+Depthwise layers (groups = channels: GhostNet's cheap operations, [convolutional] groups=C) run both convolutions on the
+fp32 depthwise kernels (qat.dwconv_stats / qat.dwconv2d) with the same fold, as the TPSQ layer does; other grouped
+convolutions are refused.
 """
 import math
 import torch
@@ -199,43 +202,23 @@ class BNFold_QuantizedConv2d_For_FPGA(nn.Conv2d):
 
     def forward(self, input):
         from b200yolo import qat
+        qat.check_groups(self)
         if not input.is_cuda:
             raise RuntimeError("QAT layers run on the CUDA device only (no CPU fallback)")
-        if self.groups != 1:
-            raise NotImplementedError("depthwise QAT layers")
         k, st, pd = self.kernel_size[0], self.stride[0], self.padding[0]
-        cb = self.bias if self.bias is not None else 0
+        link = None
         if self.training:
             self.step += 1
             if self.bn:
-                # plain conv for the batch statistics (:326-338); the channel sums come out of the conv epilogue
-                y1, s1, s2 = qat.conv2d(input, self.weight, k, st, pd, want_stats=True)
-                n = float(y1.shape[0] * y1.shape[1] * y1.shape[2])
-                mean = s1 / n + cb                                    # statistics of conv + bias: the mean shifts,
-                var = (s2 - s1 * (s1 / n)) / (n - 1.0)                # the (unbiased, torch.var) variance does not
-                self.batch_mean, self.batch_var = mean, var
-                with torch.no_grad():
-                    if float(self.first_bn) == 0 and not bool(self.running_mean.any()) and not bool(self.running_var.any()):
-                        self.first_bn.add_(1)
-                        self.running_mean.add_(mean)
-                        self.running_var.add_(var)
-                    else:
-                        self.running_mean.mul_(1 - self.momentum).add_(mean * self.momentum)
-                        self.running_var.mul_(1 - self.momentum).add_(var * self.momentum)
-                if float(self.step) < self.BN_freeze_step:
-                    s = self.gamma / torch.sqrt(var + self.eps)
-                    bias = reshape_to_bias(self.beta + (cb - mean) * s)
-                else:
-                    s = self.gamma / torch.sqrt(self.running_var + self.eps)
-                    bias = reshape_to_bias(self.beta + (cb - self.running_mean) * s)
-                weight = self.weight * reshape_to_weight(s)
+                # plain conv for the batch statistics (:326-338), then the fold (:349-370)
+                weight, bias, link = qat.fold_batch_norm(self, input, k, st, pd, self.BN_freeze_step)
             else:
                 bias, weight = self.bias, self.weight
         else:
             weight, bias = self.BN_fuse()
         q_weight = self.weight_quantizer(weight)
         q_bias = self.bias_quantizer(bias)
-        out = qat.conv2d(input, q_weight, k, st, pd) + q_bias
+        out = qat.qconv(self, input, q_weight, k, st, pd, link) + q_bias
         out = qat.activation(out, self.activate, self.maxabsscaler)
         return self.activation_quantizer(out)
 
