@@ -289,32 +289,6 @@ def test_fakequant_and_cos_search_match_reference():
     assert float(mm[0, 0]) == float(x.min()) and float(mm[0, 1]) == float(x.max())
 
 
-@pytest.mark.parametrize("case", [(2, 20, 20, 64, 128, 3, 1), (2, 20, 20, 128, 256, 1, 1), (1, 40, 40, 32, 64, 3, 2),
-                                  (2, 13, 13, 512, 1024, 3, 1)])
-def test_int8_conv_bit_exact(case):
-    """INT8 wgmma conv (int32 accumulate) vs the reference's fp32 fake-quant arithmetic: requantised outputs equal."""
-    ops = _ops()
-    B, H, W, Cin, Cout, k, stride = case
-    pad = (k - 1) // 2
-    g = torch.Generator().manual_seed(5)
-    bits = 8
-    sa, sw, so = orc.pow2_scale(2, bits), orc.pow2_scale(-1, bits), orc.pow2_scale(3, bits)
-    xq = torch.randint(-128, 128, (B, Cin, H, W), generator=g).float()
-    wq = torch.clamp(orc.round_half_away(torch.randn(Cout, Cin, k, k, generator=g) * 40), -128, 127)
-    bias = orc.fake_quant(torch.randn(Cout, generator=g), orc.pow2_scale(1, bits), bits)
-    # reference arithmetic: F.conv2d on dequantised fp32 values (ptq_cos.py:288-296) -> leaky -> fake-quant (717)
-    ref = F.conv2d(xq * sa, wq * sw, bias, stride=stride, padding=pad)
-    ref = F.leaky_relu(ref, 0.1)
-    ref_q = torch.clamp(orc.round_half_away(ref / so), -128, 127)
-    x8 = xq.permute(0, 2, 3, 1).contiguous().to(torch.int8).cuda()
-    w8 = wq.permute(0, 2, 3, 1).contiguous().to(torch.int8).cuda()
-    out = ops.qconv2d(x8, w8, bias.cuda(), k, stride, pad, sa * sw, so, act="leaky")
-    torch.cuda.synchronize()
-    got = out.permute(0, 3, 1, 2).cpu().float()
-    mism = (got != ref_q).float().mean().item()
-    assert mism == 0.0, "int8 conv differs from fake-quant fp32 reference on %.4g of outputs" % mism
-
-
 @pytest.mark.parametrize("gdt", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
 def test_data_movement_backward_kernels(gdt):
     """upsample / maxpool / add backward on 16-bit gradient tensors (channel-slice views included)."""

@@ -113,6 +113,13 @@ def _s(t):
     return float(t.reshape(-1)[0])
 
 
+def _stem_fp16_exact(w, b):
+    """True when the fused fp16 stem holds the first layer's weights and bias exactly: every weight is one fp16, the bias
+    the sum of its fp16 rounding and the fp16 rounding of the rest (csrc/stem_tc.cu)"""
+    hi = b.half().float()
+    return torch.equal(w.half().float(), w) and torch.equal(hi + (b - hi).half().float(), b)
+
+
 class QPlan:
     def __init__(self, model, x_shape, device):
         self.model, self.device = model, device
@@ -403,7 +410,9 @@ class QPlan:
                     ws = self.stem_w.get(i)
                     if ws is None:
                         # fused tensor-core stem when the fake-quantised weights (int8 code x 2^-n) are exact in fp16
-                        fits = self.stem_fused and float(wq.abs().max()) < 6.0e4
+                        # and the bias in the two fp16 terms it is split into; codes x 2^-n below fp16's subnormal
+                        # grid (tiny weight scales) would be rounded
+                        fits = self.stem_fused and _stem_fp16_exact(wq, bq)
                         ws = self.stem_w[i] = ops.pack_stem_weights(wq) if fits else False
                     if ws is not False:
                         call("b2y_stem_conv_fwd_fused_q", C.byref(d), ptr(x), 0, 1.0, ptr(ws), ptr(bq), ptr(out.buf), s_a,
