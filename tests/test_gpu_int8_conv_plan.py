@@ -136,7 +136,7 @@ def check_plan(p, expect, sms):
 # that is not a power of two; out "f32" = a head's fp32 rows in a 256-wide buffer, requant False = no fake-quant
 Q = namedtuple("Q", "B H W cin ck cout k s layout act slope bias out requant r acc expect")
 CASES = {
-    # yolov3's layer 1 and layer 3, the two narrow layers qengine._pack_qconv pairs
+    # yolov3's layer 1 and layer 3, the two narrow layers layout.pair_form pairs
     "l1_c32-64_k3s2_416_s2pairs": Q(8, 416, 416, 32, 32, 64, 3, 2, "s2", "leaky", 0.1, True, "i8", True, 4, "pow2",
                                     (64, 64, 1, True, "i8-tma")),
     "l3_c32-64_k3_208_s1pairs": Q(8, 208, 208, 32, 32, 64, 3, 1, "s1", "leaky", 0.1, True, "i8", True, 5, "pow2",
@@ -435,7 +435,7 @@ def _slot_untouched(buf, lead, n, sentinel):
 
 
 def _weights_for(c, w, bias, ops):
-    """(packed int8 weights, bias, w_layout) as qengine._pack_qconv lays them out"""
+    """(QConvPack.w8, QConvPack.bias, w_layout) as qengine.QPlan._pack_qconv lays them out for the case's form"""
     from b200yolo.lib import WLAYOUT_S2_PAIRS
     if c.layout == "s2":
         return ops.s2_pair_weights(w).to(torch.int8).contiguous(), bias, WLAYOUT_S2_PAIRS
@@ -845,9 +845,10 @@ def test_qat_stem_with_tiny_weight_scale_is_exact():
     with torch.no_grad():
         qm(x)
     plan = qm.engine().plans[qi._q1_plans(qm)[0]]
-    wq, bq, s_a, act, slope, bits = plan.packed[0]
+    stem = plan.packed[0]
+    wq, bq, s_a, act, slope = stem.w, stem.bias, stem.s_a, stem.act, stem.slope
     assert float(wq[wq != 0].abs().min()) < 2.0 ** -24, "the weights are not below fp16's subnormal grid"
-    got = plan.steps[0][3].view()
+    got = plan.steps[0].out.view()
     # k / 256 times code x 2^-n: every product and sum exact in fp64, and in fp32 (< 2^24 units of s_w / 256)
     acc = F.conv2d(x.double(), wq.double(), bq.double(), stride=1, padding=1)
     _, q, _ = requant_oracle(acc, 1.0, None, act, slope, s_a)

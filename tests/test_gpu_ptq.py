@@ -73,7 +73,7 @@ def test_ptq_int8_eval_matches_reference():
     assert worst_frac < 5e-3 and worst_lsb <= 4.0
 
 
-def test_ptq_fused_shortcut_epilogue_is_bit_identical(monkeypatch):
+def test_ptq_fused_plan_is_bit_identical_to_plain_plan():
     """b2y_qconv2d_shortcut_fwd (shortcut folded into the producing conv's epilogue, TMA int8 store) and the pixel-pair
     forms of the two Cin = 32 layers against the plain graph (b2y_qconv2d_fwd + b2y_qshortcut_i8, dense weights): same
     codes everywhere, at a size with partial M tiles."""
@@ -83,17 +83,17 @@ def test_ptq_fused_shortcut_epilogue_is_bit_identical(monkeypatch):
     with torch.no_grad():
         io_f, p_f, _ = qm(x)
     plans = [pl for pl in qm._engine.plans.values() if isinstance(pl, qengine.QPlan)]
-    assert plans and any(st[0] == 'conv_sc' for st in plans[0].steps)
-    assert all(plans[0]._fusable.get(st[1], True) for st in plans[0].steps if st[0] == 'conv_sc')
-    assert [plans[0].packed[st[1]][7] for st in plans[0].steps if st[0] in ('conv', 'conv_sc') and st[2] is not None][:3] \
+    assert plans
+    convs = [st for st in plans[0].steps if st.kind == 'conv']
+    assert any(st.shortcut for st in convs)
+    assert all(plans[0]._fusable.get(st.i, True) for st in convs if st.shortcut)
+    assert [st.form for st in convs if st.src is not None][:3] \
         == ['s2', None, 's1']       # the two narrow 3x3 layers run in their pixel-pair forms
-    monkeypatch.setenv('B2Y_Q_FUSE_SHORTCUT', '0')
-    monkeypatch.setenv('B2Y_PAIRPACK', '0')
     qm2, _ = _load_quantised_model()
+    plain = qengine.QPlan(qm2, tuple(x.shape), x.device, pair_forms=False, fuse_shortcuts=False)
     with torch.no_grad():
-        io_u, p_u, _ = qm2(x)
-    plans2 = [pl for pl in qm2._engine.plans.values() if isinstance(pl, qengine.QPlan)]
-    assert plans2 and not any(st[0] == 'conv_sc' for st in plans2[0].steps)
+        io_u, p_u, _ = plain.forward(x)
+    assert not any(st.kind == 'conv' and st.shortcut for st in plain.steps)
     assert torch.equal(io_f, io_u) and all(torch.equal(a, b) for a, b in zip(p_f, p_u))
 
 

@@ -235,13 +235,24 @@ def test_qat_int8_graph_equals_module_forwards(name, way):
 
 
 @pytest.mark.parametrize("way", [1, 2])
-def test_qat_int8_graph_unfused_shortcuts(way, monkeypatch):
+def test_qat_int8_graph_unfused_shortcuts(way):
     """the stand-alone shortcut launches (b2y_qshortcut_i8, and the clamped addends of QuantizedShortcut_max through
-    b2y_requant_i8) instead of the shortcut folded into the conv epilogue"""
-    monkeypatch.setenv("B2Y_Q_FUSE_SHORTCUT", "0")
+    b2y_requant_i8) instead of the shortcut folded into the conv epilogue, captured and eager"""
+    from b200yolo.qengine import QPlan, int8_graph_refusal
     qm = _qat_model("yolov3", way)
     _train(qm, 2)
-    _check_sizes(qm, "yolov3 unfused", [(64, 64)])
+    assert int8_graph_refusal(qm) is None
+    x = orc.synth_images(2, 64, 64, seed=128).cuda()
+    ref = _runner_eval(qm, x)
+    plan = QPlan(qm, tuple(x.shape), x.device, fuse_shortcuts=False)
+    assert not any(st.kind == 'conv' and st.shortcut for st in plan.steps)
+    for graph in (True, False):
+        qm.use_cuda_graph = graph
+        with torch.no_grad():
+            for call in range(2):          # graph: the eager first call, then the capture and its replay
+                io, p, _ = plan.forward(x)
+                _assert_same((io, p), ref, "yolov3 unfused graph=%s call %d" % (graph, call))
+    qm.use_cuda_graph = True
 
 
 def test_qat_int8_plan_follows_training():

@@ -1,5 +1,5 @@
-"""Device-timed inference step (CUDA-graph replay of the fused forward) for A/B runs of environment switches:
-   B2Y_PAIRPACK=0 python tools/time_infer.py --model yolov3 --batch 32"""
+"""Device-timed inference step (CUDA-graph replay of the fused forward):
+   python tools/time_infer.py --model yolov3 --batch 32"""
 import argparse
 import os
 import sys

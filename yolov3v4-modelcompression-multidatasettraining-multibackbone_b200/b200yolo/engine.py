@@ -21,13 +21,14 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .layout import _block_parts, build_layout, feature_slots, infer_shapes, pitch, sources, stem_path
+from .layout import _block_parts, build_layout, feature_slots, infer_shapes, pair_form, pitch, sources, stem_path
 from .lib import WLAYOUT_S2_PAIRS
 
 
 # ---- launch list vocabulary: field 0 is the step's kind; src / out / res / dst are layout._Tensor -------------------
-# conv: src is None for the stem (it reads the image), res is the source of the shortcut folded into the conv, or None
-ConvStep = collections.namedtuple('ConvStep', 'kind i src out res conv bn act slope')
+# conv: src is None for the stem (it reads the image), res is the source of the shortcut folded into the conv, or None;
+# form is its pixel-pair form (layout.pair_form: 's1', 's2' or None)
+ConvStep = collections.namedtuple('ConvStep', 'kind i src out res conv bn act slope form')
 DwStep = collections.namedtuple('DwStep', 'kind i src out conv bn act slope')
 SeStep = collections.namedtuple('SeStep', 'kind i src out fc1 fc2 ws')
 # out = first + others[0] + ...; widths may differ (layers.py:57-72): a sum covers the first min(nx, na) channels, the
@@ -79,6 +80,11 @@ def launch_pointwise(st):
         ops.upsample(st.src.view(), st.stride, out=st.out.view())
     elif st.kind == 'maxpool':
         ops.maxpool(st.src.view(), st.k, st.s, tiny_pad=st.tiny_pad, out=st.out.view())
+
+
+def _whole(t):
+    """t is an fp16 tensor that fills its buffer, which the pixel-pair views reshape"""
+    return t.c0 == 0 and t.buf.shape[3] == t.C == t.Cp and t.dtype == torch.float16
 
 
 def _pad_rows(t, n, fill=0.0):
@@ -182,8 +188,8 @@ class SlotStore:
 
 class EvalWeights:
     """Packed inference weights of one model, shared by its eval plans of every shape and re-packed once per parameter
-    version.  Entries are keyed (layer index, layout): the pixel-pair layouts depend on the plan (an odd width rules
-    them out), the base layout does not."""
+    version.  Entries are keyed (layer index, form): the pixel-pair forms depend on the plan (an odd width rules them
+    out), the dense one (form None) does not."""
 
     def __init__(self):
         self.version = None
@@ -200,7 +206,7 @@ class Plan:
         self.shared_weights = shared_weights if shared_weights is not None else EvalWeights()
         self.held = {}          # slot name -> version taken
         self.steps = []
-        self.wkey = {}          # layer index -> key (layer index, weight layout) of its pack in shared_weights.packs
+        self.wkey = {}          # layer index -> key (layer index, form or kind) of its pack in shared_weights.packs
         self.param_version = None
         self.graph = None
         self.runs = 0
@@ -275,14 +281,21 @@ class Plan:
                 if i + 1 < n and fused_into[i + 1] == i:
                     res = tens[sources(i + 1, defs[i + 1]['from'])[0]]
                 src = None if i == 0 else tens[i - 1]
+                k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+                form = None
                 if src is None:
-                    k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
                     self.stem = stem_path(conv.in_channels, k, out.Cp)
                     if self.stem == 'im2col':
                         d = ops.make_conv_desc((B, self.H, self.W, conv.in_channels), conv.in_channels, out.Cp, k, s,
                                                p, out.Cp)
                         self.stem_ws = self._take(('stem_ws',), (ops.stem_workspace_bytes(d) // 2,))
-                self.steps.append(ConvStep('conv', i, src, out, res, conv, bn, act, slope))
+                else:
+                    form = pair_form(k, s, p, conv.in_channels, conv.out_channels, src.W)
+                    if form == 's1' and not all(_whole(t) for t in (src, out, res) if t is not None):
+                        form = None
+                    elif form == 's2' and not (_whole(src) and out.C == out.Cp):
+                        form = None
+                self.steps.append(ConvStep('conv', i, src, out, res, conv, bn, act, slope, form))
             elif t == 'yolo':
                 raw = tens[i - 1]
                 rows = m.na * raw.H * raw.W
@@ -339,8 +352,7 @@ class Plan:
             if st.kind != 'conv':
                 continue
             i, conv, bn = st.i, st.conv, st.bn
-            layout = 'pair' if self._pair_packable(st) else 's2' if self._s2_pair_packable(st) else 'base'
-            key = self.wkey[i] = (i, layout)
+            key = self.wkey[i] = (i, st.form)
             if key in packs:
                 continue
             bnp = None
@@ -348,7 +360,7 @@ class Plan:
             if bn is not None:
                 bnp = (bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var)
                 eps = bn.eps
-            base = packs.get((i, 'base'))
+            base = packs.get((i, None))
             if base is None:
                 stem = st.src is None
                 # [Cp_out][K][kh][kw]: zero rows, bias and BatchNorm scale for the pad outputs (BatchNorm padded with
@@ -362,45 +374,23 @@ class Plan:
                 wp, bias, w32 = ops.pack_conv_weights(wsrc, _pad_rows(conv.bias.detach(), cp) if conv.bias is not None
                                                       else None, bnp_p, eps, want_fp32=stem)
                 wstem = ops.pack_stem_weights(w32) if stem and self.stem != 'direct' else None
-                base = packs[(i, 'base')] = (wp, bias, w32, wstem)
-            if layout == 'pair':
+                base = packs[(i, None)] = (wp, bias, w32, wstem)
+            if st.form == 's1':
                 packs[key] = base + (self._pair_pack(conv, bnp, eps),)
-            elif layout == 's2':
+            elif st.form == 's2':
                 _, bias_f, w32f = ops.pack_conv_weights(conv.weight.detach(), conv.bias.detach() if conv.bias is not None
                                                         else None, bnp, eps, want_fp32=True)
                 packs[key] = base + ((ops.s2_pair_weights(w32f).half(), bias_f),)
 
-    # ---- pixel-pair packing of the Cin = 32 3x3 layers --------------------------------------------------------------
+    # ---- pixel-pair packing of the Cin = 32 3x3 layers (layout.pair_form) ------------------------------------------
     # With 32 input channels a tap of the im2col gather is a 64-byte row: one TMA request per pixel per tap, and the
     # layer is bound by the TMA request rate (0.16 of the tensor peak, 31-46 % of HBM in round 1), not by HBM.  The NHWC
     # tensor [B,H,W,32] is the same memory as [B,H,W/2,64]: viewed as pixel PAIRS the same convolution is a 3x3 conv
     # with 64 input and 2*Cout output channels whose weights are the original taps placed at
     # s = 2(kwp-1) + i_sub - o_sub + 1 (zero elsewhere).  Half of the MACs multiply zeros, but the rows are 128 bytes,
-    # the tile count halves and N = 128 brings the CTA-pair path in -- no new kernel, only a weight layout.
-    def _pair_packable(self, st):
-        if os.environ.get('B2Y_PAIRPACK', '1') == '0':
-            return False
-        src, out, res, conv = st.src, st.out, st.res, st.conv
-        if src is None or conv.kernel_size[0] != 3 or conv.stride[0] != 1 or conv.padding[0] != 1:
-            return False
-        if conv.in_channels != 32 or conv.out_channels > 128 or conv.out_channels % 8 or src.W % 2:
-            return False
-        full = lambda t: t.c0 == 0 and t.buf.shape[3] == t.C == t.Cp and t.dtype == torch.float16
-        return full(src) and full(out) and (res is None or full(res))
-
-    def _s2_pair_packable(self, st):
-        """3x3 / stride-2 layers with 32 input channels (the first downsampling conv): B2Y_WLAYOUT_S2_PAIRS -- the input
-        read as pixel pairs makes it a 3 x 2 window with stride 2 x 1 over 128-byte rows (6 im2col boxes, not 9 halves)."""
-        if os.environ.get('B2Y_PAIRPACK', '1') == '0':
-            return False
-        src, conv = st.src, st.conv
-        if src is None or conv.kernel_size[0] != 3 or conv.stride[0] != 2 or conv.padding[0] != 1:
-            return False
-        if conv.in_channels != 32 or src.W % 2:
-            return False
-        return (src.c0 == 0 and src.buf.shape[3] == src.C == src.Cp and st.out.C == st.out.Cp
-                and src.dtype == torch.float16)
-
+    # the tile count halves and N = 128 brings the CTA-pair path in -- no new kernel, only a weight layout.  Stride 2
+    # reads the input as pixel pairs through B2Y_WLAYOUT_S2_PAIRS: a 3 x 2 window with stride 2 x 1 over 128-byte rows
+    # (6 im2col boxes, not 9 halves).
     def _pair_pack(self, conv, bnp, eps):
         _, bias, w32 = ops.pack_conv_weights(conv.weight.detach(), conv.bias.detach() if conv.bias is not None else None,
                                              bnp, eps, want_fp32=True)
@@ -410,7 +400,6 @@ class Plan:
     def _launch_conv(self, st, x):
         src, out, res, conv, act, slope = st.src, st.out, st.res, st.conv, st.act, st.slope
         wp, bias, w32, wstem = self._w(st.i)[:4]
-        layout = self.wkey[st.i][1]
         k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         if src is None:
             if self.stem == 'fused':
@@ -425,11 +414,11 @@ class Plan:
                                  out=out.view(), workspace=self.stem_ws)
             else:
                 ops.stem_conv(x, w32, bias, k, s, p, act=act, slope=slope, out=out.view())
-        elif layout == 's2':
+        elif st.form == 's2':
             wps2, bias_s2 = self._w(st.i)[4]
             ops.conv2d(src.view(), wps2, bias_s2, k, s, p, act=act, slope=slope,
                        residual=res.view() if res is not None else None, out=out.view(), w_layout=WLAYOUT_S2_PAIRS)
-        elif layout == 'pair':
+        elif st.form == 's1':
             wp2, bias2 = self._w(st.i)[4]
             pairs = lambda t: t.buf.view(t.buf.shape[0], t.H, t.W // 2, 2 * t.C)
             ops.conv2d(pairs(src), wp2, bias2, 3, 1, 1, act=act, slope=slope,

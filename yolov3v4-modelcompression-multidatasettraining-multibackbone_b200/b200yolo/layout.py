@@ -94,6 +94,23 @@ def stem_path(in_c, k, out_c, training=False, batch_norm=True):
     return 'fused' if out_c <= 64 else 'im2col'
 
 
+def pair_form(k, s, p, cin, cout, in_w):
+    """Pixel-pair form of a non-stem convolution, the one shape rule of the fp16 and INT8 eval plans (why the pairs pay:
+    engine.Plan._pair_pack).  The NHWC input [B,H,W,32] is read as pixel pairs [B,H,W/2,64]:
+
+    's1'  3x3 stride 1, cout <= 128 and a multiple of 8: a 3x3 conv over the pairs with 64 input and 2 * cout output
+          channels (ops.s1_pair_weights), its output read as pairs too
+    's2'  3x3 stride 2: B2Y_WLAYOUT_S2_PAIRS, a 3 x 2 window with stride 2 x 1 over the pairs (ops.s2_pair_weights)
+    None  the dense form
+
+    A plan may add conditions on where its tensors are placed."""
+    if k != 3 or p != 1 or cin != 32 or in_w % 2:
+        return None
+    if s == 1 and cout <= 128 and cout % 8 == 0:
+        return 's1'
+    return 's2' if s == 2 else None
+
+
 def sources(i, rel):
     """Absolute layer indices of the `layers=` / `from=` list of layer i (negative entries are relative to i)."""
     return [i + l if l < 0 else l for l in rel]

@@ -21,17 +21,48 @@ input_scale unclamped (the COSPTQ shortcut with scale_x = scale_a = input_scale)
 its one scale (the clamp_addends mode of b2y_qconv2d_shortcut_fwd, or b2y_requant_i8 of both addends); concats
 requantise onto QuantizedFeatureConcat.scale.
 """
+import collections
 import ctypes as C
 import os
 
 import torch
 
 from . import ops
-from .layout import _Tensor, infer_shapes, sources, stem_path
+from .engine import MaxpoolStep, UpsampleStep
+from .layout import _Tensor, infer_shapes, pair_form, sources, stem_path
 from .lib import OUT_F32, OUT_I8, WLAYOUT_S2_PAIRS, B2YError, call, ptr, stream_ptr
 
 _GOOGLE_SHORTCUTS = ('QuantizedShortcut_min', 'QuantizedShortcut_max')
 _Q1_LAYERS = ('convolutional', 'shortcut', 'route', 'upsample', 'maxpool', 'yolo')
+
+# ---- launch list vocabulary: field 0 is the step's kind; src / out / x / addend / own are layout._Tensor; upsample and
+# max-pool steps are engine.UpsampleStep / engine.MaxpoolStep
+# conv: src is None for the stem (it reads the image); a head writes fp32 fake-quant values for the decode; form is the
+# pixel-pair form (layout.pair_form: 's1', 's2' or None); shortcut is a FusedShortcut or None
+QConvStep = collections.namedtuple('QConvStep', 'kind i src out conv head form shortcut')
+# shortcut layer i (module) folded into the epilogue of the conv before it, which then writes the shortcut's tensor: own
+# is the conv's own output, materialised only when the fused launch is refused
+FusedShortcut = collections.namedtuple('FusedShortcut', 'i addend module own')
+# out = x + addend, both rounded onto the shortcut's scales
+QShortcutStep = collections.namedtuple('QShortcutStep', 'kind i x addend out module')
+# every source requantised onto the concat's scale, into its channel slot of out
+QConcatStep = collections.namedtuple('QConcatStep', 'kind i srcs out module')
+
+# packed weights of a body conv: int8 codes in the step's form, bias, acc_scale = s_in * s_w, s_a the output scale
+QConvPack = collections.namedtuple('QConvPack', 'w8 bias acc_scale s_a act slope bits')
+# the fp32 stem: fake-quantised weights and bias (the fused fp16 copy of the weights is made at the first launch)
+QStemPack = collections.namedtuple('QStemPack', 'w bias s_a act slope bits')
+ShortcutScales = collections.namedtuple('ShortcutScales', 'scale_x scale_a scale_sum clamp_addends')
+
+
+def _late_readers(defs):
+    """layer -> the layers that read it through a route or a shortcut"""
+    readers = {}
+    for j, dj in enumerate(defs):
+        rel = dj.get('layers', []) if dj['type'] == 'route' else dj.get('from', []) if dj['type'] == 'shortcut' else []
+        for s in sources(j, rel):
+            readers.setdefault(s, []).append(j)
+    return readers
 
 
 def int8_graph_refusal(model):
@@ -45,11 +76,7 @@ def int8_graph_refusal(model):
     n = len(defs)
     if not n or defs[0]['type'] != 'convolutional':
         return "the int8 graph starts with the fp32 stem convolution of the image"
-    late_readers = {}          # layer -> the layers after it that read it through a route or a shortcut
-    for j, dj in enumerate(defs):
-        for s in sources(j, dj.get('layers', []) if dj['type'] == 'route' else dj.get('from', [])
-                         if dj['type'] == 'shortcut' else []):
-            late_readers.setdefault(s, []).append(j)
+    late_readers = _late_readers(defs)
     for i, (d, m) in enumerate(zip(defs, mods)):
         t = d['type']
         if t not in _Q1_LAYERS:
@@ -121,22 +148,23 @@ def _stem_fp16_exact(w, b):
 
 
 class QPlan:
-    def __init__(self, model, x_shape, device):
+    def __init__(self, model, x_shape, device, *, pair_forms=True, fuse_shortcuts=True):
+        """pair_forms / fuse_shortcuts = False build the plain graph (dense weights everywhere, every shortcut a launch
+        of its own), the one the tests compare the pixel-pair forms and the fused shortcut epilogue against."""
         self.model, self.device = model, device
         self.B, self.Cin, self.H, self.W = x_shape
         self.steps = []
         self.prepared = False
         self.runs = 0
         self.graph = None
-        self._scal = {}
         self._fusable = {}
         self._scratch = {}
         # quantized=1: the QAT state the plan was packed from (see _state_fingerprint); Engine.weights_changed() clears it
         self.q1 = model.quantized == 1
         self.param_version = None
-        self._build()
+        self._build(pair_forms, fuse_shortcuts)
 
-    def _build(self):
+    def _build(self, pair_forms, fuse_shortcuts):
         model, B, dev = self.model, self.B, self.device
         defs, mods = model.module_defs, model.module_list
         n = len(defs)
@@ -147,13 +175,13 @@ class QPlan:
         tens = [None] * n
         self.yolo = []
         row_off = 0
-        # layers whose output is read by somebody other than the next layer (route sources, shortcut 'from' addends)
-        readers = set()
-        for j, dj in enumerate(defs):
-            if dj['type'] == 'route':
-                readers.update(sources(j, dj['layers']))
-            elif dj['type'] == 'shortcut':
-                readers.update(sources(j, dj['from']))
+        readers = _late_readers(defs)
+
+        def codes(C, H, W):
+            t = _Tensor(C, H, W, torch.int8)
+            t.buf = torch.empty((B, H, W, C), dtype=torch.int8, device=dev)
+            return t
+
         for i, (d, m) in enumerate(zip(defs, mods)):
             t = d['type']
             Cc, H, W = shapes[i]
@@ -175,7 +203,11 @@ class QPlan:
                     # weights get zero columns there (_pack_qconv)
                     src.Cp = (src.Cp + 31) // 32 * 32
                     src.buf = torch.zeros((B, src.H, src.W, src.Cp), dtype=torch.int8, device=dev)
-                self.steps.append(('conv', i, None if i == 0 else tens[i - 1], out, conv, head))
+                form = None
+                if pair_forms and src is not None and not head:
+                    form = pair_form(conv.kernel_size[0], conv.stride[0], conv.padding[0], conv.in_channels,
+                                     conv.out_channels, src.W)
+                self.steps.append(QConvStep('conv', i, src, out, conv, head, form, None))
                 tens[i] = out
             elif t == 'shortcut':
                 kinds = _GOOGLE_SHORTCUTS if self.q1 else ('COSPTQuantizedShortcut_min', 'COSPTQuantizedShortcut_max')
@@ -185,18 +217,15 @@ class QPlan:
                 if len(d['from']) != 1 or getattr(m, 'weight', False):
                     raise NotImplementedError("weighted / multi-source quantised shortcut")
                 src = tens[sources(i, d['from'])[0]]
-                out = _Tensor(Cc, H, W, torch.int8)
-                out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
-                prev_step = self.steps[-1] if self.steps else None
-                fuse = (os.environ.get('B2Y_Q_FUSE_SHORTCUT', '1') != '0' and prev_step is not None
-                        and prev_step[0] == 'conv' and prev_step[1] == i - 1 and prev_step[2] is not None
-                        and not prev_step[5] and (i - 1) not in readers and src is not tens[i - 1])
-                if fuse:
+                out = codes(Cc, H, W)
+                prev = self.steps[-1] if self.steps else None
+                if (fuse_shortcuts and prev is not None and prev.kind == 'conv' and prev.i == i - 1
+                        and prev.src is not None and not prev.head and (i - 1) not in readers and src is not tens[i - 1]):
                     # the conv writes the shortcut's result; its own output tensor is never materialised
-                    self.steps[-1] = ('conv_sc', i - 1, prev_step[2], out, prev_step[4], (i, src, m, tens[i - 1]))
+                    self.steps[-1] = prev._replace(out=out, shortcut=FusedShortcut(i, src, m, tens[i - 1]))
                     tens[i - 1].buf = None
                 else:
-                    self.steps.append(('shortcut', i, tens[i - 1], src, out, m))
+                    self.steps.append(QShortcutStep('shortcut', i, tens[i - 1], src, out, m))
                 tens[i] = out
             elif t == 'route':
                 srcs = sources(i, d['layers'])
@@ -205,21 +234,15 @@ class QPlan:
                 if len(srcs) == 1:
                     tens[i] = tens[srcs[0]]
                 else:
-                    out = _Tensor(Cc, H, W, torch.int8)
-                    out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
-                    self.steps.append(('concat', i, [tens[s] for s in srcs], out, m))
-                    tens[i] = out
+                    tens[i] = codes(Cc, H, W)
+                    self.steps.append(QConcatStep('concat', i, [tens[s] for s in srcs], tens[i], m))
             elif t == 'upsample':
-                out = _Tensor(Cc, H, W, torch.int8)
-                out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
-                self.steps.append(('upsample', i, tens[i - 1], out, d['stride']))
-                tens[i] = out
+                tens[i] = codes(Cc, H, W)
+                self.steps.append(UpsampleStep('upsample', tens[i - 1], tens[i], d['stride']))
             elif t == 'maxpool':
-                out = _Tensor(Cc, H, W, torch.int8)
-                out.buf = torch.empty((B, H, W, Cc), dtype=torch.int8, device=dev)
+                tens[i] = codes(Cc, H, W)
                 k, s = d['size'], d['stride']
-                self.steps.append(('maxpool', i, tens[i - 1], out, k, s, k == 2 and s == 1))
-                tens[i] = out
+                self.steps.append(MaxpoolStep('maxpool', tens[i - 1], tens[i], k, s, k == 2 and s == 1))
             elif t == 'yolo':
                 raw = tens[i - 1]
                 rows = m.na * raw.H * raw.W
@@ -228,23 +251,21 @@ class QPlan:
         self.total_rows = row_off
         self.anchors_px = [m.anchors.to(dev).float().contiguous() for (m, _, _, _) in self.yolo]
 
-    def _pack_qconv(self, src, conv, qw, bias, s_w):
-        """int8 weight codes [O][kh][kw][I] + bias, in the pixel-pair forms for the two narrow (Cin = 32) 3x3 layers:
-        's1' = ops.s1_pair_weights (the tensors viewed as [B,H,W/2,2C], doubled output channels), 's2' =
-        B2Y_WLAYOUT_S2_PAIRS.  q_weight holds code * s_w exactly, so the codes are recovered without rounding."""
-        k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-        O, I = conv.out_channels, conv.in_channels
-        lo, hi = -(1 << (conv.w_bits - 1)), (1 << (conv.w_bits - 1)) - 1
-        pair_ok = os.environ.get('B2Y_PAIRPACK', '1') != '0' and k == 3 and p == 1 and I == 32 and src.W % 2 == 0
-        if pair_ok and s == 1 and O <= 128 and O % 8 == 0:
+    def _pack_qconv(self, st, qw, bias, s_w):
+        """(int8 weight codes [O][kh][kw][I], bias) of a body conv step in its form: 's1' = ops.s1_pair_weights (the
+        tensors viewed as [B,H,W/2,2C], doubled output channels), 's2' = B2Y_WLAYOUT_S2_PAIRS, None = dense with zero
+        columns up to the input's stored width.  q_weight holds code * s_w exactly, so the codes are recovered without
+        rounding."""
+        conv = st.conv
+        if st.form == 's1':
             w2 = ops.s1_pair_weights(qw)
-            return ops.pack_qconv_weights(w2, s_w, conv.w_bits), torch.cat([bias, bias]).contiguous(), 's1'
-        if pair_ok and s == 2:
-            codes = (ops.s2_pair_weights(qw) / s_w).round().clamp(lo, hi).to(torch.int8).contiguous()
-            return codes, bias, 's2'
-        if src.Cp != I:
-            qw = torch.nn.functional.pad(qw, (0, 0, 0, 0, 0, src.Cp - I))
-        return ops.pack_qconv_weights(qw, s_w, conv.w_bits), bias, None
+            return ops.pack_qconv_weights(w2, s_w, conv.w_bits), torch.cat([bias, bias]).contiguous()
+        if st.form == 's2':
+            lo, hi = -(1 << (conv.w_bits - 1)), (1 << (conv.w_bits - 1)) - 1
+            return (ops.s2_pair_weights(qw) / s_w).round().clamp(lo, hi).to(torch.int8).contiguous(), bias
+        if st.src.Cp != conv.in_channels:
+            qw = torch.nn.functional.pad(qw, (0, 0, 0, 0, 0, st.src.Cp - conv.in_channels))
+        return ops.pack_qconv_weights(qw, s_w, conv.w_bits), bias
 
     def _quantised_conv(self, i, conv):
         """(fake-quantised folded weights, fake-quantised bias, s_w, s_a) of conv layer i.  quantized=3: the reference's
@@ -269,15 +290,15 @@ class QPlan:
         return qw.detach().float().contiguous(), qb.detach().float().contiguous(), s_w, s_a
 
     def _shortcut_scales(self, m):
-        """(scale_x, scale_a, scale_sum, clamp_addends) of a quantised shortcut (module eval forwards)"""
+        """ShortcutScales of a quantised shortcut (module eval forwards)"""
         name = m.__class__.__name__
         if name == 'QuantizedShortcut_min':
-            v = (_s(m.input_scale), _s(m.input_scale), _s(m.scale), 0)
+            v = ShortcutScales(_s(m.input_scale), _s(m.input_scale), _s(m.scale), 0)
         elif name == 'QuantizedShortcut_max':
-            v = (_s(m.scale), _s(m.scale), _s(m.scale), 1)
+            v = ShortcutScales(_s(m.scale), _s(m.scale), _s(m.scale), 1)
         else:
-            v = (_s(m.scale_x), _s(m.scale_a), _s(m.scale_sum), 0)
-        if self.q1 and min(v[:3]) <= 0:
+            v = ShortcutScales(_s(m.scale_x), _s(m.scale_a), _s(m.scale_sum), 0)
+        if self.q1 and min(v.scale_x, v.scale_a, v.scale_sum) <= 0:
             raise RuntimeError("shortcut %s is not calibrated (scale == 0): load a calibrated state_dict" % m.name)
         return v
 
@@ -288,34 +309,32 @@ class QPlan:
         self.sc_scales = {}
         self.q_steps = []
         for st in self.steps:
-            kind = st[0]
-            if kind in ('conv', 'conv_sc'):
-                i, src, out, conv = st[1], st[2], st[3], st[4]
-                qw, qb, s_w, s_a = self._quantised_conv(i, conv)
+            if st.kind == 'conv':
+                conv, sc = st.conv, st.shortcut
+                qw, qb, s_w, s_a = self._quantised_conv(st.i, conv)
                 act, slope, bits_a = conv.activate, 0.25 if conv.maxabsscaler else 0.1, conv.a_bits
-                if src is None:
-                    self.packed[i] = (qw, qb, s_a, act, slope, bits_a)
+                if st.src is None:
+                    self.packed[st.i] = QStemPack(qw, qb, s_a, act, slope, bits_a)
                 else:
-                    w8, bq, mode = self._pack_qconv(src, conv, qw, qb, s_w)
-                    self.packed[i] = (w8, bq, scale_of[id(src)] * s_w, s_a, act, slope, bits_a, mode)
+                    w8, bq = self._pack_qconv(st, qw, qb, s_w)
+                    self.packed[st.i] = QConvPack(w8, bq, scale_of[id(st.src)] * s_w, s_a, act, slope, bits_a)
                 if self.q1:
                     # the quantisers count their forwards in eval too (quantized_google.py Quantizer.forward)
                     self.q_steps += [conv.weight_quantizer.step, conv.bias_quantizer.step,
                                      conv.activation_quantizer.step]
-                if kind == 'conv':
-                    scale_of[id(out)] = s_a
+                if sc is None:
+                    scale_of[id(st.out)] = s_a
                 else:
-                    isc, m, own = st[5][0], st[5][2], st[5][3]
-                    self.sc_scales[isc] = self._shortcut_scales(m)
-                    scale_of[id(own)] = s_a
-                    scale_of[id(out)] = self.sc_scales[isc][2]
-            elif kind == 'shortcut':
-                self.sc_scales[st[1]] = self._shortcut_scales(st[5])
-                scale_of[id(st[4])] = self.sc_scales[st[1]][2]
-            elif kind == 'concat':
-                scale_of[id(st[3])] = _s(st[4].scale)
-            elif kind in ('upsample', 'maxpool'):
-                scale_of[id(st[3])] = scale_of[id(st[2])]
+                    self.sc_scales[sc.i] = self._shortcut_scales(sc.module)
+                    scale_of[id(sc.own)] = s_a
+                    scale_of[id(st.out)] = self.sc_scales[sc.i].scale_sum
+            elif st.kind == 'shortcut':
+                self.sc_scales[st.i] = self._shortcut_scales(st.module)
+                scale_of[id(st.out)] = self.sc_scales[st.i].scale_sum
+            elif st.kind == 'concat':
+                scale_of[id(st.out)] = _s(st.module.scale)
+            else:       # upsample, maxpool: the codes keep their grid
+                scale_of[id(st.out)] = scale_of[id(st.src)]
         self.scale_of = scale_of
         self.stem_w = {}
         self.prepared = True
@@ -360,16 +379,8 @@ class QPlan:
             return io, p, feats
         return io.clone(), tuple(t.clone() for t in p), feats
 
-    def _sv(self, t):
-        """python float of a scale buffer, read once (a host sync is illegal while the forward is being captured)"""
-        v = self._scal.get(id(t))
-        if v is None:
-            v = self._scal[id(t)] = _s(t)
-        return v
-
     def invalidate(self):
         self.graph = None
-        self._scal = {}
         self.prepared = False
         self.runs = 0
 
@@ -392,99 +403,91 @@ class QPlan:
         call("b2y_qshortcut_i8", ptr(xv), ops._pitch(xv), ptr(av), ops._pitch(av), ptr(ov), ops._pitch(ov), pixels, c,
              sx_in, scale_x, sa_in, scale_a, scale_sum, float(lo), float(hi), stream_ptr())
 
+    def _launch_stem(self, st, x):
+        """layer 0: the fp32 conv of the float image on the fake-quantised weights, int8 out"""
+        pk, conv = self.packed[st.i], st.conv
+        lo, hi = -(1 << (pk.bits - 1)), (1 << (pk.bits - 1)) - 1
+        d = ops.make_conv_desc((self.B, self.H, self.W, self.Cin), self.Cin, conv.out_channels, conv.kernel_size[0],
+                               conv.stride[0], conv.padding[0], ops._pitch(st.out.view()), pk.act, pk.slope, OUT_I8)
+        ws = self.stem_w.get(st.i)
+        if ws is None:
+            # fused tensor-core stem when the fake-quantised weights (int8 code x 2^-n) are exact in fp16 and the bias in
+            # the two fp16 terms it is split into; codes x 2^-n below fp16's subnormal grid (tiny weight scales) would be
+            # rounded
+            fits = self.stem_fused and _stem_fp16_exact(pk.w, pk.bias)
+            ws = self.stem_w[st.i] = ops.pack_stem_weights(pk.w) if fits else False
+        if ws is not False:
+            call("b2y_stem_conv_fwd_fused_q", C.byref(d), ptr(x), 0, 1.0, ptr(ws), ptr(pk.bias), ptr(st.out.buf), pk.s_a,
+                 float(lo), float(hi), stream_ptr())
+        else:
+            call("b2y_stem_conv_fwd_q", C.byref(d), ptr(x), ptr(pk.w), ptr(pk.bias), ptr(st.out.buf), pk.s_a, float(lo),
+                 float(hi), stream_ptr())
+
+    def _launch_conv(self, st):
+        """A body conv step: the int8 conv, with its folded shortcut in the epilogue.  When the fused launch is refused
+        as unsupported (e.g. a scale that is not a power of two) the conv writes its own output and the shortcut runs as
+        a launch of its own, for this layer from then on."""
+        pk, conv, sc = self.packed[st.i], st.conv, st.shortcut
+        k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+        view = _pairs if st.form == 's1' else _Tensor.view
+        w_layout = WLAYOUT_S2_PAIRS if st.form == 's2' else 0
+        xv, ov = view(st.src), view(st.out)
+        if sc is not None:
+            av, s_addend, scales = view(sc.addend), self.scale_of[id(sc.addend)], self.sc_scales[sc.i]
+            slo, shi = -(1 << (sc.module.bits - 1)), (1 << (sc.module.bits - 1)) - 1
+            if self._fusable.get(st.i, True):
+                cd = ops.make_conv_desc(xv.shape, ops._pitch(xv), pk.w8.shape[0], k, s, p, ops._pitch(ov), pk.act,
+                                        pk.slope, OUT_I8, 0, w_layout)
+                qd = ops.QConvDesc(cd, float(pk.acc_scale), float(pk.s_a), float(-(1 << (pk.bits - 1))),
+                                   float((1 << (pk.bits - 1)) - 1), OUT_I8, 1, scales.clamp_addends)
+                try:
+                    call("b2y_qconv2d_shortcut_fwd", C.byref(qd), ptr(xv), ptr(pk.w8), ptr(pk.bias), ptr(av),
+                         ops._pitch(av), s_addend, scales.scale_x, scales.scale_a, scales.scale_sum, float(slo),
+                         float(shi), ptr(ov), stream_ptr())
+                    return
+                except B2YError as e:
+                    if 'unsupported' not in str(e).lower():
+                        raise
+                    self._fusable[st.i] = False
+            if sc.own.buf is None:
+                sc.own.buf = torch.empty((self.B, sc.own.H, sc.own.W, sc.own.C), dtype=torch.int8, device=self.device)
+        yv = ov if sc is None else view(sc.own)
+        ops.qconv2d(xv, pk.w8, pk.bias, k, s, p, pk.acc_scale, pk.s_a, act=pk.act, slope=pk.slope, bits=pk.bits, out=yv,
+                    out_kind=OUT_F32 if st.head else OUT_I8, w_layout=w_layout)
+        if sc is not None:
+            self._qshortcut(sc.i, sc.module, yv, pk.s_a, av, s_addend, ov, yv.shape[3])
+
     def _forward_eager(self, x):
         B = self.B
         sc = self.scale_of
         if self.q_steps:
             torch._foreach_add_(self.q_steps, 1)
         for st in self.steps:
-            kind = st[0]
-            if kind == 'conv':
-                _, i, src, out, conv, head = st
-                k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-                if src is None:
-                    wq, bq, s_a, act, slope, bits = self.packed[i]
-                    lo, hi = -(1 << (bits - 1)), (1 << (bits - 1)) - 1
-                    d = ops.make_conv_desc((B, self.H, self.W, self.Cin), self.Cin, conv.out_channels, k, s, p,
-                                           ops._pitch(out.view()), act, slope, OUT_I8)
-                    ws = self.stem_w.get(i)
-                    if ws is None:
-                        # fused tensor-core stem when the fake-quantised weights (int8 code x 2^-n) are exact in fp16
-                        # and the bias in the two fp16 terms it is split into; codes x 2^-n below fp16's subnormal
-                        # grid (tiny weight scales) would be rounded
-                        fits = self.stem_fused and _stem_fp16_exact(wq, bq)
-                        ws = self.stem_w[i] = ops.pack_stem_weights(wq) if fits else False
-                    if ws is not False:
-                        call("b2y_stem_conv_fwd_fused_q", C.byref(d), ptr(x), 0, 1.0, ptr(ws), ptr(bq), ptr(out.buf), s_a,
-                             float(lo), float(hi), stream_ptr())
-                    else:
-                        call("b2y_stem_conv_fwd_q", C.byref(d), ptr(x), ptr(wq), ptr(bq), ptr(out.buf), s_a, float(lo),
-                             float(hi), stream_ptr())
+            if st.kind == 'conv':
+                if st.src is None:
+                    self._launch_stem(st, x)
                 else:
-                    w8, bq, acc_scale, s_a, act, slope, bits, mode = self.packed[i]
-                    if head:
-                        ops.qconv2d(src.view(), w8, bq, k, s, p, acc_scale, s_a, act=act, slope=slope, bits=bits,
-                                    out=out.buf[..., :conv.out_channels], out_kind=OUT_F32, requant=True)
-                    elif mode == 's1':
-                        ops.qconv2d(_pairs(src), w8, bq, k, s, p, acc_scale, s_a, act=act, slope=slope, bits=bits,
-                                    out=_pairs(out), out_kind=OUT_I8)
-                    else:
-                        ops.qconv2d(src.view(), w8, bq, k, s, p, acc_scale, s_a, act=act, slope=slope, bits=bits,
-                                    out=out.view(), out_kind=OUT_I8, w_layout=WLAYOUT_S2_PAIRS if mode == 's2' else 0)
-            elif kind == 'conv_sc':
-                _, i, src, out, conv, (isc, at, m, own) = st
-                k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-                w8, bq, acc_scale, s_a, act, slope, bits, mode = self.packed[i]
-                scale_x, scale_a, scale_sum, clamp = self.sc_scales[isc]
-                slo, shi = -(1 << (m.bits - 1)), (1 << (m.bits - 1)) - 1
-                if mode == 's1':
-                    xv, av, ov = _pairs(src), _pairs(at), _pairs(out)
-                else:
-                    xv, av, ov = src.view(), at.view(), out.view()
-                fused = self._fusable.get(i, True)
-                if fused:
-                    cd = ops.make_conv_desc(xv.shape, ops._pitch(xv), w8.shape[0], k, s, p, ops._pitch(ov), act,
-                                            slope, OUT_I8, 0, WLAYOUT_S2_PAIRS if mode == 's2' else 0)
-                    qd = ops.QConvDesc(cd, float(acc_scale), float(s_a), float(-(1 << (bits - 1))),
-                                       float((1 << (bits - 1)) - 1), OUT_I8, 1, clamp)
-                    try:
-                        call("b2y_qconv2d_shortcut_fwd", C.byref(qd), ptr(xv), ptr(w8), ptr(bq), ptr(av), ops._pitch(av),
-                             sc[id(at)], scale_x, scale_a, scale_sum, float(slo), float(shi), ptr(ov), stream_ptr())
-                    except B2YError as e:
-                        if 'unsupported' not in str(e).lower():
-                            raise
-                        fused = self._fusable[i] = False       # e.g. a scale that is not a power of two
-                if not fused:
-                    if own.buf is None:
-                        own.buf = torch.empty((B, own.H, own.W, own.C), dtype=torch.int8, device=self.device)
-                    ops.qconv2d(xv, w8, bq, k, s, p, acc_scale, s_a, act=act, slope=slope, bits=bits,
-                                out=_pairs(own) if mode == 's1' else own.view(), out_kind=OUT_I8,
-                                w_layout=WLAYOUT_S2_PAIRS if mode == 's2' else 0)
-                    wv = _pairs(own) if mode == 's1' else own.view()
-                    self._qshortcut(isc, m, wv, s_a, av, sc[id(at)], ov, wv.shape[3])
-            elif kind == 'shortcut':
-                _, i, xt, at, out, m = st
-                self._qshortcut(i, m, xt.view(), sc[id(xt)], at.view(), sc[id(at)], out.view(), out.C)
-            elif kind == 'concat':
-                _, i, srcs, out, m = st
-                lo, hi = -(1 << (m.bits - 1)), (1 << (m.bits - 1)) - 1
+                    self._launch_conv(st)
+            elif st.kind == 'shortcut':
+                self._qshortcut(st.i, st.module, st.x.view(), sc[id(st.x)], st.addend.view(), sc[id(st.addend)],
+                                st.out.view(), st.out.C)
+            elif st.kind == 'concat':
+                lo, hi = -(1 << (st.module.bits - 1)), (1 << (st.module.bits - 1)) - 1
                 off = 0
-                for t in srcs:
+                for t in st.srcs:
                     tv = t.view()
-                    ov = out.buf[..., off:off + t.C]
+                    ov = st.out.buf[..., off:off + t.C]
                     call("b2y_requant_i8", ptr(tv), ops._pitch(tv), ptr(ov), ops._pitch(ov), B * t.H * t.W, t.C,
-                         sc[id(t)], self._sv(m.scale), float(lo), float(hi), stream_ptr())
+                         sc[id(t)], sc[id(st.out)], float(lo), float(hi), stream_ptr())
                     off += t.C
-            elif kind == 'upsample':
-                _, i, src, out, s = st
-                sv, ov = src.view(), out.view()
+            elif st.kind == 'upsample':
+                src, sv, ov = st.src, st.src.view(), st.out.view()
                 call("b2y_upsample_nearest_i8", ptr(sv), ops._pitch(sv), ptr(ov), ops._pitch(ov), B, src.H, src.W,
-                     src.C, int(s), stream_ptr())
-            elif kind == 'maxpool':
-                _, i, src, out, k, s, tiny = st
-                sv, ov = src.view(), out.view()
-                call("b2y_maxpool_i8", ptr(sv), ops._pitch(sv), ptr(ov), ops._pitch(ov), B, src.H, src.W, src.C, int(k),
-                     int(s), 1 if tiny else 0, stream_ptr())
+                     src.C, int(st.stride), stream_ptr())
+            elif st.kind == 'maxpool':
+                src, sv, ov = st.src, st.src.view(), st.out.view()
+                call("b2y_maxpool_i8", ptr(sv), ops._pitch(sv), ptr(ov), ops._pitch(ov), B, src.H, src.W, src.C,
+                     int(st.k), int(st.s), 1 if st.tiny_pad else 0, stream_ptr())
         no = self.yolo[0][0].no
         io = torch.empty((B, self.total_rows, no), dtype=torch.float32, device=self.device)
         p_out = []
